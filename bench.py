@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the gradient-inversion hot path (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W [--config C]             # product arm: the sm_100a engine
+    python bench.py --gpus N --steps K --warmup W [--config C] [--dump-outputs DIR]   # product arm: the sm_90a engine
     python bench.py --impl reference --steps K --warmup W [--config C]     # reference arm: CPU restatement of the reference loop
 
 A "step" is one iteration of ``OptimizationBasedAttacker._run_trial`` (closure + optimiser step + projection + best-so-far)
@@ -16,7 +16,10 @@ on one candidate batch.  ``--config`` picks the BASELINE.json configuration (def
 With N GPUs every rank runs an independent restart (trial) of the same workload, no data-path collective (weak scaling);
 value = N*K / max-over-ranks device time.  The ``e2e`` leg goes through ``prepare_attack(...).reconstruct(...)`` with
 ``restarts.num_trials = N`` (trial k on rank k, NCCL MIN select + broadcast of the winner) from pinned host buffers.
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  ``--dump-outputs DIR`` also writes, after the timed steps, what rank 0's timed trial computed
+(the arrays a caller of the engine would read back: current and best candidate, the objective history, for config 5 the label
+logits) as ``DIR/<name>.npy`` in float32.  Inputs are seeded, so two builds run with the same arguments can be compared
+output for output.
 """
 import argparse
 import copy
@@ -48,14 +51,20 @@ WORKLOADS = {
 }
 
 
+# NVIDIA's data sheet for the H100 SXM (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16.  Data-sheet figures, not measured rates:
+# a card set to a lower power limit sustains less.
+H100_DATASHEET = dict(hbm_gbs=3350.0, bf16_tflops=989.0)
+
+
 def measured_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as fh:
             d = json.load(fh)
-        return dict(hbm_gbs=d.get("hbm_gbs", 6650.0), bf16_tflops=d.get("bf16_tflops", 1590.0),
-                    bf16_tflops_sustained=d.get("bf16_tflops_sustained", 1400.0), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+        return dict(hbm_gbs=d.get("hbm_gbs", H100_DATASHEET["hbm_gbs"]), bf16_tflops=d.get("bf16_tflops", H100_DATASHEET["bf16_tflops"]),
+                    bf16_tflops_sustained=d.get("bf16_tflops_sustained", H100_DATASHEET["bf16_tflops"]), source="measured")
+    return dict(hbm_gbs=H100_DATASHEET["hbm_gbs"], bf16_tflops=H100_DATASHEET["bf16_tflops"], bf16_tflops_sustained=H100_DATASHEET["bf16_tflops"],
+                source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -181,8 +190,8 @@ def gemm_family_roofline(dev, prog, backend, local_steps=0):
     """Live device time of the dominant kernel family -- the conv/linear implicit GEMMs -- for exactly the launches one
     iteration issues (per layer: fprop, wgrad, dgrad, dual-source tangent fprop, dual-source tangent dgrad; FedAvg: per local
     step, plus the dual-source tangent wgrad), replayed from one CUDA graph through the C ABI (`bre_conv_gemm`, the engine's
-    own dispatch rule) and timed with CUDA events on the launching stream.  Operands of one replay exceed the 126 MB L2 for the
-    224x224 configurations, so a replay does not run L2-hot."""
+    own dispatch rule) and timed with CUDA events on the launching stream.  Operands of one replay exceed the 50 MB L2 of the
+    H100 for the 224x224 configurations, so a replay does not run L2-hot."""
     import torch
 
     from breaching_b200 import engine as E
@@ -244,14 +253,14 @@ def gemm_family_roofline(dev, prog, backend, local_steps=0):
 
 def matching_reduction_roofline(dev, n_params):
     """Isolated device time of the matching-reduction kernel (the HBM-bound kernel the north star names): the bare kernel is
-    captured 16x into a CUDA graph over rotating (G, g) buffer pairs whose total exceeds the 126 MB L2, so every launch streams
+    captured 16x into a CUDA graph over rotating (G, g) buffer pairs whose total exceeds the 50 MB L2, so every launch streams
     from HBM; the replay is timed with CUDA events on the launching stream."""
     import torch
 
     from breaching_b200 import engine as E
 
     peaks = measured_peaks()
-    npairs = max(4, int(2 * 126e6 / (8 * n_params)) + 1)
+    npairs = max(4, int(2 * 50e6 / (8 * n_params)) + 1)
     pairs = [(torch.randn(n_params, device=dev), torch.randn(n_params, device=dev)) for _ in range(npairs)]
     E.match_reduce(*pairs[0])
     reps = max(16, npairs)
@@ -275,9 +284,8 @@ def matching_reduction_roofline(dev, n_params):
     ms = e0.elapsed_time(e1) / (reps * replays)
     out = dict(bound="hbm", achieved=8.0 * n_params / (ms * 1e-3) / 1e9, peak=peaks["hbm_gbs"], unit="GB/s", kernel="match_reduce_kernel",
                ms=ms, peak_source=peaks["source"], algorithmic_bytes=8 * n_params,
-               traffic=(91086080 + 2710784) if n_params == 11_380_173 else None,
                note=f"mean of {replays} graph replays of {reps} launches over {npairs} rotating buffer pairs (cold in L2); includes "
-                    "inter-kernel gaps; traffic = dram read+write bytes of one ncu --set full capture (profiles/r2_match_reduce_summary.txt)")
+                    "inter-kernel gaps")
     out["frac"] = out["achieved"] / out["peak"]
     return out
 
@@ -433,6 +441,26 @@ class EngineRunner:
     def timed(self, n):
         return self.eng.run_timed(n)
 
+    def outputs(self):
+        """What the timed trial computed, as a caller reads it back: float32 host arrays by name."""
+        self.eng.sync()
+        out = dict(candidate=self.eng.candidate(), best=self.eng.best(), objective_history=self.eng.history())
+        if self.config == 5:
+            out["label_logits"] = self.eng.joint_labels(best=False)
+            out["best_label_logits"] = self.eng.joint_labels(best=True)
+        return {k: v.detach().float().cpu().numpy() for k, v in out.items()}
+
+
+def dump_outputs(directory, arrays, limit_bytes=64 << 20):
+    import numpy as np
+
+    total = sum(a.nbytes for a in arrays.values())
+    if total > limit_bytes:
+        raise SystemExit(f"bench.py: outputs of {total} bytes exceed the {limit_bytes}-byte dump limit")
+    os.makedirs(directory, exist_ok=True)
+    for name, arr in arrays.items():
+        np.save(os.path.join(directory, f"{name}.npy"), np.ascontiguousarray(arr, dtype=np.float32))
+
 
 def host_payload(case, config):
     """The attack inputs as a caller holds them: pinned host tensors (server payload + shared update)."""
@@ -490,6 +518,8 @@ def product_arm(args):
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms_max = float(t.item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, runner.outputs())
     st = runner.eng.status()
     launches = runner.eng.launches_per_iteration()
     prog, n_params, local_steps = runner.prog, runner.n_params, runner.local_steps
@@ -533,16 +563,14 @@ def product_arm(args):
     flops_iter = algorithmic_flops(prog, local_steps)
     fam = gemm_family_roofline(dev, prog, args.backend, local_steps)
     peak = peaks["bf16_tflops_sustained"]
-    roof = dict(bound="tensor", achieved=fam["tflops"], peak=peak, unit="TFLOP/s", frac=fam["tflops"] / peak,
-                traffic=2059008 if config == 2 else None, peak_source=peaks["source"],
-                kernel="igemm_tc_kernel (tcgen05 kind::tf32) + SIMT kernels for the shapes it does not cover",
+    roof = dict(bound="tensor", achieved=fam["tflops"], peak=peak, unit="TFLOP/s", frac=fam["tflops"] / peak, peak_source=peaks["source"],
+                kernel="igemm_tc_kernel (wgmma / mma.sync .tf32) + SIMT kernels for the shapes it does not cover",
                 launches_per_step=fam["n_launches"], avg_launch_us=1e3 * fam["ms_per_launch"], algorithmic_gflop_per_step=fam["flops"] / 1e9,
                 peak_tf32_equivalent=peak / 2, frac_of_tf32_peak=fam["tflops"] / (peak / 2), share_of_step=fam["ms_total"] / (ms_max / args.steps),
                 whole_step_tflops=flops_iter * (args.steps / (ms_max * 1e-3)) / 1e12,
                 note="achieved = algorithmic conv+linear FLOPs of one iteration (SURVEY 8d) / live CUDA-event time of exactly those GEMM "
-                     "launches (one graph replay through the C ABI); peak = the measured sustained bf16 cuBLAS rate (the only measured "
-                     "tensor peak; the work is TF32, whose dense peak is half of it -> frac_of_tf32_peak); traffic = dram bytes of one "
-                     "captured launch (the batch-1 layer2 tangent GEMM, profiles/r2_tc_fprop_dual_b1_summary.txt: = its algorithmic operand bytes)")
+                     "launches (one graph replay through the C ABI); peak = the dense bf16 tensor rate (peak_source; the work is TF32, "
+                     "whose dense peak is half of it -> frac_of_tf32_peak)")
     match = matching_reduction_roofline(dev, n_params)
     threads, sweep = cpu_thread_sweep(config, case)
     cpu_its, cpu_dt = oracle_iters_per_sec(config, case, "cpu", 1, args.cpu_steps if args.cpu_steps > 0 else w["ref_steps"])
@@ -551,7 +579,7 @@ def product_arm(args):
         try:
             eager_its, _ = oracle_iters_per_sec(config, case, dev, 50, args.eager_steps)
             eager = {"value": eager_its, "unit": "it/s", "steps": args.eager_steps, "warmup": 50,
-                     "what": "the reference loop (oracle/restate.py = same torch ops as the reference) in eager PyTorch on the same B200, "
+                     "what": "the reference loop (oracle/restate.py = same torch ops as the reference) in eager PyTorch on the same GPU, "
                              "cudnn.benchmark on, TF32 convolutions (torch default); denominator of the north-star >=10x target"}
         except Exception as exc:  # noqa: BLE001
             eager = {"value": None, "error": str(exc)}
@@ -563,7 +591,7 @@ def product_arm(args):
                    "parallelism": f"restarts x{world} (no data-path collective; NCCL MIN select + broadcast once per reconstruct)",
                    "gemm_backend": args.backend, "arithmetic": "fp32 storage; TF32 tensor-core products with fp32 accumulation (= cuDNN's default "
                    "for the reference on a GPU)" if args.backend == "tc" else "fp32",
-                   "l2": "per-iteration working set (4+ parameter-sized arenas + activations) exceeds the 126 MB L2 for the 224x224 "
+                   "l2": "per-iteration working set (4+ parameter-sized arenas + activations) exceeds the 50 MB L2 for the 224x224 "
                          "configurations; no explicit flush"},
         "e2e": {"value": e2e_iters / e2e_dt, "unit": "it/s", "h2d_bytes_per_step": world * h2d / e2e_iters, "d2h_bytes_per_step": world * d2h / e2e_iters,
                 "steps": e2e_steps, "trials": world, "iterations_executed": e2e_iters, "seconds": e2e_dt, "select_seconds": select_s,
@@ -645,6 +673,8 @@ def main():
     ap.add_argument("--cpu-steps", type=int, default=0)
     ap.add_argument("--eager-steps", type=int, default=200)
     ap.add_argument("--skip-eager", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the timed trial computed as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         args.steps = WORKLOADS[args.config]["ref_steps"] if args.steps is None else args.steps

@@ -14,7 +14,7 @@ _OTHER_ATTACKS = (
 def prepare_attack(model, loss, cfg_attack, setup=dict(dtype=torch.float, device=torch.device("cpu"))):
     """Same signature and error behaviour as the reference's ``prepare_attack``.
 
-    ``attack_type == "optimization"`` is served by the sm_100a engine.  Other attack types are outside the
+    ``attack_type == "optimization"`` is served by the sm_90a engine.  Other attack types are outside the
     accelerated hot path; when the original ``breaching`` package is importable they are delegated to it,
     otherwise a ``NotImplementedError`` names what is missing (never a silent fallback).
     """

@@ -42,11 +42,11 @@ def build_plan(cfg_attack, batch, channels, setup):
         opts = dict(aug[key]) if aug[key] is not None else {}
         if key == "discrete_shift":                        # Jitter(lim=32)
             if plan.continuous_shift is not None:
-                raise NotImplementedError("discrete_shift after continuous_shift is not implemented by the B200 engine")
+                raise NotImplementedError("discrete_shift after continuous_shift is not implemented by the engine")
             plan.steps.append((SHIFT, float(opts.get("lim", 32))))
         elif key == "flip":                                # Flip(p=0.5)
             if plan.continuous_shift is not None:
-                raise NotImplementedError("flip after continuous_shift is not implemented by the B200 engine")
+                raise NotImplementedError("flip after continuous_shift is not implemented by the engine")
             plan.steps.append((FLIP, float(opts.get("p", 0.5))))
         elif key == "colorjitter":                         # ColorJitter(mean=0.0, std=1.0): (img - mean) / std, drawn once (:77-83)
             if channels != 3:
@@ -59,15 +59,15 @@ def build_plan(cfg_attack, batch, channels, setup):
             any_colour = True
         elif key == "continuous_shift":                    # RandomTransform(shift=8, padding="reflection", ...)
             if plan.continuous_shift is not None:
-                raise NotImplementedError("two continuous_shift steps are not implemented by the B200 engine")
+                raise NotImplementedError("two continuous_shift steps are not implemented by the engine")
             if opts.get("fliplr", False) or opts.get("flipud", False) or opts.get("mode", "bilinear") != "bilinear":
                 raise NotImplementedError("continuous_shift: only bilinear sampling without grid flips is implemented")
             padding = opts.get("padding", "reflection")
             if padding not in ("circular", "zeros"):
-                raise NotImplementedError(f"continuous_shift padding {padding} is not implemented by the B200 engine (circular / zeros)")
+                raise NotImplementedError(f"continuous_shift padding {padding} is not implemented by the engine (circular / zeros)")
             plan.continuous_shift, plan.circular = float(opts.get("shift", 8)), padding == "circular"
         elif key in _UNSUPPORTED:
-            raise NotImplementedError(f"augmentation {key} is not implemented by the B200 engine")
+            raise NotImplementedError(f"augmentation {key} is not implemented by the engine")
         else:
             raise KeyError(key)
     if len(plan.steps) > 4:

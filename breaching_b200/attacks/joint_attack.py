@@ -1,4 +1,4 @@
-"""``OptimizationJointAttacker`` on the sm_100a engine: data and labels are optimised together ("deep leakage from
+"""``OptimizationJointAttacker`` on the sm_90a engine: data and labels are optimised together ("deep leakage from
 gradients"-style attacks; reference ``attacks/optimization_with_label_attack.py:38-230``, presets ``deepleakage.yaml``).
 
 The label candidate is a second leaf ``[N, classes]``; the closure hands ``labels.softmax(-1)`` to the task loss as class
@@ -29,7 +29,7 @@ from .optimization_attack import OptimizationBasedAttacker
 log = logging.getLogger(__name__)
 
 class OptimizationJointAttacker(OptimizationBasedAttacker):
-    """Optimises jointly for candidate data and labels on the B200 engine."""
+    """Optimises jointly for candidate data and labels on the engine."""
 
     _LOSSES = ("CrossEntropyLoss", "CausalLoss")   # CausalLoss: token models (tag.yaml), see _prepare_text
 
@@ -37,12 +37,12 @@ class OptimizationJointAttacker(OptimizationBasedAttacker):
     def _label_template(self, shared_data, metadata):
         n = shared_data[0]["metadata"]["num_data_points"]
         if metadata["task"] != "classification":
-            raise NotImplementedError("joint optimisation of token labels (text models) is not implemented by the B200 engine")
+            raise NotImplementedError("joint optimisation of token labels (text models) is not implemented by the engine")
         return host.initialize_data(self.cfg.init, [n, metadata.classes], self.dm, self.ds, self.setup)
 
     # ---- text models (tag.yaml, BASELINE config 5) ----------------------------------------------------------------
     # The closure of this path on the engine (compiler.compile_transformer program, all four sweeps, soft token labels) is
-    # verified on the B200 against the reference's TAG closure at miniature and full size, the attacker-level glue below
+    # verified on the GPU against the reference's TAG closure at miniature and full size, the attacker-level glue below
     # (prologue, loop, scoring, token recovery) against the reference trajectory (tests/test_tokens_gpu.py); its host pieces
     # are additionally tested on the CPU against the reference (tests/test_install_dropin.py, tests/test_host_loops_cpu.py).
     def _prepare_text(self, server_payload, shared_data):

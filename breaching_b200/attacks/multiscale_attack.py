@@ -1,4 +1,4 @@
-"""``MultiScaleOptimizationAttacker`` on the sm_100a engine (SURVEY section 8 f-4).
+"""``MultiScaleOptimizationAttacker`` on the sm_90a engine (SURVEY section 8 f-4).
 
 Reference: ``attacks/multiscale_optimization_attack.py:18-122`` -- the candidate is optimised on a pyramid of resolutions; every
 stage starts from the bilinearly up-sampled result of the previous one (optionally pasted into the centre of a fresh
@@ -51,7 +51,7 @@ class MultiScaleOptimizationAttacker(OptimizationBasedAttacker):
         if scale not in self._stage_engines:
             rec_models, shared_data, labels = self._stage_context
             if len(rec_models) != 1:
-                raise NotImplementedError("multi-scale attacks with several model queries are not implemented by the B200 engine")
+                raise NotImplementedError("multi-scale attacks with several model queries are not implemented by the engine")
             self._stage_engines[scale] = self._get_engine(rec_models, shared_data, labels, data_shape=(C, scale, scale), primary=False)
         return self._stage_engines[scale]
 

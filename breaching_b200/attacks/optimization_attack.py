@@ -1,4 +1,4 @@
-"""``OptimizationBasedAttacker`` served by the sm_100a engine.
+"""``OptimizationBasedAttacker`` served by the sm_90a engine.
 
 API-compatible with the reference class of the same name (``attacks/optimization_based_attack.py:24-218``):
 ``prepare_attack(model, loss_fn, cfg_attack, setup)`` builds it, ``reconstruct(server_payload, shared_data,
@@ -52,7 +52,7 @@ class _EngineSum:
 
 
 class OptimizationBasedAttacker:
-    """Implements the optimisation-based attacks of the reference on the B200 engine."""
+    """Implements the optimisation-based attacks of the reference on the engine."""
 
     _LOSSES = ("CrossEntropyLoss",)
 
@@ -77,13 +77,13 @@ class OptimizationBasedAttacker:
         self.last_timing = {}  # seconds per phase of the last reconstruct() call
         self.last_select_seconds = 0.0
         if self.setup["dtype"] != torch.float32:
-            raise NotImplementedError("the B200 engine computes in fp32 (cfg.impl.dtype=float)")
+            raise NotImplementedError("the engine computes in fp32 (cfg.impl.dtype=float)")
         if cfg_get(self.cfg.impl, "mixed_precision", False):
-            raise NotImplementedError("impl.mixed_precision is not implemented by the B200 engine")
+            raise NotImplementedError("impl.mixed_precision is not implemented by the engine")
         if self.setup["device"].type != "cuda":
-            raise EngineError("the B200 engine needs setup['device'] to be a CUDA device (there is no CPU fallback)")
+            raise EngineError("the engine needs setup['device'] to be a CUDA device (there is no CPU fallback)")
         if _loss_name(self.loss_fn) not in self._LOSSES:
-            raise NotImplementedError(f"loss {_loss_name(self.loss_fn)} is not implemented by the B200 engine ({', '.join(self._LOSSES)} only)")
+            raise NotImplementedError(f"loss {_loss_name(self.loss_fn)} is not implemented by the engine ({', '.join(self._LOSSES)} only)")
         self._engine = None
         self._engine_key = None
 
@@ -91,7 +91,7 @@ class OptimizationBasedAttacker:
         n = "\n"
         regs = (n + " " * 18).join(f"{k}: {v}" for k, v in self.regularizers)
         opt = (n + " " * 8).join(f"{key}: {val}" for key, val in self.cfg.optim.items())
-        return f"""Attacker (of type {self.__class__.__name__}, B200 engine) with settings:
+        return f"""Attacker (of type {self.__class__.__name__}, H100 engine) with settings:
     Hyperparameter Template: {self.cfg.type}
 
     Objective: {self.cfg.objective.type} with scale={cfg_get(self.cfg.objective, 'scale', 1.0)} and task reg={cfg_get(self.cfg.objective, 'task_regularization', 0.0)}
@@ -112,7 +112,7 @@ class OptimizationBasedAttacker:
         self.data_shape = metadata.shape
         self.dm, self.ds = host.preprocessing_constants(metadata, self.setup)
         if getattr(metadata, "modality", "vision") == "text":
-            raise NotImplementedError("text modality is not implemented by the B200 engine")
+            raise NotImplementedError("text modality is not implemented by the engine")
         rec_models = host.construct_models(self.model_template, server_payload, shared_data, self.setup)
         shared_data = host.cast_shared_data(shared_data, self.setup["dtype"])
         self._rec_models = rec_models
@@ -139,7 +139,7 @@ class OptimizationBasedAttacker:
         seed = int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if cfg_get(self.cfg.optim, "langevin_noise", 0.0) else 0
         if self._engine is not None and index == 0 and primary:
             self._engine.close()
-        # setup["backend"]: "tc" (tcgen05 TF32, default = torch's cuDNN-TF32 numerics) or "simt" (fp32, = allow_tf32 False)
+        # setup["backend"]: "tc" (TF32 tensor cores, default = torch's cuDNN-TF32 numerics) or "simt" (fp32, = allow_tf32 False)
         eng = Engine(model, shape, cfg, self.setup["device"], noise_seed=seed, backend=self.backend)
         eng.load_model()
         tw = None
@@ -169,9 +169,9 @@ class OptimizationBasedAttacker:
         """One engine per (model, update) pair of a multi-query attack (optimization_based_attack.py:157-160: the objective
         is summed over ``zip(rec_model, shared_data)``, the regularisers are added once)."""
         if any(d["metadata"]["local_hyperparams"] is not None for d in shared_data):
-            raise NotImplementedError("multi-step local updates with several model queries are not implemented by the B200 engine")
+            raise NotImplementedError("multi-step local updates with several model queries are not implemented by the engine")
         if any(k in ("deep_inversion", "features") for k, _ in self.regularizers):
-            raise NotImplementedError("DeepInversion / feature priors with several model queries are not implemented by the B200 engine")
+            raise NotImplementedError("DeepInversion / feature priors with several model queries are not implemented by the engine")
         no_priors = copy.deepcopy(self.cfg)
         reg = cfg_get(no_priors, "regularization")
         if reg is not None:

@@ -1,4 +1,4 @@
-"""Lower an ``nn.Module`` to the static layer program the sm_100a engine executes.
+"""Lower an ``nn.Module`` to the static layer program the sm_90a engine executes.
 
 The reference runs the attacked model through the PyTorch autograd engine twice per iteration
 (``attacks/auxiliaries/objectives.py:40-46`` forward + ``autograd.grad(create_graph=True)``,

@@ -1,7 +1,6 @@
 // Row-wise kernels over very wide rows (the 50 257-token vocabulary of BASELINE config 5): one *thread-block cluster* per row.
 //
-// With one CTA per row, 32 rows occupy 32 of 148 SMs and every reduction pass walks 200 KB per tensor serially (round 1:
-// 130-240 us per kernel, 30 % of a config-5 iteration).  Here the CS CTAs of a cluster (grid (rows, 1, CS), cluster along z) each
+// With one CTA per row, 32 rows occupy 32 of 132 SMs and every reduction pass walks 200 KB per tensor serially.  Here the CS CTAs of a cluster (grid (rows, 1, CS), cluster along z) each
 // take a contiguous segment of the row; the row reductions (max, sum, dot) are combined through distributed shared memory: every
 // CTA publishes its partial in its own shared memory, one cluster barrier, then every CTA reads the CS partials with
 // ld.shared::cluster in rank order -- the same total in every CTA, deterministic, no global scratch, no atomics.
@@ -83,8 +82,7 @@ __device__ __forceinline__ void cluster_exit() { cluster_barrier(); }
 
 // ---- register-resident row segments ------------------------------------------------------------------------------------------------
 // A CTA's segment of a 50 257-wide row is ~6 300 elements = 25 per thread.  The row kernels make two or three passes over it; with the
-// plain loops every pass is a chain of dependent L2 round trips (ncu: 15 long-scoreboard stalls per issue, 27 us for a 25 MB
-// cross-entropy).  When the segment fits, each thread loads its elements once, all loads in flight together, and the passes run out of
+// plain loops every pass is a chain of dependent L2 round trips.  When the segment fits, each thread loads its elements once, all loads in flight together, and the passes run out of
 // registers.  `seg_fits` depends only on the row width and the cluster size, so it is uniform over the cluster (the barriers inside the
 // reductions need every CTA on the same path).
 constexpr int kSegCache = 26;

@@ -1,4 +1,4 @@
-// Shared helpers for the breaching_b200 sm_100a kernels.
+// Shared helpers for the breaching_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -30,11 +30,11 @@ void set_error(const std::string& msg);
     }                                                                                               \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // ---- programmatic dependent launch (PDL) -------------------------------------------------------------------
 // Every kernel of the iteration is launched with cudaLaunchAttributeProgrammaticStreamSerialization: it may be
-// scheduled while its predecessor is still draining, runs its private prologue (barrier init, TMEM allocation, index
+// scheduled while its predecessor is still draining, runs its private prologue (barrier init, index
 // pre-computation) and then blocks in griddepcontrol.wait until the predecessor grid has completed and flushed its
 // memory.  This hides the ~2-3 us launch latency between the ~200 dependent kernels of one iteration; stream capture
 // records the edges as programmatic dependencies of the CUDA graph.  Without the launch attribute both instructions
@@ -86,7 +86,7 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
 
 static inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
-// Round-to-nearest onto the TF32 grid (10-bit mantissa, low 13 bits cleared).  tcgen05 kind::tf32 reads fp32 operands and
+// Round-to-nearest onto the TF32 grid (10-bit mantissa, low 13 bits cleared).  the tensor cores read fp32 operands and
 // simply ignores the low mantissa bits (truncation, biased towards zero); tensors that feed the tensor-core GEMMs are
 // therefore rounded by the kernel that produces them, so that the products are those of cuDNN's TF32 path (cvt.rna).
 __device__ __forceinline__ float tf32_rna(float v) {

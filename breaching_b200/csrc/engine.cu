@@ -94,7 +94,7 @@ struct bre_engine {
 
   long long P_pad = 0, max_param = 0, max_tensor = 0;
   float *W = nullptr, *g = nullptr, *G = nullptr, *V = nullptr, *stage = nullptr, *chunk_w = nullptr;
-  // TF32-rounded shadows of the parameter and direction arenas: what the tcgen05 GEMMs read (the masters stay fp32: a local
+  // TF32-rounded shadows of the parameter and direction arenas: what the tensor-core GEMMs read (the masters stay fp32: a local
   // SGD step or an adjoint update is far below one TF32 ulp of the weights).  See tf32_rna in common.cuh.
   float *Wt = nullptr, *Vt = nullptr;
   std::vector<float*> ms_Wt;
@@ -144,9 +144,9 @@ struct bre_engine {
   std::vector<cudaEvent_t> ev_fork;
   cudaEvent_t ev_join = nullptr;
   bool overlap_wgrad = true;
-  // BN + residual + ReLU (and its tangent) in the epilogue of the producing tcgen05 fprop.  Off by default: measured on the
-  // B200 it removes 32 of 201 launches per config-2 iteration and is still 1.5 % slower (the split-K epilogue's extra global
-  // loads cost more than the PDL-overlapped element-wise kernels they replace).  BRE_FUSE_BNACT=1 / option "fuse_bnact".
+  // BN + residual + ReLU (and its tangent) in the epilogue of the producing tensor-core fprop.  Off by default: it removes 32 of
+  // 201 launches per config-2 iteration, but the split-K epilogue's extra global loads can cost more than the PDL-overlapped
+  // element-wise kernels they replace.  BRE_FUSE_BNACT=1 / option "fuse_bnact".
   bool fuse_bnact = [] { const char* e = getenv("BRE_FUSE_BNACT"); return e ? atoi(e) != 0 : false; }();
   float* ws2 = nullptr;
   int* gemm_counters2 = nullptr;
@@ -273,7 +273,7 @@ struct bre_engine {
   }
   // execution
   bool use_graph = true;
-  int gemm_backend = 0;  // 0 = SIMT fp32, 1 = tcgen05 TF32 where supported
+  int gemm_backend = 0;  // 0 = SIMT fp32, 1 = TF32 tensor cores where supported
   cudaGraphExec_t exec = nullptr;
   bool graph_ready = false;
   int launch_count = 0, launches_per_iter = 0;
@@ -290,7 +290,7 @@ struct bre_engine {
   float* Wp(int idx) const { return W + params[idx].off; }
   float* Gp(int idx) const { return G + params[idx].off; }
   float* Vp(int idx) const { return V + params[idx].off; }
-  // conv / linear weights as GEMM operands: the TF32-rounded shadow for the layers the tcgen05 back end covers, the fp32
+  // conv / linear weights as GEMM operands: the TF32-rounded shadow for the layers the tensor-core back end covers, the fp32
   // master for the layers that run on the SIMT kernels (so that a network with no eligible layer is bit-identical on both
   // back ends)
   size_t op_index(const bre_op_desc& op) const { return (size_t)(&op - ops.data()); }
@@ -324,7 +324,7 @@ struct bre_engine {
     return 0;
   }
   // Which activation tensors are operands of a tensor-core GEMM: inputs (value / tangent) and output deltas of the
-  // convolutions the tcgen05 back end covers.  Only those are stored TF32-rounded; layers that run on the fp32 SIMT kernels
+  // convolutions the tensor-core back end covers.  Only those are stored TF32-rounded; layers that run on the fp32 SIMT kernels
   // (3-channel stem, narrow test networks, the classifier head) keep full fp32 operands.
   std::vector<char> rnd_val, rnd_d;
   void compute_round_flags() {
@@ -395,7 +395,7 @@ struct bre_engine {
     return launch_igemm_simt(a, st);
   }
 
-  // The BN/residual/ReLU op that directly follows conv `i` and reads its output can run in the GEMM epilogue (tcgen05 back end).
+  // The BN/residual/ReLU op that directly follows conv `i` and reads its output can run in the GEMM epilogue (tensor-core back end).
   bool fuses_with_next(size_t i, const GemmArgs& a) const {
     if (!fuse_bnact || gemm_backend != 1 || i + 1 >= ops.size()) return false;
     const bre_op_desc& nx = ops[i + 1];
@@ -559,8 +559,8 @@ struct bre_engine {
           a.g_gamma = op.has_bn ? Gp(op.gamma) : nullptr; a.g_beta = op.has_bn ? Gp(op.beta) : nullptr;
           a.partials = red_partials; a.counters = red_counters; a.defer = 0;
           if (op.has_bn && !op.bn_train && !bn_partials.empty() && bn_partials[i] != nullptr) { a.partials = bn_partials[i]; a.defer = 1; deferred_bn = true; }
-          // (splitting this op into an element-wise kernel on the main stream and the gamma / beta reductions on the side
-          // stream was measured: config 2 unchanged, configs 1 and 3 3-5 % slower -- the side stream is already full)
+          // (not split into an element-wise kernel on the main stream and the gamma / beta reductions on the side stream:
+          // the side stream already carries the weight gradients)
           if (op.has_bn && op.bn_train) {
             // pass 1: sum(du), sum(du xh) (= the gamma / beta gradients) and the residual delta; pass 2: dx needs those sums
             BnActBwdArgs r = a;
@@ -1028,7 +1028,7 @@ int bre_engine::refresh_bn_constants(int k) {
 extern "C" {
 
 const char* bre_last_error(void) { return bre::g_last_error.c_str(); }
-const char* bre_version(void) { return "breaching_b200 0.1.0 (sm_100a)"; }
+const char* bre_version(void) { return "breaching_b200 0.1.0 (sm_90a)"; }
 
 int bre_engine_create(const bre_tensor_desc* tensors, int32_t n_tensors, const bre_op_desc* ops, int32_t n_ops,
                       const bre_param_desc* params, int32_t n_params, int32_t logits_tensor, const bre_attack_cfg* cfg,
@@ -1248,7 +1248,7 @@ int bre_engine_load_model(bre_engine* e, const float* const* params, int32_t n_p
     BRE_TRY(launch_bn_prepare(e->Wp(op.gamma), e->Wp(op.beta), b.rm, b.rv, op.eps, b.C, b.scale, b.shift, b.inv, b.nrm, e->stream));
   }
   BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
-  BRE_TRY(launch_round_tf32(e->W, e->Wt, e->P_pad, e->stream));   // GEMM-operand shadow (used by the tcgen05 back end)
+  BRE_TRY(launch_round_tf32(e->W, e->Wt, e->P_pad, e->stream));   // GEMM-operand shadow (used by the tensor-core back end)
   if (e->stem_op >= 0) {   // zero-padded [Co][Kp] copy of the stem weight (TF32-rounded like Wt when the tensor-core back end rounds)
     const bre_op_desc& op = e->ops[e->stem_op];
     BRE_TRY(launch_stem_pad_rows(e->Wp(op.w), e->Wcol, e->td(op.tout).C, op.R * op.S * e->td(op.tin).C, e->stem_Kp, false, e->tc_round_env, e->stream));
@@ -1799,7 +1799,7 @@ int bre_engine_set_option(bre_engine* e, const char* name, int64_t value) {
     e->logits_valid = (int)value; e->graph_ready = false; return BRE_OK;
   }
   if (n == "gemm_backend") {
-    if (value != 0 && value != 1) { set_error("gemm_backend must be 0 (simt) or 1 (tcgen05)"); return BRE_ERR_INVALID; }
+    if (value != 0 && value != 1) { set_error("gemm_backend must be 0 (simt) or 1 (tensor cores)"); return BRE_ERR_INVALID; }
     e->gemm_backend = (int)value; e->graph_ready = false; e->chunk_mode_ready = false; return BRE_OK;
   }
   set_error("unknown option " + n);
@@ -1867,7 +1867,7 @@ int bre_conv_gemm(int32_t mode, int32_t backend, const float* a, const float* w,
   g.ws = ws; g.counters = counters; g.ws_tiles = 1024;
   if (linear_tall_supported(g)) return launch_linear_tall(g, s) == 0 ? BRE_OK : BRE_ERR_CUDA;   // the engine's dispatch rule (gemm_on)
   if (backend == 1) {
-    if (!igemm_tc_supported(g)) { set_error("tcgen05 back end does not cover this shape"); return BRE_ERR_UNSUPPORTED; }
+    if (!igemm_tc_supported(g)) { set_error("tensor-core back end does not cover this shape"); return BRE_ERR_UNSUPPORTED; }
     return launch_igemm_tc(g, s);
   }
   if (backend == 2 && linear_small_preferred(g)) return launch_linear_small(g, s) == 0 ? BRE_OK : BRE_ERR_CUDA;

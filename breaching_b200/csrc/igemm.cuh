@@ -16,7 +16,7 @@ struct ConvGeom {
   int R, S, stride, pad;
 };
 
-// Optional consumer fused into the FPROP epilogue of the tcgen05 back end: the BN + residual + ReLU op that follows a
+// Optional consumer fused into the FPROP epilogue of the tensor-core back end: the BN + residual + ReLU op that follows a
 // convolution (layers.cu bnact_fwd_kernel, kind 1) or its tangent (bnact_tan_fwd_kernel, kind 2).  The GEMM result is still
 // written to `out` when `out` is non-null (the backward sweeps need the pre-BN value; nobody reads the pre-BN tangent).
 struct GemmEpilogue {
@@ -54,7 +54,7 @@ struct GemmArgs {
   int ws_tiles;
   int splits;             // 0 = choose automatically
   int force_fp32;         // engine: run this contraction on the fp32 kernels even on the tensor-core back end (precision knob)
-  // bit s: wgt[s] (fprop / dgrad) was fully written before the *predecessor* kernel of this launch started, so the tcgen05 back end
+  // bit s: wgt[s] (fprop / dgrad) was fully written before the *predecessor* kernel of this launch started, so the tensor-core back end
   // may start loading it before griddepcontrol.wait (model weights; the direction v once a serialised launch follows make_v)
   unsigned wgt_static;
 };
@@ -70,7 +70,7 @@ bool linear_small_preferred(const GemmArgs& a);   // engine dispatch: small-row 
 // fp32 registers + a fixed-order fold (linear_small.cu); uses a.ws for the per-chunk partial sums
 bool linear_tall_supported(const GemmArgs& a);
 int launch_linear_tall(const GemmArgs& a, cudaStream_t stream);
-// tcgen05 TF32 back end (igemm_tc.cu); returns BRE_ERR_UNSUPPORTED (-4) for shapes it does not cover.
+// TF32 tensor-core back end (igemm_tc.cu); returns BRE_ERR_UNSUPPORTED (-4) for shapes it does not cover.
 int launch_igemm_tc(const GemmArgs& a, cudaStream_t stream);
 bool igemm_tc_supported(const GemmArgs& a);
 

@@ -1,5 +1,5 @@
 // fp32 SIMT implicit-GEMM back end (CUDA cores).  Bit-faithful fp32 arithmetic: this is the parity
-// back end and the fallback for shapes the tcgen05 TF32 back end (igemm_tc.cu) does not cover
+// back end and the fallback for shapes the TF32 tensor-core back end (igemm_tc.cu) does not cover
 // (tiny channel counts such as the 3-channel stem, ragged K).
 //
 // Tile 64x64x16, 256 threads, 4x4 outputs per thread, register-prefetch double buffering, deterministic

@@ -1,16 +1,20 @@
-// tcgen05 TF32 implicit-GEMM back end (sm_100a): the dense contractions of the four sweeps on the 5th-generation
-// tensor cores.  D[128 x BN] accumulates in TMEM (fp32), one elected thread issues tcgen05.mma.kind::tf32 with
-// both operands read from shared memory through UMMA descriptors (128-byte-swizzled K-major or MN-major layouts, as the
-// global layout of the operand dictates, so no transposed copies of activations / weights are ever materialised),
-// completion is tracked with tcgen05.commit -> mbarrier, the epilogue reads the accumulator back with tcgen05.ld
-// (32 lanes x 32 columns per warp).  Operand staging, TC_STAGES-deep ring, two producers:
+// Hopper TF32 implicit-GEMM back end (sm_90a): the dense contractions of the four sweeps on the tensor cores.  A CTA
+// computes a 128 x BN tile with one consumer warpgroup (warps 0-3) holding the fp32 accumulator in registers, fed from a
+// TC_STAGES-deep shared-memory ring by a producer warpgroup (warps 4-7) over mbarriers:
+//   * FPROP (both operands K-major in memory): wgmma.mma_async m64nBNk8 .tf32 straight from the 128-byte-swizzled ring
+//     stages through shared-memory matrix descriptors (two wgmma per 8-wide k step: rows 0-63 and 64-127);
+//   * DGRAD / WGRAD: one operand (the weight of dgrad) or both (wgrad) are contiguous along M / N in memory, and wgmma
+//     reads tf32 operands K-major only.  Rather than materialise transposed copies, the consumer warps load mma.sync
+//     m16n8k8 .tf32 fragments from the swizzled stages with ld.shared (any layout is addressable that way).
+// Both consumers leave the accumulator in the same register layout (warp w: rows 16w + [0, 16) and 64 + 16w + [0, 16)),
+// so the epilogue is shared.  Operand staging, two producers:
 //   * TMA (default wherever the geometry allows): one thread issues cp.async.bulk.tensor loads -- im2col-mode tensor
 //     maps for the gathered activation operand (the hardware walks 128 output pixels x 32 channels of one filter tap,
-//     zero-filling the padding halo), tiled maps for the weight operand -- which land directly in the swizzled UMMA
+//     zero-filling the padding halo), tiled maps for the weight operand -- which land directly in the 128-byte-swizzled
 //     layouts and complete on the stage's mbarrier (expect_tx);
-//   * cp.async (strided dgrad, whose "every stride-th tap" gather no tensor map expresses, and BRE_TC_TMA=0): four loader
-//     warps issue 16-byte LDGSTS with precomputed per-row tap masks, completion via cp.async.mbarrier.arrive.
-// Split-K runs inside a thread-block cluster (<= 16 CTAs along z) with a deterministic DSMEM reduction.
+//   * cp.async (strided dgrad, whose "every stride-th tap" gather no tensor map expresses, and BRE_TC_TMA=0): the four
+//     producer warps issue 16-byte LDGSTS with precomputed per-row tap masks, completion via cp.async.mbarrier.arrive.
+// Split-K runs inside a thread-block cluster (<= 8 CTAs along z) with a deterministic DSMEM reduction.
 //
 // fp32 storage everywhere; TF32 (10-bit mantissa) multiplies with fp32 accumulation -- the numeric mode cuDNN uses
 // for the reference's GPU path by default (SURVEY.md section 8c, torch.backends.cudnn.allow_tf32).
@@ -30,12 +34,12 @@ namespace bre {
 
 namespace {
 
-constexpr int TC_BM = 128;      // UMMA M
-constexpr int TC_BK = 32;       // k-block per pipeline stage (4 MMAs of K = 8)
+constexpr int TC_BM = 128;      // tile rows: two wgmma M = 64 halves
+constexpr int TC_BK = 32;       // k-block per pipeline stage (4 MMA steps of K = 8)
 constexpr int TC_STAGES = 4;       // default ring depth
 constexpr int TC_MAX_STAGES = 8;   // deep ring (chosen per launch, TcDims::stage_shift): stage / phase of k-block i are i & (n - 1), (i >> log2 n) & 1
-constexpr int TC_THREADS = 128;       // loader / epilogue threads (warps 0-3 <-> TMEM lane quadrants)
-constexpr int TC_BLOCK = TC_THREADS + 32;  // + one MMA-issuer warp
+constexpr int TC_THREADS = 128;       // consumer warpgroup (MMA + epilogue) = producer warpgroup size
+constexpr int TC_BLOCK = 2 * TC_THREADS;
 
 struct TcDims {
   int M, Nc, K;
@@ -65,74 +69,82 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
+// ---- wgmma (FPROP) ---------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor of a K-major, 128-byte-swizzled operand: start address and stride byte offset (8-row
+// groups, 1024 B) in 16-byte units, leading byte offset unused for swizzled K-major layouts, layout type 1 = SWIZZLE_128B
+// in bits 62-63.  The k step of 8 tf32 (32 bytes) inside the 128-byte swizzle atom is a plain start-address offset: the
+// swizzle is a function of the absolute address (ring stages are 1024-byte aligned).
+__device__ __forceinline__ uint64_t wgmma_desc_k128(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols));
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from touching accumulator registers across an outstanding wgmma (it does not see the async write)
+template <int NR>
+__device__ __forceinline__ void fence_regs(float (&d)[NR]) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x BN] += A[64 x 8] . B[BN x 8]^T, both from shared memory (K-major), fp32 accumulate
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t da, uint64_t db);
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(1));
 }
 
-// UMMA shared-memory descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor): start address, leading / stride byte
-// offsets in 16-byte units, version = 1 (Blackwell), layout type 0 = no swizzle ("interleave").
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type) {
-  uint64_t d = (uint64_t)(layout_type & 7u) << 61;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
+// ---- mma.sync (DGRAD / WGRAD) ------------------------------------------------------------------------------------
+// m16n8k8 .tf32: a = A(g, t), A(g + 8, t), A(g, t + 4), A(g + 8, t + 4); b = B(n = g, t), B(g, t + 4);
+// d = D(g, 2t), D(g, 2t + 1), D(g + 8, 2t), D(g + 8, 2t + 1)   (g = lane / 4, t = lane % 4)
+__device__ __forceinline__ void mma_tf32(float* d, const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// Shared-memory layouts of a [ROWS x 32] fp32 operand tile (ROWS = extent along M or N), as the tensor core reads them.
-// Both were verified on the B200 with profiles/experiments/umma_layout_probe.cu (one-hot probing of every byte offset):
-//   K-major, SWIZZLE_128B (layout type 2): one 128-byte smem row per operand row = the whole 32-wide k-block, its eight
-//   16-byte granules XOR-swizzled with (row % 8), 8-row groups at SBO = 1024:
+// Shared-memory layouts of a [ROWS x 32] fp32 operand tile (ROWS = extent along M or N).  Both are what TMA writes with
+// CU_TENSOR_MAP_SWIZZLE_128B into a 1024-byte-aligned box (16-byte granule c of 128-byte smem row r lands at c ^ (r % 8)):
+//   K-major (the operand is contiguous along k): one 128-byte smem row per operand row = the whole 32-wide k-block:
 //       byte(row, k) = (row/8) * 1024 + (row%8) * 128 + (((k/4) ^ (row%8)) * 16) + (k%4) * 4
-//       MMA covering k in [8j, 8j+8): start + 32 j (the swizzle is a function of the absolute address), LBO = 16
-//   (the no-swizzle K-major layout also works -- first version of this kernel -- but forces either uncoalesced global
-//   reads or 8-way conflicting shared stores; 128B swizzle gives coalesced 128-byte reads AND conflict-free stores)
-//   MN-major for 32-bit operands only exists as SWIZZLE_128B_BASE32B (layout type 1; the plain / 16-byte-atom MN-major
-//   layouts produce zeros for kind::tf32): 32 elements (128 B) contiguous along MN, rows of 128 B along k, the four
-//   32-byte chunks of a row XOR-swizzled with (k % 4), k-groups of 4 at SBO, MN-groups of 32 at LBO:
-//       byte(row, k) = (row/32) * 4096 + (k/4) * 512 + (k%4) * 128 + ((((row%32)/8) ^ (k%4)) * 32) + (row%8) * 4
-//       MMA covering k in [8j, 8j+8): start + j*1024, LBO = 4096, SBO = 512
-// K-major SWIZZLE_128B: granule = 16 bytes (4 k), `g` = granule column 0..7 of the 32-wide k-block
+//   MN-major (contiguous along M / N; boxes of 32 rows x 32 k, 4 KB each): one 128-byte smem row per k:
+//       byte(row, k) = (row/32) * 4096 + k * 128 + ((((row%32)/4) ^ (k%8)) * 16) + (row%4) * 4
+// 128-byte swizzle gives coalesced 128-byte global reads and conflict-free 16-byte shared stores for the cp.async producer;
+// the mma.sync fragment loads are conflict-free on the K-major layout and 2-way on the MN-major one.
+// K-major: granule = 16 bytes (4 k), `g` = granule column 0..7 of the 32-wide k-block
 __device__ __forceinline__ uint32_t off_k128(int row, int g) {
   return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((g ^ (row & 7)) << 4));
 }
-template <int ROWS>
-__device__ __forceinline__ uint32_t off_mnmajor(int row, int k) {
-  return (uint32_t)((row >> 5) * 4096 + (k >> 2) * 512 + (k & 3) * 128 + ((((row >> 3) & 3) ^ (k & 3)) << 5) + (row & 7) * 4);
+__device__ __forceinline__ uint32_t off_mn128(int row, int k) {
+  return (uint32_t)((row >> 5) * 4096 + k * 128 + ((((row >> 2) & 7) ^ (k & 7)) << 4) + (row & 3) * 4);
+}
+template <bool MN>
+__device__ __forceinline__ uint32_t ld_op(const uint8_t* base, int row, int k) {
+  return *reinterpret_cast<const uint32_t*>(base + (MN ? off_mn128(row, k) : off_k128(row, k >> 2) + (k & 3) * 4));
 }
 
 // 16-byte asynchronous global -> shared copy; src_bytes = 0 zero-fills the destination (padding, out-of-range taps)
@@ -146,7 +158,7 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 __device__ __forceinline__ void cp_async_arrive(uint64_t* bar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void loader_sync() { asm volatile("bar.sync 1, %0;" ::"n"(TC_THREADS) : "memory"); }
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(TC_THREADS) : "memory"); }
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -157,7 +169,7 @@ __device__ __forceinline__ float4 ld_dsmem4(uint32_t saddr, uint32_t rank) {
   asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(saddr), "r"(rank));
   float4 v;
   // volatile (not reordered across the cluster barriers, themselves volatile) but no memory clobber: a batch of these is issued
-  // back to back instead of one round trip at a time (1.5 us -> of the split-K tail, profiles/experiments/tc_trace.py)
+  // back to back instead of one round trip at a time
   asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(raddr));
   return v;
 }
@@ -174,7 +186,7 @@ struct TcMaps {
 //     din[y, x] = sum_{tr, ts} dout[iy + cy - tr, ix + cx - ts] . w[ey + stride tr, ex + stride ts]
 // i.e. an im2col load over dout with traversal stride 1, lower corner L = c - (T - 1) and filter offset (T - 1) - t.  One launch
 // covers all classes (blockIdx.x enumerates (class, m-tile) pairs); a class no tap reaches writes zeros.  Replaces the cp.async
-// producer with its 4x zero-filled taps (round 1: 10 % of a config-2 and 13 % of a config-3 iteration).
+// producer with its 4x zero-filled taps.
 constexpr int TC_MAXCLS = 4;   // stride 2
 struct ClsPlan {
   int ncls, stride;
@@ -231,7 +243,7 @@ __device__ __forceinline__ void fused_bnact(const GemmEpilogue& e, long long row
   }
 }
 
-// Phase timestamps of CTA (0,0,0) (SM clock), compiled in with -DBRE_TC_TRACE for profiles/experiments/tc_trace.py only.
+// Phase timestamps of CTA (0,0,0) (SM clock), compiled in with -DBRE_TC_TRACE (read back with bre_debug_tc_trace).
 #ifdef BRE_TC_TRACE
 __device__ long long g_tc_trace[16];
 #define TC_MARK(i, cond) do { if ((cond) && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) g_tc_trace[i] = clock64(); } while (0)
@@ -248,15 +260,15 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
   uint8_t* sA = smem;                                  // [STAGES][A_BYTES]
   const int nst = 1 << d.stage_shift, stage_mask = nst - 1;
   uint8_t* sB = smem + nst * A_BYTES;                  // [stages][B_BYTES]
-  __shared__ __align__(8) uint64_t bar_full[TC_MAX_STAGES];   // loaders -> MMA issuer (cp.async completion, 128 arrivals)
-  __shared__ __align__(8) uint64_t bar_empty[TC_MAX_STAGES];  // MMA issuer -> loaders (tcgen05.commit)
-  __shared__ __align__(8) uint64_t bar_done;
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t bar_full[TC_MAX_STAGES];   // producers -> consumers (TMA transaction bytes / 128 cp.async arrivals)
+  __shared__ __align__(8) uint64_t bar_empty[TC_MAX_STAGES];  // consumers -> producers (one arrival per consumer warp)
 
   TC_MARK(0, threadIdx.x == 0);
   pdl_launch_dependents();   // the successor may start its own prologue; it blocks in its griddepcontrol.wait
   const ConvGeom g = a.g;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int ptid = tid & (TC_THREADS - 1);   // index inside the producer warpgroup (warps 4-7)
+  const bool consumer = warp < TC_THREADS / 32;
   const int n0 = blockIdx.y * BN, z = blockIdx.z;
   int m0 = blockIdx.x * TC_BM;
   int kb_begin = z * d.kblocks_per_split;
@@ -279,22 +291,15 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
 
   if (tid == 0) {
 #pragma unroll
-    for (int s = 0; s < TC_MAX_STAGES; ++s) { mbar_init(&bar_full[s], TMA ? 1 : TC_THREADS); mbar_init(&bar_empty[s], 1); }
-    mbar_init(&bar_done, 1);
+    for (int s = 0; s < TC_MAX_STAGES; ++s) { mbar_init(&bar_full[s], TMA ? 1 : TC_THREADS); mbar_init(&bar_empty[s], TC_THREADS / 32); }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(&s_tmem, BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = s_tmem;
   TC_MARK(1, threadIdx.x == 0);
 
-  // instruction descriptor (UMMA::InstrDescriptor): D = F32, A = B = TF32, majors, N >> 3, M >> 4
-  constexpr uint32_t a_mn = (MODE == GEMM_WGRAD) ? 1u : 0u;
-  constexpr uint32_t b_mn = (MODE == GEMM_FPROP) ? 0u : 1u;
-  constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (a_mn << 15) | (b_mn << 16) | ((uint32_t)(BN >> 3) << 17) |
-                             ((uint32_t)(TC_BM >> 4) << 24);
+  // operand majors in shared memory: A is MN-major for WGRAD (dout, contiguous along ko), B for DGRAD and WGRAD
+  constexpr bool a_mn = MODE == GEMM_WGRAD;
+  constexpr bool b_mn = MODE != GEMM_FPROP;
 
   // ---- per-thread fixed decode of the gathered (activation) operand ----------------------------------------
   // Loader thread t handles 16-byte granule column (t % 8) of A rows (t / 8) + 16 j, j = 0..7: the eight lanes of a
@@ -304,11 +309,11 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
   // k-block costs one shift/and + one add + one cp.async per row (the loader warps are issue-latency bound otherwise).
   constexpr int A_VEC = TC_BM * TC_BK / 4 / TC_THREADS;  // 16-byte granules per thread per stage: 8
   constexpr int B_VEC = BN * TC_BK / 4 / TC_THREADS;     // 4 (BN = 64)
-  const int gcol = tid & 7, grow = (tid >> 3) & 15;
+  const int gcol = ptid & 7, grow = (ptid >> 3) & 15;
   int a_off[A_VEC];                  // element offset of the anchor pixel (+ granule column)
   unsigned long long a_taps[A_VEC];  // bit rs: tap (r, s) of this row reads inside the tensor
   int a_yx[A_VEC];                   // slow path (strided dgrad): packed (y << 16) | x and image index in a_off
-  if (!TMA && (MODE == GEMM_FPROP || MODE == GEMM_DGRAD)) {
+  if (!TMA && !consumer && (MODE == GEMM_FPROP || MODE == GEMM_DGRAD)) {
 #pragma unroll
     for (int j = 0; j < A_VEC; ++j) {
       const int m = m0 + grow + 16 * j;
@@ -467,19 +472,20 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.wgt[sidx])) : "memory");
     }
   }
-  // `nprod` producer lanes (lane 0 of loader warps 0..nprod-1, default 2), k-blocks dealt round-robin: a cp.async.bulk.tensor
-  // costs its issuing thread ~140 cycles (profiles/experiments/tc_trace.py); two issuers keep up with the six loads per
-  // k-block of the wgrad form, more make no difference
+  // `nprod` producer lanes (lane 0 of producer warps 4..4+nprod-1, default 2), k-blocks dealt round-robin: a
+  // cp.async.bulk.tensor costs its issuing thread on the order of 100 cycles, so the six loads per k-block of the wgrad form
+  // want two issuers
   const int nprod = (proxy_fence >> 2) & 7;
-  const bool producer = TMA && (tid & 31) == 0 && warp < nprod && warp < nkb;
+  const int pw = warp - TC_THREADS / 32;   // producer warp index
+  const bool producer = TMA && !consumer && lane == 0 && pw < nprod && pw < nkb;
   KbState pst;
   memset(&pst, 0, sizeof(pst));
   uint32_t pre_wgt = 0;   // ring stages whose weight loads are already in flight when the wait below returns
   if (producer) {
-    pst = kb_init(kb_begin + warp);
+    pst = kb_init(kb_begin + pw);
     if (MODE != GEMM_WGRAD && a.wgt_static != 0) {
       KbState st = pst;
-      for (int i = warp; i < nkb && i < nst; i += nprod) {
+      for (int i = pw; i < nkb && i < nst; i += nprod) {
         if ((a.wgt_static >> st.src) & 1) {
           mbar_expect_tx(&bar_full[i], A_BYTES + B_BYTES);
           issue_wgt_tma(i, st);
@@ -490,13 +496,13 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
     }
   }
 
-  // Everything above touched only kernel parameters, shared memory, TMEM and weights the caller declared constant across the
+  // Everything above touched only kernel parameters, shared memory and weights the caller declared constant across the
   // predecessor (GemmArgs::wgt_static); from here on global memory written by the predecessor kernel is read.
   pdl_wait();
   TC_MARK(2, threadIdx.x == 0);
 
   // Stage one k-block: cp.async (LDGSTS, 16 B, zero-fill for padding / out-of-range taps) straight from global memory
-  // into the UMMA operand layouts -- no register staging, so up to TC_STAGES k-blocks of loads stay in flight.
+  // into the swizzled operand layouts -- no register staging, so up to TC_STAGES k-blocks of loads stay in flight.
   auto issue_block = [&](int stage) {
     const int src = it_src;
     const int kch = (MODE == GEMM_DGRAD) ? g.Co : g.Ci;
@@ -539,17 +545,17 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
         }
       }
       // B(n = ci, k) = W[ko][r][s][ci]: contiguous along n -> MN-major.  lanes along n (16 granules = 64 ci), 8 k per pass
-      const int n4 = tid & 15, kk = tid >> 4;
+      const int n4 = ptid & 15, kk = ptid >> 4;
 #pragma unroll
       for (int j = 0; j < B_VEC; ++j) {
         const int k = kk + 8 * j;
         const float* gb = wgt + ((long long)(k0 + k) * (g.R * g.S) + rs) * g.Ci + n0 + n4 * 4;
-        cp_async16(pb + off_mnmajor<BN>(4 * n4, k), gb, 16u);
+        cp_async16(pb + off_mn128(4 * n4, k), gb, 16u);
       }
     } else {
       // WGRAD: k = pixel.  A(m = ko, k) = dout[pixel][ko] (MN-major): lanes along m (32 granules = 128 ko), 4 k per pass
       {
-        const int m4 = tid & 31, kk = tid >> 5;
+        const int m4 = ptid & 31, kk = ptid >> 5;
 #pragma unroll
         for (int j = 0; j < A_VEC; ++j) {
           const int k = kk + 4 * j;
@@ -557,12 +563,12 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
           const bool kok = pix < d.K;
           const bool mok = kok && (m0 + m4 * 4 < d.M);
           const float* ga = mok ? wgt + (long long)pix * g.Co + m0 + m4 * 4 : wgt;
-          cp_async16(pa + off_mnmajor<TC_BM>(4 * m4, k), ga, mok ? 16u : 0u);
+          cp_async16(pa + off_mn128(4 * m4, k), ga, mok ? 16u : 0u);
         }
       }
       // B(n = (r, s, c), k) = in[img, p*stride - pad + r, q*stride - pad + s, c] (MN-major, Ci % 4 == 0)
       {
-        const int n4 = tid & 15, kk = tid >> 4;
+        const int n4 = ptid & 15, kk = ptid >> 4;
         const int n = n0 + n4 * 4;
         const int rs = n / g.Ci, c = n - rs * g.Ci;
         const int r = rs / g.S, s = rs - r * g.S;
@@ -579,7 +585,7 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
             ok = h >= 0 && h < g.H && w >= 0 && w < g.W;
             if (ok) gb = act + img * a.x_sN + (long long)(h * g.W + w) * a.x_sP + c;
           }
-          cp_async16(pb + off_mnmajor<BN>(4 * n4, k), gb, ok ? 16u : 0u);
+          cp_async16(pb + off_mn128(4 * n4, k), gb, ok ? 16u : 0u);
         }
       }
     }
@@ -593,43 +599,78 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
     }
   };
 
-  // ---- main loop, warp-specialised: warps 0-3 stream k-blocks into a TC_STAGES-deep ring with cp.async and signal
-  //      "full" through cp.async.mbarrier.arrive; one thread of warp 4 waits for "full", issues the four tcgen05.mma of
-  //      the k-block and lets tcgen05.commit signal "empty" when the tensor core has consumed the stage.  No CTA-wide
-  //      barrier inside the loop.
-  if (warp == TC_THREADS / 32) {
-    if (tid == TC_THREADS) {
-      // descriptors of stage 0 / MMA slice 0; the 14-bit address field counts 16-byte units, so stage and slice offsets are
-      // plain additions on the low word (shared memory is < 256 KB: no carry out of the field)
-      const uint64_t adesc0 = a_mn ? make_desc(smem_u32(sA), 4096, 512, 1) : make_desc(smem_u32(sA), 16, 1024, 2);
-      const uint64_t bdesc0 = b_mn ? make_desc(smem_u32(sB), 4096, 512, 1) : make_desc(smem_u32(sB), 16, 1024, 2);
-      constexpr uint32_t a_step = (a_mn ? 1024u : 32u) >> 4, b_step = (b_mn ? 1024u : 32u) >> 4;
-      for (int i = 0; i < nkb; ++i) {
-        const int stage = i & stage_mask;
-        mbar_wait(&bar_full[stage], (uint32_t)((i >> d.stage_shift) & 1));
-        TC_MARK(4, i == 0);
-        TC_MARK(11, i == nkb - 1);
-        // The mbarrier phase completes only after every cp.async of this stage has been performed, so the data is in
-        // shared memory when the wait returns; like CUTLASS' sm100 cp.async mainloop no fence.proxy.async is issued
-        // here (measured: it costs ~0.5 us per k-block on the single-thread critical path).  BRE_TC_PROXY_FENCE=1 re-enables it.
-        if (proxy_fence & 1) fence_proxy_async();
-        tc_fence_after();
-        const uint64_t adesc_s = adesc0 + (uint64_t)((uint32_t)stage * (A_BYTES >> 4));
-        const uint64_t bdesc_s = bdesc0 + (uint64_t)((uint32_t)stage * (B_BYTES >> 4));
+  // ---- main loop, warp-specialised: the producer warpgroup streams k-blocks into the TC_STAGES-deep ring (TMA: one or two
+  //      issuing lanes, completion by transaction bytes; cp.async: all 128 threads, cp.async.mbarrier.arrive), the consumer
+  //      warpgroup waits for "full", runs the MMAs of the k-block and signals "empty" (one arrival per warp) once the stage
+  //      has been read.  No CTA-wide barrier inside the loop.
+  // acc[h][4 j + q] = tile element (64 h + 16 w + g + 8 (q >> 1), 8 j + 2 t + (q & 1)), w = warp, g = lane / 4, t = lane % 4
+  // (the wgmma m64nN accumulator fragment of half h, and the union of the mma.sync m16n8 fragments of the same elements)
+  float acc[2][BN / 2];
 #pragma unroll
-        for (int j = 0; j < TC_BK / 8; ++j)
-          umma_tf32(tmem_d, adesc_s + (uint64_t)(j * a_step), bdesc_s + (uint64_t)(j * b_step), idesc, (i > 0 || j > 0) ? 1u : 0u);
-        umma_commit(&bar_empty[stage]);
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
+  const int gq = lane >> 2, tq = lane & 3;
+  if (consumer) {
+    for (int i = 0; i < nkb; ++i) {
+      const int stage = i & stage_mask;
+      mbar_wait(&bar_full[stage], (uint32_t)((i >> d.stage_shift) & 1));
+      TC_MARK(4, i == 0 && tid == 0);
+      if constexpr (MODE == GEMM_FPROP) {
+        // cp.async stores are generic-proxy writes and wgmma reads through the async proxy (TMA writes need no fence)
+        if (!TMA || (proxy_fence & 1)) fence_proxy_async();
+        const uint32_t sa = smem_u32(sA) + stage * A_BYTES, sb = smem_u32(sB) + stage * B_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < TC_BK / 8; ++j) {
+          const uint64_t db = wgmma_desc_k128(sb + 32 * j);
+          wgmma_tf32<BN>(acc[0], wgmma_desc_k128(sa + 32 * j), db);
+          wgmma_tf32<BN>(acc[1], wgmma_desc_k128(sa + 64 * 128 + 32 * j), db);
+        }
+        wgmma_commit();
+        // this k-block's MMAs stay in flight while the next stage is waited for; the previous stage is free once its group is
+        wgmma_wait<1>();
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+        __syncwarp();
+        if (i > 0 && lane == 0) mbar_arrive(&bar_empty[(i - 1) & stage_mask]);
+      } else {
+        const uint8_t* pa = sA + stage * A_BYTES;
+        const uint8_t* pb = sB + stage * B_BYTES;
+#pragma unroll
+        for (int j = 0; j < TC_BK / 8; ++j) {
+          const int k0 = 8 * j + tq;
+          uint32_t af[2][4];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = 64 * h + 16 * warp + gq;
+            af[h][0] = ld_op<a_mn>(pa, r, k0);
+            af[h][1] = ld_op<a_mn>(pa, r + 8, k0);
+            af[h][2] = ld_op<a_mn>(pa, r, k0 + 4);
+            af[h][3] = ld_op<a_mn>(pa, r + 8, k0 + 4);
+          }
+#pragma unroll
+          for (int jn = 0; jn < BN / 8; ++jn) {
+            const uint32_t b0 = ld_op<b_mn>(pb, 8 * jn + gq, k0), b1 = ld_op<b_mn>(pb, 8 * jn + gq, k0 + 4);
+            mma_tf32(&acc[0][4 * jn], af[0], b0, b1);
+            mma_tf32(&acc[1][4 * jn], af[1], b0, b1);
+          }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bar_empty[stage]);
       }
-      umma_commit(&bar_done);
-      TC_MARK(5, true);
     }
-    __syncwarp();
+    if constexpr (MODE == GEMM_FPROP) {
+      wgmma_wait<0>();
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
+    }
+    TC_MARK(5, tid == 0);
   } else {
     if (TMA) {
       if (producer) {
         KbState st = pst;
-        for (int i = warp; i < nkb; i += nprod) {
+        for (int i = pw; i < nkb; i += nprod) {
           const int stage = i & stage_mask;
           if (i >= nst) mbar_wait(&bar_empty[stage], (uint32_t)(((i >> d.stage_shift) - 1) & 1));
           if (i >= nst || !((pre_wgt >> i) & 1u)) {
@@ -649,20 +690,12 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
         issue_block(stage);
         cp_async_arrive(&bar_full[stage]);
       }
+      cp_async_wait<0>();
     }
-    mbar_wait(&bar_done, 0);
-    TC_MARK(6, tid == 0);
-    tc_fence_after();
   }
 
-  // ---- epilogue: TMEM -> registers; thread `tid` holds row m0 + tid, BN columns in chunks of 32 -----------------
+  // ---- epilogue (consumer warpgroup): accumulator registers -> global memory, or -> this CTA's split-K partial ----------
   const int splits = gridDim.z;
-  const int tile = blockIdx.y * gridDim.x + blockIdx.x;
-  const uint32_t lane_base = tmem_d + ((uint32_t)(warp * 32) << 16);
-  float v[32];
-  const int m = m0 + tid;
-  const bool row_ok = m < Mrows;
-  const bool is_loader = warp < TC_THREADS / 32;
   auto out_row = [&](int mm, long long& row, int& cs) {
     if (CLS) {   // class pixel (img, iy, ix) -> input pixel (y0 + stride * iy, x0 + stride * ix)
       const int per = cHc * cWc;
@@ -679,70 +712,66 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
       cs = 1;
     }
   };
-  if (!is_loader) {
-    // MMA-issuer warp: nothing to write back
-  } else if (splits == 1) {
-    long long row = 0;
-    int cs = 1;
-    if (row_ok) out_row(m, row, cs);
+  if (consumer && splits == 1) {
+    // (a class no filter tap reaches has nkb = 0 and writes the zero accumulator)
 #pragma unroll
-    for (int c = 0; c < BN; c += 32) {
-      if (nkb > 0) tmem_ld32(lane_base + c, v);  // warp-collective: executed by all lanes, also for rows beyond M
-      else {                                    // (a class no filter tap reaches: zeros)
+    for (int h = 0; h < 2; ++h) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0.f;
-      }
-      if (!row_ok) continue;
-      const int n = n0 + c;
-      if (MODE == GEMM_FPROP && a.bias != nullptr) {
+      for (int hr = 0; hr < 2; ++hr) {
+        const int mm = m0 + 64 * h + 16 * warp + gq + 8 * hr;
+        if (mm >= Mrows) continue;
+        long long row;
+        int cs;
+        out_row(mm, row, cs);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] += __ldg(a.bias + n + j);
-      }
-      float* op = a.out + row + (long long)n * cs;
-      if (MODE == GEMM_FPROP && a.epi.kind != 0) {
-        if (a.out != nullptr) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(op + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        }
-        fused_bnact<32>(a.epi, row, n, v);
-        float* op2 = a.epi.out2 + row + n;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(op2 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-      } else if (cs == 1) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float4 t = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-          if (a.accumulate) {
-            const float4 o = *reinterpret_cast<const float4*>(op + j);
-            t.x += o.x; t.y += o.y; t.z += o.z; t.w += o.w;
+        for (int jn = 0; jn < BN / 8; ++jn) {
+          const int n = n0 + 8 * jn + 2 * tq;
+          float v[2] = {acc[h][4 * jn + 2 * hr], acc[h][4 * jn + 2 * hr + 1]};
+          if (MODE == GEMM_FPROP && a.bias != nullptr) {
+            v[0] += __ldg(a.bias + n);
+            v[1] += __ldg(a.bias + n + 1);
           }
-          *reinterpret_cast<float4*>(op + j) = t;
-        }
-      } else {
+          float* op = a.out + row + (long long)n * cs;
+          if (MODE == GEMM_FPROP && a.epi.kind != 0) {
+            if (a.out != nullptr) *reinterpret_cast<float2*>(op) = make_float2(v[0], v[1]);
+            fused_bnact<2>(a.epi, row, n, v);
+            *reinterpret_cast<float2*>(a.epi.out2 + row + n) = make_float2(v[0], v[1]);
+          } else if (cs == 1) {
+            float2 t2 = make_float2(v[0], v[1]);
+            if (a.accumulate) {
+              const float2 o = *reinterpret_cast<const float2*>(op);
+              t2.x += o.x; t2.y += o.y;
+            }
+            *reinterpret_cast<float2*>(op) = t2;
+          } else {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          float* q = op + (long long)j * cs;
-          *q = a.accumulate ? *q + v[j] : v[j];
+            for (int j = 0; j < 2; ++j) {
+              float* q = op + (long long)j * cs;
+              *q = a.accumulate ? *q + v[j] : v[j];
+            }
+          }
         }
       }
     }
-  } else {
+  } else if (consumer) {
     // split-K inside a thread-block cluster (cluster = the `splits` CTAs of one output tile along z): every CTA parks
-    // its partial accumulator tile in its own shared memory (the operand ring is idle now), one cluster barrier, then
-    // CTA `z` sums rows [z*128/S, (z+1)*128/S) of all S partials straight out of the peers' shared memory (DSMEM,
-    // ld.shared::cluster) in fixed rank order -- deterministic, no global workspace, no atomics, no "last CTA" tail.
+    // its partial accumulator tile in its own shared memory (the operand ring is idle once all consumer warps are done
+    // reading it), one cluster barrier, then CTA `z` sums rows [z*128/S, (z+1)*128/S) of all S partials straight out of
+    // the peers' shared memory (DSMEM, ld.shared::cluster) in fixed rank order -- deterministic, no global workspace, no
+    // atomics, no "last CTA" tail.
+    consumer_sync();
     float* part = reinterpret_cast<float*>(sA);  // [128 rows][BN] fp32, 16-byte chunks XOR-swizzled by (row & 15)
 #pragma unroll
-    for (int c = 0; c < BN; c += 32) {
-      if (nkb > 0) tmem_ld32(lane_base + c, v);
-      else {
+    for (int h = 0; h < 2; ++h) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0.f;
-      }
+      for (int hr = 0; hr < 2; ++hr) {
+        const int r = 64 * h + 16 * warp + gq + 8 * hr;
 #pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const int chunk = ((c + j) >> 2) ^ (tid & (BN / 4 - 1) & 15);
-        *reinterpret_cast<float4*>(part + tid * BN + chunk * 4) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+        for (int jn = 0; jn < BN / 8; ++jn) {
+          const int c = 8 * jn + 2 * tq;
+          const int chunk = (c >> 2) ^ (r & (BN / 4 - 1) & 15);
+          *reinterpret_cast<float2*>(part + r * BN + chunk * 4 + (c & 3)) = make_float2(acc[h][4 * jn + 2 * hr], acc[h][4 * jn + 2 * hr + 1]);
+        }
       }
     }
   }
@@ -750,14 +779,13 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
     TC_MARK(7, tid == 0);
     cluster_sync_all();   // every thread of every CTA in the cluster (partials visible cluster-wide)
     TC_MARK(8, tid == 0);
-    if (is_loader) {
+    if (consumer) {
       // Every thread owns BN/(4 S) float4 slots of this CTA's row slice and needs the S peers' copies of each: BN/4 = 16
       // remote 16-byte loads per thread whatever S is.  All of them are issued before the first is consumed (a DSMEM round
       // trip is ~0.5 us; one slot at a time made this phase 2.2 us), then summed in fixed rank order.
       auto reduce_rows = [&](auto s_tag) {
         constexpr int S = decltype(s_tag)::value;
         constexpr int C4 = BN / 4, SLOTS = (TC_BM / S) * C4 / TC_THREADS > 0 ? (TC_BM / S) * C4 / TC_THREADS : 1;
-        static_assert(BN >= 64 || S <= 8, "narrow tiles: at most 8 splits");
         const uint32_t part_s = smem_u32(sA);
         float4 t[SLOTS][S];
         int rr[SLOTS], cc[SLOTS];
@@ -809,18 +837,12 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
       switch (splits) {
         case 2: reduce_rows(std::integral_constant<int, 2>{}); break;
         case 4: reduce_rows(std::integral_constant<int, 4>{}); break;
-        case 8: reduce_rows(std::integral_constant<int, 8>{}); break;
-        default:
-          if constexpr (BN >= 64) reduce_rows(std::integral_constant<int, 16>{});
-          break;
+        default: reduce_rows(std::integral_constant<int, 8>{}); break;
       }
     }
     TC_MARK(9, tid == 0);
     cluster_sync_all();   // nobody leaves (and frees its shared memory) while a peer may still be reading it
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_d, BN);
   TC_MARK(10, tid == 0);
 }
 
@@ -925,7 +947,7 @@ bool tma_eligible(const GemmArgs& a) {
 
 bool build_maps(const GemmArgs& a, int BN, TcMaps* maps) {
   const ConvGeom& g = a.g;
-  const CUtensorMapSwizzle K128 = CU_TENSOR_MAP_SWIZZLE_128B, MN32 = CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B;
+  const CUtensorMapSwizzle K128 = CU_TENSOR_MAP_SWIZZLE_128B;
   for (int s = 0; s < a.nsrc; ++s) {
     if (a.mode == GEMM_FPROP) {
       if (!im2col_map(&maps->act[s], a.act[s], g.N, g.H, g.W, g.Ci, a.x_sN, a.x_sP, -g.pad, -g.pad, g.pad - (g.S - 1), g.pad - (g.R - 1),
@@ -943,15 +965,15 @@ bool build_maps(const GemmArgs& a, int BN, TcMaps* maps) {
         return false;
       const long long dims[3] = {g.Ci, (long long)g.R * g.S, g.Co}, strides[2] = {g.Ci, (long long)g.R * g.S * g.Ci};
       const int box[3] = {32, 1, TC_BK};
-      if (!tiled_map(&maps->wgt[s], a.wgt[s], 3, dims, strides, box, MN32)) return false;
+      if (!tiled_map(&maps->wgt[s], a.wgt[s], 3, dims, strides, box, K128)) return false;
     } else {
       // A(m = ko, k = pixel) = dout[pixel][ko]; B(n = (r, s, c), k = pixel) = im2col of the activation, 32 pixels x 32 channels
       const long long npix = (long long)g.N * g.Ho * g.Wo;
       const long long dims[2] = {g.Co, npix}, strides[1] = {g.Co};
       const int box[2] = {32, TC_BK};
-      if (!tiled_map(&maps->wgt[s], a.wgt[s], 2, dims, strides, box, MN32)) return false;
+      if (!tiled_map(&maps->wgt[s], a.wgt[s], 2, dims, strides, box, K128)) return false;
       if (!im2col_map(&maps->act[s], a.act[s], g.N, g.H, g.W, g.Ci, a.x_sN, a.x_sP, -g.pad, -g.pad, g.pad - (g.S - 1), g.pad - (g.R - 1),
-                      g.stride, 32, TC_BK, MN32))
+                      g.stride, 32, TC_BK, K128))
         return false;
     }
   }
@@ -1020,7 +1042,7 @@ bool build_cls(const GemmArgs& a, ClsPlan* plan, TcMapsCls* maps) {
   for (int s = 0; s < a.nsrc; ++s) {
     const long long dims[3] = {g.Ci, (long long)g.R * g.S, g.Co}, strides[2] = {g.Ci, (long long)g.R * g.S * g.Ci};
     const int box[3] = {32, 1, TC_BK};
-    if (!tiled_map(&maps->wgt[s], a.wgt[s], 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return false;
+    if (!tiled_map(&maps->wgt[s], a.wgt[s], 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return false;
   }
   return n > 0;
 }
@@ -1044,8 +1066,8 @@ int launch_tc(const GemmArgs& a, const TcDims& d0, const std::conditional_t<CLS,
   // split-K factor = cluster size along z: a power of two <= 8 (portable cluster limit) that brings the grid to ~100 CTAs
   static const int max_splits_env = [] { const char* e = getenv("BRE_TC_MAX_SPLITS"); return e ? atoi(e) : 0; }();
   static const int target_ctas_env = [] { const char* e = getenv("BRE_TC_TARGET_CTAS"); return e ? atoi(e) : 0; }();
-  const int target = target_ctas_env > 0 ? target_ctas_env : 144;   // re-tuned with the TMA producer: 96 -> 144 is +2 % on config 2, 288 is -4 %
-  constexpr int kMaxCluster = BN >= 64 ? 16 : 8;  // non-portable cluster size 16 (8 is the portable limit; narrow tiles: see reduce_rows)
+  const int target = target_ctas_env > 0 ? target_ctas_env : kNumSMs;   // about one wave of CTAs
+  constexpr int kMaxCluster = 8;  // portable cluster size
   int splits = a.splits;
   if (splits <= 0) {
     splits = 1;
@@ -1058,17 +1080,14 @@ int launch_tc(const GemmArgs& a, const TcDims& d0, const std::conditional_t<CLS,
   while (splits > 1 && splits > d.total_kblocks) splits /= 2;
   d.kblocks_per_split = ceil_div(d.total_kblocks, splits);
   if (tn > 65535) { set_error("igemm_tc: grid too large"); return -1; }
-  // (an 8-deep ring for single-wave launches was tried: 192 KB of shared memory per CTA stops the next kernel's CTAs from
-  // becoming resident during this one's tail -- programmatic dependent launch loses its overlap -- and layer4 got 2x slower)
-  // Ring depth: 4 stages (96 KB: two CTAs per SM, and the next kernel's CTAs become resident during this one's tail -- what
-  // programmatic dependent launch needs).  Measured on the B200 (profiles/README.md): an 8-deep ring (192 KB, one CTA per SM) is
-  // 25-30 % slower on config 2 *and* on the multi-wave batch-8 launches of config 3 -- occupancy beats ring depth.
-  // BRE_TC_STAGES=2|4|8 forces a depth for experiments.
+  // Ring depth: 4 stages (96 KB: two CTAs per SM within the 227 KB an SM offers, and the next kernel's CTAs can become
+  // resident during this one's tail -- what programmatic dependent launch needs).  BRE_TC_STAGES=2|4|8 forces a depth for
+  // experiments (8 stages = 192 KB, one CTA per SM).
   static const int stages_env = [] { const char* e = getenv("BRE_TC_STAGES"); return e ? atoi(e) : 0; }();
   // Short reductions on many tiles (the token models' decoder fprop: 786 tiles x 3-6 k-blocks): a 2-deep ring halves the shared
-  // memory so four CTAs share an SM and the per-CTA prologue / epilogue overlap: config 5 1187 -> 1220 it/s (BRE_TC_SHORTK_STAGES=4 turns it off)
+  // memory so more CTAs share an SM and the per-CTA prologue / epilogue overlap (BRE_TC_SHORTK_STAGES=4 turns it off)
   static const int shortk_env = [] { const char* e = getenv("BRE_TC_SHORTK_STAGES"); return e ? atoi(e) : 2; }();
-  const bool shortk = shortk_env == 2 && d.kblocks_per_split <= 6 && tm == 1 && tiles * splits > 2LL * kNumSMs;   // (with full 128-row tiles -- config 3's 1x1 convolutions -- it costs 1 %)
+  const bool shortk = shortk_env == 2 && d.kblocks_per_split <= 6 && tm == 1 && tiles * splits > 2LL * kNumSMs;
   const int stages = (stages_env == 8 || stages_env == 2) ? stages_env : (shortk ? 2 : TC_STAGES);
   d.stage_shift = stages == 8 ? 3 : (stages == 2 ? 1 : 2);
   const size_t smem = (size_t)stages * (TC_BM + BN) * TC_BK * 4;
@@ -1076,7 +1095,6 @@ int launch_tc(const GemmArgs& a, const TcDims& d0, const std::conditional_t<CLS,
   static bool attr_done = false;
   if (!attr_done) {
     BRE_CUDA_CHECK(cudaFuncSetAttribute(igemm_tc_kernel<MODE, BN, TMA, CLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-    BRE_CUDA_CHECK(cudaFuncSetAttribute(igemm_tc_kernel<MODE, BN, TMA, CLS>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     attr_done = true;
   }
   static const int proxy_fence_env = [] {
@@ -1133,7 +1151,7 @@ int launch_igemm_tc(const GemmArgs& a, cudaStream_t stream) {
   d.total_kblocks = d.kblocks_per_src * a.nsrc;
   d.kblocks_per_split = d.total_kblocks;
   // TMA producer where the geometry allows it and the driver encodes the maps; otherwise the cp.async producer of the same
-  // kernel (still tcgen05, still on the GPU: a different loader, not a fallback to another implementation)
+  // kernel (same consumer, still on the GPU: a different loader, not a fallback to another implementation)
   TcMaps maps;
   memset(&maps, 0, sizeof(maps));
   if (cls_eligible(a)) {   // strided dgrad: per-parity-class gathers through im2col tensor maps

@@ -277,8 +277,7 @@ __global__ void channel_stats_kernel(const float* __restrict__ x, long long P, i
 
 // ======================================================================================================================
 // 128-bit variants of the BN / residual / ReLU sweeps (C % 4 == 0, which every conv net here satisfies).  The scalar kernels
-// above moved 4 bytes per thread and instruction and reached 20-40 % of the HBM rate on the batch-8 tensors of config 3
-// (profiles/launches_r2*: 33 % of that iteration); these move 16 bytes per thread with several independent loads in flight.
+// above move 4 bytes per thread and instruction, far from the HBM rate on the batch-8 tensors of config 3; these move 16 bytes per thread with several independent loads in flight.
 // Same expressions, element by element.
 // ======================================================================================================================
 __device__ __forceinline__ float4 ld4(const float* p, long long i4) { return __ldg(reinterpret_cast<const float4*>(p) + i4); }
@@ -437,7 +436,7 @@ inline void slab_grid4(long long P, int C, dim3& grid, int& LX, int& LY, long lo
   while (256 % LX != 0) --LX;          // C4 = 16, 32, 64 ... in practice; keep LX a divisor of 256 for odd widths
   LY = 256 / LX;
   const int cg = ceil_div(C4, LX);
-  // `waves` x 148 blocks: 2 when the last block of a column group sums the slabs itself (a longer tail per slab), 4 when the slabs are
+  // `waves` x kNumSMs blocks: 2 when the last block of a column group sums the slabs itself (a longer tail per slab), 4 when the slabs are
   // summed by a later batched kernel (deferred BN gradients, batched statistics)
   // (a batched launch over many tensors passes this tensor's share of the whole grid as `target_blocks` instead)
   const long long want = target_blocks > 0 ? target_blocks : (long long)waves * kNumSMs;
@@ -558,7 +557,7 @@ __global__ void __launch_bounds__(256) channel_stats_vec_kernel(const float* __r
 }
 
 // ---- per-channel statistics of many tensors in one launch (DeepInversion: every BN input of the forward pass) --------------------
-// 53 separate slab reductions (ResNet-50) cost ~8 us of fixed two-phase overhead each; batched: one launch writes the slab partials
+// 53 separate slab reductions (ResNet-50) each pay a fixed two-phase overhead; batched: one launch writes the slab partials
 // of all layers (blockIdx.x -> (layer, channel group, slab) through a prefix table), one launch turns them into mean / variance.
 __global__ void __launch_bounds__(256) channel_stats_batched_kernel(const StatSlot* __restrict__ table, int n_layers) {
   pdl_prologue();
@@ -638,12 +637,12 @@ __global__ void __launch_bounds__(256) channel_stats_batched_finalize_kernel(con
 
 // ---- deferred, batched finalisation of the BN parameter gradients ---------------------------------------------------------------
 // Every bnact_bwd launch used to end with a serial tail: atomic ticket, the last block of each channel group re-reads the slab
-// partials and sums them (5-8 us of a 9-20 us launch, on the critical path of the backward sweep 20-53 times per iteration).  With
+// partials and sums them (on the critical path of the backward sweep 20-53 times per iteration).  With
 // `defer` the kernels stop after writing their partials; one launch at the end of the sweep sums the slabs of *all* layers (one
 // block per 32 channels of a layer, fixed summation order) -- the gradients of gamma / beta are only read by the matching reduction.
 __global__ void __launch_bounds__(1024) bn_grad_finalize_kernel(const BnGradSlot* __restrict__ table, int n_layers) {
   // block = 32 channels x 2 quantities (64 adjacent floats of a slab row: coalesced) x 16 interleaved slices of the slab list; the
-  // slices are folded in a fixed order.  (One thread per (channel, quantity) walking all slabs was 25 us at ~600 slabs.)
+  // slices are folded in a fixed order.
   __shared__ float part[16][64];
   pdl_prologue();
   int layer = 0;
@@ -838,7 +837,7 @@ __global__ void maxpool_bwd_kernel(const float* __restrict__ dout, const int* __
 
 // 128-bit forms of the three pooling kernels (C % 4 == 0, 16-byte aligned tensors, < 2^31 elements): a thread owns four adjacent
 // channels of one pixel, so the index arithmetic is paid once per 16 bytes and every access is a full-width load / store.  The
-// scalar kernels above spend most of their time in 64-bit divisions (batch 8: 78 us for a 40 MB sweep).
+// scalar kernels above spend most of their time in 64-bit divisions.
 __device__ __forceinline__ void take_max(float v, int at, float& best, int& bi) {
   if (v > best || v != v || bi < 0) { best = v; bi = at; }
 }

@@ -20,7 +20,7 @@ int launch_bn_prepare(const float* gamma, const float* beta, const float* rm, co
                       float* scale, float* shift, float* inv, float* nrm, cudaStream_t s);
 
 // out = relu?( bn?(in) + res? )
-// round_out: store `out` rounded onto the TF32 grid (it is an operand of tcgen05 GEMMs, see tf32_rna in common.cuh)
+// round_out: store `out` rounded onto the TF32 grid (it is an operand of tensor-core GEMMs, see tf32_rna in common.cuh)
 int launch_bnact_fwd(const float* in, const float* res, float* out, long long P, int C, bool has_bn, bool relu,
                      BnConsts bn, bool round_out, cudaStream_t s);
 

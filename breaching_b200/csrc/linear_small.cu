@@ -1,8 +1,7 @@
 // Small-batch linear layers (the classification head at batch 1-16, token-model projections at <= 32 rows): fprop / dgrad / wgrad of  out[n][co] = sum_k in[n][k] W[co][k]
 // with the optional K-concatenated second source of the tangent sweeps.  At these sizes the contraction is a handful of
 // matrix-vector products over a [Co][Ci] weight matrix (ResNet-18 head: 397 x 512 = 0.8 MB): HBM/L2-latency bound, no reuse to
-// tile for -- the 64x64-tile implicit GEMM spent 16 us per launch on a single row of tiles (profiles/launches_r1_summary.txt:
-// 7 % of a config-2 iteration in the five head launches).  fp32 throughout (bit-class parity with the fp32 SIMT back end: the
+// tile for -- the 64x64-tile implicit GEMM would run a single row of tiles.  fp32 throughout (bit-class parity with the fp32 SIMT back end: the
 // same products, summed in a fixed order).
 #include "igemm.cuh"
 #include <type_traits>
@@ -146,8 +145,7 @@ int launch_nb(const GemmArgs& a, cudaStream_t stream) {
 
 // ---- tall-K dgrad: din[n][ci] = sum_co dy[n][co] W[co][ci] with few rows (n <= 32), a narrow input (ci <= 128) and a very long
 //      reduction (the 96 -> 50257 decoder of the token models: Co = 50304).  As an implicit GEMM this is one row of 128 x 32 output
-//      tiles whose split-K is capped by the cluster size: 24 CTAs streamed the 19 MB weight matrix in 65 us (123 us for the
-//      two-source tangent form), 19 % of a config-5 iteration.  Here the reduction is cut into ~2 chunks per SM; a block keeps all
+//      tiles whose split-K is capped by the cluster size, so few CTAs stream the 19 MB weight matrix.  Here the reduction is cut into ~2 chunks per SM; a block keeps all
 //      n x ci partial sums of its chunk in registers (warp = 8 rows x one half of the chunk's output channels, lanes along ci, so the
 //      weight rows are read as coalesced 128-byte lines exactly once per block) and a second small kernel adds the per-chunk
 //      partials in a fixed order.  Same products as the GEMM back ends (the operands are the same arrays), fp32 accumulation.
@@ -158,8 +156,8 @@ __device__ __forceinline__ void lt_cp_async16(float* smem_dst, const float* gsrc
 }
 
 // The weight rows of a chunk are one contiguous block of memory ([Co][Ci] row-major): they are brought into shared memory with 16-byte
-// cp.async granules, every load of the block in flight at once (with register loads the kernel ran as a chain of ~11 dependent HBM
-// round trips per block: 20 / 41 us per launch).  The products then run out of shared memory: per output channel a warp reads CJ
+// cp.async granules, every load of the block in flight at once (with register loads the kernel runs as a chain of dependent HBM
+// round trips per block).  The products then run out of shared memory: per output channel a warp reads CJ
 // conflict-free 128-byte rows and two broadcast 16-byte vectors for 8 CJ fused multiply-adds per lane.
 template <int CJ>   // CJ = Ci / 32
 __global__ void __launch_bounds__(256, 4) linear_tall_dgrad_kernel(GemmArgs a, int chunk, float* __restrict__ partials) {
@@ -320,9 +318,8 @@ int launch_linear_small(const GemmArgs& a, cudaStream_t stream) {
 }
 
 // Experiment switch (BRE_LINEAR_SMALL_ROWS=1): send linear layers on <= 32 rows with a short reduction (token models at batch 1:
-// 96 -> 288 / 96 / 1536 projections) to the matrix-vector kernels even where the tcgen05 kernel covers the shape.  Measured on the
-// B200: at 32 rows these kernels are much slower than the 128 x 32-tile GEMM (config 5: 716 vs 1316 it/s) -- 32 accumulators per
-// thread and 32 broadcast loads per weight element are no match for one MMA -- so the default is off.
+// 96 -> 288 / 96 / 1536 projections) to the matrix-vector kernels even where the tensor-core kernel covers the shape.  At 32 rows
+// 32 accumulators per thread and 32 broadcast loads per weight element are no match for one MMA, so the default is off.
 bool linear_small_preferred(const GemmArgs& a) {
   static const int env = [] { const char* e = getenv("BRE_LINEAR_SMALL_ROWS"); return e ? atoi(e) : 0; }();
   if (!env || a.mode == GEMM_WGRAD || !linear_small_supported(a)) return false;

@@ -561,8 +561,7 @@ __global__ void loss_mean_kernel(const float* loss_n, int N, Scalars* sc) {
   sc->task_loss = (double)(float)(s / N);
 }
 
-// DeepInversion value and adjoint coefficients: one block per BN layer (round 1: one block walked all 20-53 layers, 170 us for
-// ResNet-50), then a one-warp sum of the per-layer values in layer order.
+// DeepInversion value and adjoint coefficients: one block per BN layer (not one block walking all 20-53 layers), then a one-warp sum of the per-layer values in layer order.
 __global__ void __launch_bounds__(256) di_layer_kernel(const DiLayer* layers, double* layer_values) {
   pdl_prologue();
   __shared__ double scratch[32];
@@ -661,7 +660,7 @@ int launch_orthogonality(const float* x, float* grad, int N, long long D, bool o
   return 0;
 }
 
-// launch shape of the matching reduction (tuned on the B200 with profiles/experiments/tune_match_reduce.py)
+// launch shape of the matching reduction
 static int g_match_blocks_per_sm = 4, g_match_unroll = 4;
 
 int launch_match_reduce(const float* G, const float* g, const float* chunk_w, long long n, float mask_value,
@@ -760,7 +759,7 @@ int launch_feature_reg(const float* feat, const float* measured, float* tdelta, 
 
 }  // namespace bre
 
-// tuning hook for profiles/experiments/tune_match_reduce.py (not part of the reference-facing ABI)
+// tuning hook for the launch shape of the matching reduction (not part of the reference-facing ABI)
 extern "C" void bre_debug_match_config(int blocks_per_sm, int unroll) {
   if (blocks_per_sm >= 1 && blocks_per_sm <= 8) bre::g_match_blocks_per_sm = blocks_per_sm;
   if (unroll == 4 || unroll == 8) bre::g_match_unroll = unroll;

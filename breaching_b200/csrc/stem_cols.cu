@@ -1,10 +1,9 @@
 // The convolution fed by the candidate (ResNet stem 7x7/2 on 3 channels, first 3x3 conv of the ConvNets) on the tensor cores.
 //
-// With 3 input channels the implicit-GEMM k-blocks cannot come from a tensor map (one pixel is 12 bytes), so in round 1 this
-// layer ran on the fp32 SIMT kernels: stem fprop / wgrad 5 % and the stem dgrad onto the candidate 6.9 % of a config-2
-// iteration (profiles/launches_r1_summary.txt).  Here the candidate is unfolded once per forward into a column matrix
+// With 3 input channels the implicit-GEMM k-blocks cannot come from a tensor map (one pixel is 12 bytes), so this layer would
+// run on the fp32 SIMT kernels.  Here the candidate is unfolded once per forward into a column matrix
 //     xcol[m = (n, p, q)][k = (r, s, c)]   (K = R*S*Ci zero-padded to a multiple of 64, values on the TF32 grid)
-// and the four contractions of the layer become plain 1x1 "convolutions" over xcol that the tcgen05 kernel covers:
+// and the four contractions of the layer become plain 1x1 "convolutions" over xcol that the tensor-core kernel covers:
 //     F / TF :  fprop  xcol . Wcol^T , xcol . Vcol^T          B :  wgrad  dout^T . xcol  -> Gcol
 //     TB     :  dgrad  [td | d] . [Wcol ; Vcol] -> dcol[m][k], folded back onto the NCHW candidate gradient by col2im
 // (an explicit GEMM + col2im is the textbook form of a strided dgrad: every input pixel gathers the <= ceil(R/stride)^2 column
@@ -47,8 +46,7 @@ __global__ void __launch_bounds__(256) stem_im2col_kernel(const float* __restric
 }
 
 // Same unfold with the k -> (r, s, c) decode done once per block into shared memory (Kp <= 256: the 7x7x3 stem pads to 192, a
-// 3x3x3 first conv to 64) and 32-bit index arithmetic: the generic kernel above spends its time in the per-element divisions
-// (batch 8: 84 us for a 77 MB write).
+// 3x3x3 first conv to 64) and 32-bit index arithmetic: the generic kernel above spends its time in the per-element divisions.
 __global__ void __launch_bounds__(256) stem_im2col_lut_kernel(const float* __restrict__ x, float* __restrict__ xcol, ColGeom g, int total, int round_out) {
   __shared__ int tap_off[256];   // c * H * W + r * W + s
   __shared__ int tap_rs[256];    // r | s << 8, -1 for the zero padding of K

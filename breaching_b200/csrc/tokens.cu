@@ -103,7 +103,6 @@ __global__ void layernorm_kernel(int sweep, const float* __restrict__ x, const f
 
 // gamma / beta gradients of LayerNorm: G_gamma[c] = sum_rows dy xh, G_beta[c] = sum_rows dy.  Block = 32 columns x 8 row slices
 // (warp w takes rows w, w + 8, ...: coalesced 128-byte row segments, 8 independent chains), folded over the slices in a fixed order.
-// (One thread per column walking all rows serially was 10 us per launch at 32 rows.)
 __global__ void __launch_bounds__(256) layernorm_param_grad_kernel(const float* __restrict__ x, const float* __restrict__ dy,
                                                                    const float* __restrict__ stats, int rows, int C,
                                                                    float* __restrict__ g_gamma, float* __restrict__ g_beta) {
@@ -136,7 +135,7 @@ __global__ void __launch_bounds__(256) layernorm_param_grad_kernel(const float* 
 // matrices live in shared memory; P (and the tangent P') are also kept in global memory [B, heads, T, T] between sweeps.
 // Every sweep has two phases: (A) one warp per query row, lanes along the key index -- scores, the row reductions of the softmax
 // and of its first / second derivative via warp shuffles; (B) all threads over the (row, channel) outputs, each a T-long dot
-// product.  (Round 1 ran one *thread* per query row: 48 us per launch, 21 % of a config-5 iteration.)
+// product (not one *thread* per query row, which serialises the key loop).
 //   sweep 0 (F):  O = P V                                  writes out [rows, d], P
 //   sweep 1 (B):  d(qkv) from dO (= in1 [rows, d])          writes out [rows, 3 d]
 //   sweep 2 (TF): O' from (qkv)' (= in1 [rows, 3 d])        writes out [rows, d], P'

@@ -1,7 +1,7 @@
 """Multi-GPU restarts: independent trials shard one-per-rank, one MIN all-reduce selects the winner.
 
 The reference runs its restarts sequentially in one process (``optimization_based_attack.py:70-74``; there is no
-``torch.distributed`` call anywhere in it).  Trials only share read-only inputs, so the B200 layout is one process
+``torch.distributed`` call anywhere in it).  Trials only share read-only inputs, so the multi-GPU layout is one process
 per GPU with trial ``k`` on rank ``k mod world`` and **no data-path collective**.  Selection
 (``_select_optimal_reconstruction``, ``:206-218``: ``torch.min`` -> first index wins; non-finite -> +inf) becomes a
 single all-reduce(MIN) over a packed 63-bit key ``(sortable_float32_bits(score) << 31) | trial_index`` followed by

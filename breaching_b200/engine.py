@@ -239,7 +239,7 @@ class Engine:
     """One engine = one model replica + one trial state on one GPU."""
 
     def __init__(self, model, input_shape, cfg_attack, device, noise_seed=0, backend=None, program=None):
-        """``backend``: "tc" (tcgen05 TF32 tensor-core GEMMs, default; shapes it does not cover run on the fp32 SIMT
+        """``backend``: "tc" (TF32 tensor-core GEMMs, default; shapes it does not cover run on the fp32 SIMT
         kernels) or "simt" (fp32 CUDA-core GEMMs everywhere: bit-faithful fp32 products).  Default from
         ``BRE_GEMM_BACKEND``."""
         self.lib = load_library()

@@ -27,7 +27,7 @@ def reference_prepare_attack():
 
 
 def install():
-    """Rebind ``breaching.attacks.prepare_attack`` to the B200 engine.  Returns the original function."""
+    """Rebind ``breaching.attacks.prepare_attack`` to the engine.  Returns the original function."""
     from . import attacks as ours
 
     ref_attacks = importlib.import_module("breaching.attacks")

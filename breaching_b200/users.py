@@ -25,7 +25,7 @@ class UserSingleStep:
         self.loss_fn = loss_fn
         self.setup = dict(device=torch.device(setup["device"]), dtype=setup.get("dtype", torch.float))
         if self.setup["device"].type != "cuda":
-            raise EngineError("the B200 engine needs a CUDA device (there is no CPU fallback)")
+            raise EngineError("the engine needs a CUDA device (there is no CPU fallback)")
         name = getattr(loss_fn, "original_name", None) or type(loss_fn).__name__
         if name != "CrossEntropyLoss":
             raise NotImplementedError(f"user-side updates on the engine: CrossEntropyLoss only (got {name})")

@@ -1,4 +1,4 @@
-/* breaching_b200 -- C ABI of the sm_100a gradient-inversion engine.
+/* breaching_b200 -- C ABI of the sm_90a gradient-inversion engine.
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference has no native code and no FFI of its own; the
  * interface a maintainer would bind is the body of
@@ -262,8 +262,8 @@ int bre_token_match(const float* rec, const float* emb, const int64_t* subset, i
  * mode 0 fprop  : out[N,Ho,Wo,Co]  = conv(in[N,H,W,Ci], w[Co,R,S,Ci]) (+ conv(in2, w2) when in2 != NULL)
  * mode 1 dgrad  : din[N,H,W,Ci]    = conv^T(dout[N,Ho,Wo,Co], w) (+ conv^T(dout2, w2))
  * mode 2 wgrad  : dw[Co,R,S,Ci]    = sum_pixels dout (x) in
- * backend 0 = SIMT fp32, 1 = tcgen05 TF32 (where available, else BRE_ERR_UNSUPPORTED), 2 = the engine's dispatch
- * (tcgen05 where the shape is covered, SIMT otherwise). */
+ * backend 0 = SIMT fp32, 1 = TF32 tensor cores (where available, else BRE_ERR_UNSUPPORTED), 2 = the engine's dispatch
+ * (tensor cores where the shape is covered, SIMT otherwise). */
 int bre_conv_gemm(int32_t mode, int32_t backend, const float* a, const float* w, const float* a2, const float* w2,
                   float* out, int32_t N, int32_t H, int32_t W, int32_t Ci, int32_t Co, int32_t R, int32_t S,
                   int32_t stride, int32_t pad, void* stream);

@@ -2,7 +2,7 @@
 
 CPU restatement of the reference hot path (JonasGeiping/breaching,
 ``OptimizationBasedAttacker._run_trial`` and what it calls) used to *check* the
-sm_100a engine in ``breaching_b200``.  Nothing under ``breaching_b200/`` may
+sm_90a engine in ``breaching_b200``.  Nothing under ``breaching_b200/`` may
 import this package; only ``tests/``, ``__graft_entry__.smoke()`` and the
 ``cpu_baseline`` / ``--impl reference`` legs of ``bench.py`` do.
 

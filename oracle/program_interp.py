@@ -1,6 +1,6 @@
 """Torch (CPU) interpreter of the engine's four-sweep layer program.  TEST INFRASTRUCTURE ONLY.
 
-The sm_100a engine does not replay PyTorch's reverse-over-reverse autograd graph.  It evaluates
+The sm_90a engine does not replay PyTorch's reverse-over-reverse autograd graph.  It evaluates
 ``d Phi / d x`` for ``Phi(x) = h(G(x), g)``, ``G = grad_W L(x, W)`` as a *weight-direction tangent* of the
 input gradient (SURVEY.md section 7.3, DESIGN.md section 3):
 

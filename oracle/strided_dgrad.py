@@ -1,9 +1,9 @@
 """Specification (CPU, torch) of the strided data-gradient as per-parity-class stride-1 gathers -- the form in which the
-tcgen05 kernel can feed it through im2col-mode TMA tensor maps.  TEST INFRASTRUCTURE / design note, not product code.
+tensor-core kernel can feed it through im2col-mode TMA tensor maps.  TEST INFRASTRUCTURE / design note, not product code.
 
 Why: ``din[y, x] = sum_{r, s} dout[(y + pad - r) / st, (x + pad - s) / st] w[r, s]`` only has the taps with
 ``(y + pad - r) % st == 0``; a tensor map cannot express "every st-th tap", so ``igemm_tc.cu`` still stages strided dgrad with
-cp.async (10 % of a config-2 iteration, profiles/launches_r1_summary.txt).  Splitting the output pixels into the st x st
+cp.async.  Splitting the output pixels into the st x st
 classes ``(ey, ex) = ((y + pad) % st, (x + pad) % st)`` turns every class into a *stride-1* correlation of ``dout`` with the
 sub-kernel ``w[ey::st, ex::st]``:
 
@@ -13,7 +13,7 @@ sub-kernel ``w[ey::st, ex::st]``:
 which is an im2col load over ``dout`` with lower corner ``L = c - (T - 1)`` per axis, filter offset ``(T - 1) - t``, traversal
 stride 1 and an upper corner that makes the bounding box hold exactly the class's pixel count:  ``U = Hc - Ho + L``.
 ``class_plan`` returns those numbers; ``dgrad_by_classes`` evaluates the data gradient through a faithful emulation of the
-im2col traversal (``im2col_rows``: semantics established on the B200 with profiles/experiments/tma_im2col_probe.cu) and
+im2col traversal (``im2col_rows``, the semantics of CUDA's im2col-mode tensor maps) and
 ``tests/test_strided_dgrad_spec.py`` checks it against ``torch.nn.grad.conv2d_input``.
 """
 import torch

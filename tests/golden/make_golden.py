@@ -1,12 +1,13 @@
 """Generate the golden fixtures in this directory by running the UNMODIFIED reference.
 
-Run in the build container (needs /root/reference):  ``python tests/golden/make_golden.py``
+Run where the reference is importable (``BREACHING_REFERENCE_ROOT``, see oracle/refshim.py):
+``python tests/golden/make_golden.py [fixture names]``
 
 The reference ships no tests or golden vectors for the optimisation hot path (SURVEY.md section 4), so the parity pin
 is produced here: the reference attacker (``breaching.attacks.prepare_attack`` imported from /root/reference through
 ``oracle/refshim.py``) is driven on small seeded synthetic cases and its per-iteration outputs are stored.
 ``tests/test_golden.py`` checks the oracle restatement against these files on any machine; the ``-m gpu`` tests check
-the CUDA engine against them on the B200 box, where /root/reference does not exist.
+the CUDA engine against them on the GPU, where the reference need not be installed.
 """
 import copy
 import os
@@ -306,9 +307,56 @@ def lr_fixtures(ref):
 
 
 def config_fixtures():
-    names = ["invertinggradients", "modern", "seethroughgradients", "clsattack", "legacy", "sanitycheck", "tag",
-             "deepleakage", "beyondinfering", "wei", "multiscale_ghiasi", "_default_optimization_attack"]
+    return config_fixtures_for(["invertinggradients", "modern", "seethroughgradients", "clsattack", "legacy", "sanitycheck", "tag",
+                                "deepleakage", "beyondinfering", "wei", "multiscale_ghiasi", "_default_optimization_attack"])
 
+
+def dropin_fixtures(ref):
+    """What tests/test_install_dropin.py compares against: the reference's text prologue / token recovery on the miniature
+    causal-LM case, and gradients through an instance of the reference's own ``TransformerModel``."""
+    from torch.nn.attention import SDPBackend, sdpa_kernel
+
+    from breaching.cases.models.language_models import TransformerModel
+
+    out = {"analytic_cfg": config_fixtures_for(["analytic"])["analytic"]}
+    model, loss_fn, payload, shared, true = synthetic.make_text_case(batch=2, seq_len=6, seed=77)
+    cfg = refshim.load_reference_attack_cfg("tag", {})
+    att = ref.attacks.prepare_attack(model, loss_fn, cfg, dict(device=torch.device("cpu"), dtype=torch.float))
+    sh_ref = copy.deepcopy(shared)
+    rec_models, _, _ = att.prepare_attack(payload, sh_ref)
+    gen = torch.Generator().manual_seed(5)
+    tokens = true["data"]
+    dim = att.embeddings[0]["weight"].shape[1]
+    rec = dict(data=model.encoder.weight.detach()[tokens] + 0.01 * torch.randn(2, 6, dim, generator=gen), labels=tokens.clone())
+    recovered = {}
+    for mode in ("from-embedding", "from-labels", "from-limited-embedding"):
+        att.cfg.token_recovery = mode
+        recovered[mode] = att._postprocess_text_data(dict(data=rec["data"].clone(), labels=rec["labels"].clone()))["data"]
+    out["text"] = dict(embedding_dim=dim, data_shape=tuple(att.data_shape), gradients=sh_ref[0]["gradients"],
+                       embedding_grads=att.embeddings[0]["grads"], rec_data=rec["data"], labels=rec["labels"],
+                       encoder_is_identity=isinstance(rec_models[0].encoder, torch.nn.Identity),
+                       parameter_names=[n for n, _ in rec_models[0].named_parameters()], recovered=recovered)
+    torch.manual_seed(4)
+    tm = TransformerModel(ntokens=40, ninp=16, nhead=4, nhid=24, nlayers=2, dropout=0.0, positional_embedding="learnable").double().eval()
+    B, T = 2, 6
+    x = torch.randn(B, T, 16, dtype=torch.double)
+    q = torch.softmax(torch.randn(B, T, 40, dtype=torch.double), dim=-1)
+    names = [n for n, _ in tm.named_parameters()]
+    state = {k: v.clone() for k, v in tm.state_dict().items()}
+    tm.encoder = torch.nn.Identity()
+    params = [p for p in tm.parameters()]
+    with sdpa_kernel(SDPBackend.MATH):
+        loss = synthetic.causal_loss(tm(x), q)
+        G = torch.autograd.grad(loss, params)
+    # only the first T rows of the positional table are read (the rest have zero gradient): store those rows
+    pos = "pos_encoder.embedding.weight"
+    state[pos] = state[pos][:T].clone()
+    grads = [g[:T].clone() if n == pos else g for n, g in zip([n for n in names if n != "encoder.weight"], G)]
+    out["transformer"] = dict(parameter_names=names, state_dict=state, x=x, q=q, loss=float(loss), grads=grads)
+    return out
+
+
+def config_fixtures_for(names):
     def plain(node):
         if isinstance(node, dict):
             return {k: plain(v) for k, v in node.items()}
@@ -319,6 +367,8 @@ def config_fixtures():
 
 def main():
     ref = refshim.import_reference()
+    if not sys.argv[1:] or "dropin" in sys.argv[1:]:
+        torch.save(dropin_fixtures(ref), os.path.join(HERE, "dropin.pt"))
     torch.manual_seed(0)
     only = sys.argv[1:]   # optional: regenerate just the named fixtures
     for name, (case_kwargs, attack, overrides, iters) in {**CASES, **FEDAVG_CASES, **LBFGS_CASES, **MULTI_QUERY_CASES, **TRAIN_BN_CASES}.items():

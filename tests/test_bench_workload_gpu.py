@@ -1,6 +1,6 @@
 """Parity of the paths ``bench.py`` times, at the sizes it times them (VERDICT round 1, item 1).
 
-* config 2 (``bench.py`` default): tcgen05 back end, torchvision ResNet-18, 397 classes, 1x3x224x224, seed 233 -- one closure
+* config 2 (``bench.py`` default): tensor-core back end, torchvision ResNet-18, 397 classes, 1x3x224x224, seed 233 -- one closure
   evaluation against the CPU oracle in float32 and float64, with the *reference's own* GPU numerics (eager PyTorch, cuDNN TF32
   convolutions = torch's default) as the yardstick for the TF32 gradient; a 50-iteration trajectory; and
 * a long-run quality test (>= 1000 iterations, 64x64, 3 seeds): final objective and PSNR against the ground truth
@@ -102,7 +102,7 @@ def test_config2_tc_closure_at_the_benchmarked_size():
     # fp32 back end: the algorithm, to fp32 noise (SURVEY 7.4(3)(ii): 1e-3 / 99 %)
     v, r, s, g = res["simt"]
     assert math.isclose(v, float(phi64), rel_tol=2e-4) and r < max(1e-3, 2 * dev_fp32) and s > 0.99 and g < 1e-3, res["simt"]
-    # tcgen05 back end: objective to 2e-3; gradient no further from float64 than 1.5x the reference's own TF32 GPU path
+    # tensor-core back end: objective to 2e-3; gradient no further from float64 than 1.5x the reference's own TF32 GPU path
     v, r, s, g = res["tc"]
     assert math.isclose(v, float(phi64), rel_tol=2e-3), (v, float(phi64))
     assert r < 1.5 * max(dev_tf32, 2e-3), (r, dev_tf32)
@@ -113,7 +113,7 @@ def test_config2_tc_closure_at_the_benchmarked_size():
 
 
 def test_config2_tc_trajectory_50_iterations():
-    """50 signed-Adam iterations from the same initial candidate: the objective history of the tcgen05 engine against the CPU
+    """50 signed-Adam iterations from the same initial candidate: the objective history of the tensor-core engine against the CPU
     oracle (fp32) and against the reference's GPU numerics.  A hard sign() turns numerically-zero gradient entries into +-lr
     jumps, so two correct implementations drift apart pixel-wise; the yardstick is how far the reference's own TF32 GPU run
     drifts from its CPU run."""
@@ -155,7 +155,7 @@ def _psnr(rec, true, meta):
 
 def test_long_run_quality_inside_the_reference_spread():
     """1200 iterations of `invertinggradients` on a 64x64 ResNet-18 case, three initialisations: final objective and PSNR
-    against the ground truth for the engine (tcgen05 and fp32 back ends) and for the reference algorithm run in eager PyTorch
+    against the ground truth for the engine (tensor-core and fp32 back ends) and for the reference algorithm run in eager PyTorch
     on the same GPU.  Different summation orders + hard sign = different trajectories; the claim is statistical: the engine's
     results lie inside the reference's spread."""
     model, loss_fn, payload, shared, true = synthetic.make_case("resnet18", "imagenet", batch=1, seed=233, bn_random=True, image_size=64,

@@ -1,4 +1,4 @@
-"""Engine-level parity on the B200: objective, parameter gradients and d(objective)/d(candidate) of one closure
+"""Engine-level parity on the GPU: objective, parameter gradients and d(objective)/d(candidate) of one closure
 evaluation; short trajectories; the attacker API -- against the CPU oracle and the reference's golden fixtures."""
 import copy
 import math
@@ -291,7 +291,7 @@ def test_config3_resnet50_batch8_full_size_closure():
     phi64, _, raw64, _ = o64.closure_gradient(x.double(), 0, 0.0)
     ref_err = _relerr(raw, raw64)
     # ... and under TF32 products the gradient of this case is dominated by rounding noise: the reference's own GPU path
-    # (eager PyTorch with cuDNN TF32 convolutions, torch's default) is O(1) away from float64.  The tcgen05 back end is
+    # (eager PyTorch with cuDNN TF32 convolutions, torch's default) is O(1) away from float64.  The tensor-core back end is
     # held to that deviation; its forward quantities (objective, BN-statistics prior) are checked tightly above.
     tf32_err = _reference_tf32_deviation(m_gpu, loss_fn, cfg, shared, labels, dm, ds, x, raw64)
     print("config 3 gradient deviations from float64: fp32 CPU reference", ref_err, "TF32 GPU reference", tf32_err)

@@ -1,4 +1,4 @@
-"""Per-kernel parity on the B200: each CUDA kernel, called through the C ABI, against a torch fp32/fp64 restatement."""
+"""Per-kernel parity on the GPU: each CUDA kernel, called through the C ABI, against a torch fp32/fp64 restatement."""
 import math
 
 import pytest
@@ -142,7 +142,7 @@ TC_SHAPES = [s for s in CONV_SHAPES if s[3] % 32 == 0 and s[4] % 64 == 0] + [
 
 @pytest.mark.parametrize("shape", TC_SHAPES)
 def test_conv_tcgen05_tf32_backend(shape):
-    """tcgen05 TF32 back end (tensor cores, TMEM accumulators): TF32 products (10-bit mantissa), fp32 accumulation,
+    """TF32 tensor-core back end (tensor cores: wgmma / mma.sync): TF32 products (10-bit mantissa), fp32 accumulation,
     tolerance 2e-3 relative l2 -- the precision of the reference's default cuDNN TF32 conv path."""
     N, H, W, Ci, Co, R, st, pd = shape
     x = _rand(N, Ci, H, W, seed=1)
@@ -220,7 +220,7 @@ def test_small_row_linear_kernels_match_float64(rows, Ci, Co):
     def rel(a, b):
         return ((a.double() - b).norm() / b.norm()).item()
 
-    for backend, tol in ((0, 2e-6), (2, 2e-3)):   # 2 = engine dispatch: TF32 products where the tcgen05 kernel takes the shape
+    for backend, tol in ((0, 2e-6), (2, 2e-3)):   # 2 = engine dispatch: TF32 products where the tensor-core kernel takes the shape
         out = torch.empty(rows, Co, device=dev)
         E.conv_gemm(0, x, w, out, *geom, backend=backend)
         assert rel(out, x.double() @ w.double().T) < tol, ("fprop", backend)

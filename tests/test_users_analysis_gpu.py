@@ -46,7 +46,7 @@ def test_user_gradient_matches_autograd(arch, size, batch):
     user_tc = UserSingleStep(model, loss_fn, dict(SETUP), batch, backend="tc")
     sd_tc, _ = user_tc.compute_local_updates(payload[0], dict(inputs=true["data"], labels=true["labels"]))
     rel, worst = _update_error(sd_tc["gradients"], shared[0]["gradients"])
-    # measured on the B200: ResNet-18 2.2e-2 / 5.9e-2; ConvNet-tiny 1.4e-3 overall, 0.23 on its smallest-norm tensor
+    # typical: ResNet-18 ~2e-2 / ~6e-2; ConvNet-tiny ~1e-3 overall, ~0.2 on its smallest-norm tensor
     assert rel < 4e-2 and worst < 0.5, (rel, worst)
 
 
