@@ -401,6 +401,13 @@ struct bre_engine {
     const bre_op_desc& nx = ops[i + 1];
     return nx.kind == BRE_OP_BNACT && nx.tin == ops[i].tout && !nx.bn_train && igemm_tc_supported(a);
   }
+  // what the last sweeps did per op (bre_engine_debug_op): 1 = ran in the epilogue of the preceding GEMM (last forward),
+  // 2 = its input tangent (the pre-BN tangent) was not stored (last tangent-forward sweep)
+  std::vector<unsigned char> op_flags;
+  void clear_op_flags(unsigned char bits) {
+    op_flags.resize(ops.size(), 0);
+    for (unsigned char& f : op_flags) f &= (unsigned char)~bits;
+  }
   int consumers_of(int tensor) const {
     int n = 0;
     for (const bre_op_desc& o : ops) n += (o.tin == tensor) + (o.res == tensor);
@@ -437,6 +444,7 @@ struct bre_engine {
 
   // ---- sweeps ---------------------------------------------------------------------------------------
   int sweep_forward() {
+    clear_op_flags(1);
     for (size_t i = 0; i < ops.size(); ++i) {
       const bre_op_desc& op = ops[i];
       const bre_tensor_desc& to = td(op.tout);
@@ -462,6 +470,7 @@ struct bre_engine {
             a.epi.kind = 1; a.epi.has_bn = nx.has_bn != 0; a.epi.relu = nx.relu != 0; a.epi.round_out = round_val(nx.tout);
             a.epi.out2 = t[nx.tout].val; a.epi.res = nx.res >= 0 ? t[nx.res].val : nullptr;
             a.epi.scale = c.scale; a.epi.shift = c.shift;
+            op_flags[i + 1] |= 1;
             ++i;   // the BNACT op ran in the epilogue
           }
           BRE_LAUNCH(gemm(a));
@@ -613,6 +622,7 @@ struct bre_engine {
   }
 
   int sweep_tangent_forward() {
+    clear_op_flags(2);
     for (size_t i = 0; i < ops.size(); ++i) {
       const bre_op_desc& op = ops[i];
       const bre_tensor_desc& to = td(op.tout);
@@ -645,7 +655,9 @@ struct bre_engine {
             a.epi.scale = c.scale; a.epi.inv = c.inv; a.epi.nrm = c.nrm;
             a.epi.v_gamma = nx.has_bn ? Vp(nx.gamma) : nullptr; a.epi.v_beta = nx.has_bn ? Vp(nx.beta) : nullptr;
             a.epi.pre = t[nx.tin].val; a.epi.post = t[nx.tout].val;
-            if (consumers_of(op.tout) == 1) a.out = nullptr;   // nobody else reads the pre-BN tangent
+            // nobody else reads the pre-BN tangent -- unless this BN's tangent-backward reduces the tangent of its gamma gradient
+            // from it (FedAvg steps k > 0, bnact_tan_bwd_g_kernel)
+            if (consumers_of(op.tout) == 1 && !want_tangent_G) { a.out = nullptr; op_flags[i + 1] |= 2; }
             ++i;
           }
           BRE_LAUNCH(gemm(a));
@@ -1745,9 +1757,15 @@ int bre_engine_last_terms(bre_engine* e, double* terms6) {
 }
 
 int bre_engine_debug_param(bre_engine* e, int32_t which, int32_t index, float* out_host) {
-  if (!e || !out_host || index < 0 || index >= (int)e->params.size() || which < 0 || which > 3) return BRE_ERR_INVALID;
+  if (!e || !out_host || index < 0 || index >= (int)e->params.size() || which < 0 || which > 5) return BRE_ERR_INVALID;
   BRE_CUDA_CHECK(cudaSetDevice(e->device));
-  const float* arenas[4] = {e->G, e->V, e->W, e->g};
+  // 4 / 5: the direction / weights as the GEMMs read them -- the TF32 shadow for the weight of a layer that Vg / Wg route to it
+  bool shadow = false;
+  if (which >= 4)
+    for (const bre_op_desc& op : e->ops)
+      if ((op.kind == BRE_OP_CONV || op.kind == BRE_OP_LINEAR) && op.w == index && e->round_val(op.tin) && !e->is_precise(e->op_index(op)))
+        shadow = true;
+  const float* arenas[6] = {e->G, e->V, e->W, e->g, shadow ? e->Vt : e->V, shadow ? e->Wt : e->W};
   const ParamInfo& pi = e->params[index];
   const float* src = arenas[which] + pi.off;
   if (pi.desc.perm != BRE_PERM_NONE) {
@@ -1772,6 +1790,13 @@ int bre_engine_debug_tensor(bre_engine* e, int32_t which, int32_t tensor, float*
   }
   BRE_CUDA_CHECK(cudaMemcpyAsync(out_host, src, tb.numel * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
   BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  return BRE_OK;
+}
+
+int bre_engine_debug_op(bre_engine* e, int32_t op, int32_t* flags) {
+  if (!e || !flags || op < 0 || op >= (int)e->ops.size()) return BRE_ERR_INVALID;
+  e->op_flags.resize(e->ops.size(), 0);
+  *flags = e->op_flags[op] | (e->use_stem_cols((size_t)op) ? 4 : 0);
   return BRE_OK;
 }
 

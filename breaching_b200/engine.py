@@ -78,7 +78,7 @@ EXPORTS = [
     "bre_engine_load_feature_targets", "bre_engine_set_local_steps", "bre_engine_begin_trial", "bre_engine_run", "bre_engine_run_timed", "bre_engine_sync",
     "bre_engine_status", "bre_engine_read_history", "bre_engine_get_best", "bre_engine_get_candidate",
     "bre_engine_score", "bre_engine_objective_and_gradient", "bre_engine_last_terms", "bre_engine_debug_param",
-    "bre_engine_debug_tensor", "bre_engine_launches_per_iteration", "bre_engine_set_option", "bre_match_reduce",
+    "bre_engine_debug_tensor", "bre_engine_debug_op", "bre_engine_launches_per_iteration", "bre_engine_set_option", "bre_match_reduce",
     "bre_total_variation", "bre_conv_gemm", "bre_last_error", "bre_version",
     "bre_engine_load_soft_labels", "bre_engine_label_gradient", "bre_engine_set_labels",
     "bre_token_layernorm", "bre_token_attention", "bre_token_match",
@@ -126,6 +126,7 @@ def load_library(path=None):
     lib.bre_engine_last_terms.argtypes = [vp, P(ctypes.c_double)]
     lib.bre_engine_debug_param.argtypes = [vp, i32, i32, vp]
     lib.bre_engine_debug_tensor.argtypes = [vp, i32, i32, vp]
+    lib.bre_engine_debug_op.argtypes = [vp, i32, P(i32)]
     lib.bre_engine_launches_per_iteration.argtypes = [vp, P(i32)]
     lib.bre_engine_set_option.argtypes = [vp, ctypes.c_char_p, i64]
     lib.bre_match_reduce.argtypes = [vp, vp, vp, i64, f32, P(ctypes.c_double), vp]
@@ -519,7 +520,8 @@ class Engine:
     def debug_param(self, which, index):
         p = self.prog.params[index]
         out = torch.empty(p.shape, dtype=torch.float32)
-        code = {"G": 0, "v": 1, "W": 2, "g": 3}[which]
+        # "v_operand" / "W_operand": what the GEMMs read (the TF32 shadow for tensor-core layers; "v" is stale for those)
+        code = {"G": 0, "v": 1, "W": 2, "g": 3, "v_operand": 4, "W_operand": 5}[which]
         _check(self.lib, self.lib.bre_engine_debug_param(self.h, code, index, _ptr(out)), "bre_engine_debug_param")
         return out
 
@@ -529,6 +531,13 @@ class Engine:
         code = {"val": 0, "delta": 1, "tangent": 2, "tangent_delta": 3}[which]
         _check(self.lib, self.lib.bre_engine_debug_tensor(self.h, code, tid, _ptr(out)), "bre_engine_debug_tensor")
         return out
+
+    def debug_op(self, index):
+        """What the engine did with op ``index`` in the last sweeps: dict(fused, tangent_in_unwritten, stem_columns)."""
+        out = ctypes.c_int32()
+        _check(self.lib, self.lib.bre_engine_debug_op(self.h, int(index), ctypes.byref(out)), "bre_engine_debug_op")
+        f = out.value
+        return dict(fused=bool(f & 1), tangent_in_unwritten=bool(f & 2), stem_columns=bool(f & 4))
 
     def launches_per_iteration(self):
         out = ctypes.c_int32()

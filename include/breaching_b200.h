@@ -170,10 +170,20 @@ int bre_engine_objective_and_gradient(bre_engine* e, const float* candidate, dou
 /* Objective terms of the last evaluation: match, task loss, tv, norm, deep inversion, features. */
 int bre_engine_last_terms(bre_engine* e, double* terms6);
 /* Debug access (tests): parameter-gradient list G / direction v in torch layout for parameter `index`;
- * which: 0 = G, 1 = v, 2 = W, 3 = g.  out: host, numel floats. */
+ * which: 0 = G, 1 = v, 2 = W, 3 = g, 4 = v as the GEMMs read it, 5 = W as the GEMMs read it.  out: host, numel floats.
+ * On the tensor-core back end the single-step direction of the weights of tensor-core layers is written to its TF32 shadow
+ * only, so which = 1 returns stale memory for them; which = 4 / 5 return the TF32 shadow for those weights and the fp32
+ * arena for every other parameter. */
 int bre_engine_debug_param(bre_engine* e, int32_t which, int32_t index, float* out_host);
-/* which: 0 = activation, 1 = delta (sweep B), 2 = tangent, 3 = tangent delta; NCHW fp32 to host. */
+/* which: 0 = activation, 1 = delta (sweep B), 2 = tangent, 3 = tangent delta; NCHW fp32 to host.  Tensor 0 (the candidate)
+ * has no tangent; its delta is the task-loss gradient and its tangent delta the candidate gradient.  With fuse_bnact, the
+ * tangent of a conv output whose only consumer is the BN op fused into the conv's epilogue is not written in single-step
+ * evaluations (it holds whatever an earlier evaluation left). */
 int bre_engine_debug_tensor(bre_engine* e, int32_t which, int32_t tensor, float* out_host);
+/* What the engine did with op `op` (tests): bit 0 = it ran in the epilogue of the preceding tensor-core GEMM in the last forward
+ * sweep (fuse_bnact), bit 1 = its input tangent was not stored in the last tangent-forward sweep (that fused case), bit 2 = the
+ * op runs on the column path of the candidate-fed convolution, which rounds the candidate, weight and direction to TF32 itself. */
+int bre_engine_debug_op(bre_engine* e, int32_t op, int32_t* flags);
 /* Number of kernel launches per iteration (for gpu_launches in bench.py) and whether graphs are used. */
 int bre_engine_launches_per_iteration(bre_engine* e, int32_t* out);
 int bre_engine_set_option(bre_engine* e, const char* name, int64_t value);

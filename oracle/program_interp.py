@@ -74,6 +74,11 @@ def objective_direction(kind, G, g, scale=1.0, tag_scale=0.1, scale_scheme="line
 class ProgramInterpreter:
     """Evaluates the program with torch ops.  Parameters / running stats are read from ``model``."""
 
+    # test hook: tamper(sweep, op_index, tensor_id, stored, contribution=None) -> what is stored instead, called whenever a
+    # tangent (sweep "TF") or a (tangent) delta accumulation (sweeps "B" / "TB", ``contribution`` = this op's term) is stored,
+    # so that a corrupted buffer propagates to the ops that read it as a faulty kernel's output would
+    tamper = None
+
     def __init__(self, model, prog, dtype=torch.float64):
         self.prog = prog
         self.dtype = dtype
@@ -205,6 +210,8 @@ class ProgramInterpreter:
 
         def add(tid, val):
             d[tid] = val if tid not in d else d[tid] + val
+            if self.tamper is not None:
+                d[tid] = self.tamper("B" if V is None else "TB", i, tid, d[tid], contribution=val)
 
         for i in reversed(range(len(prog.ops))):
             op = prog.ops[i]
@@ -387,6 +394,8 @@ class ProgramInterpreter:
                 Sd = (Qd @ K.transpose(-1, -2) + Q @ Kd.transpose(-1, -2)) * sc
                 Pd = P_ * (Sd - (P_ * Sd).sum(dim=-1, keepdim=True))
                 ta[op.tout], self.taux[i] = self._merge_heads(Pd @ Vv + P_ @ Vd), (Qd, Kd, Vd, Pd)
+            if self.tamper is not None:
+                ta[op.tout] = self.tamper("TF", i, op.tout, ta[op.tout])
         self.ta = ta
         return ta
 
@@ -406,6 +415,7 @@ class ProgramInterpreter:
             return d[0].flatten(1).view(n // T, T, -1)
         seed = (p * zdot - p * (p * zdot).sum(dim=1, keepdim=True)) / n
         d, _, _ = self._reverse(seed, V=V, d_prev=self.d_B, inject=inject)
+        self.d_T, self.inject = d, inject or {}
         return d[0]
 
     # ------------------------------------------------------------------ regulariser adjoints
@@ -447,6 +457,7 @@ class ProgramInterpreter:
         G = self.backward(want_dx=task_regularization != 0)
         gg = [t.to(self.dtype) for t in g]
         val, V = objective_direction(kind, G, gg, scale=scale, **kw)
+        self.V = V
         self.tangent_forward(V)
         inject = inject_fn(self) if inject_fn is not None else None
         dx = self.tangent_backward(V, inject)

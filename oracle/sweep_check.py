@@ -1,0 +1,575 @@
+"""Layer-local check of the engine's four sweeps.  TEST INFRASTRUCTURE ONLY.
+
+The closure-level tests compare one number and one image-sized gradient at the end of some two hundred launches, so their
+tolerances have to absorb the conditioning of the whole network.  This checker judges every kernel on its own: for every op
+and every sweep it recomputes, in float64, *that op's output from the engine's own inputs to that op* (the rules of
+``oracle/program_interp.py`` applied locally) and compares it element by element with what the engine stored, against a
+rounding-error bound derived for that element:
+
+  * GEMM outputs (conv / linear, one or two sources): ``(K + 2) 2^-23 (|A| * |B|)`` with ``|A| * |B|`` the same op on
+    absolute values and K the reduction length (Higham's summation bound with 2u, which also covers accumulation that does
+    not round to nearest).  The reference uses the operands the kernel read: activations and deltas as stored (the engine
+    stores tensor-core operands on the TF32 grid), weights / direction in operand form (``W_operand`` / ``v_operand``),
+    and the candidate and weights rounded to TF32 for an op whose kernel rounds them itself (the stem column path).
+    TF32 x TF32 products are exact in fp32, so no TF32 term is needed.
+  * element-wise ops: a few fp32 ulps of the magnitudes involved;
+  * reductions (bias sums, BN gamma / beta gradients, pooling): ``(P + 4) 2^-23 sum |terms|``;
+  * train-mode BN and the DeepInversion adjoints (composites of per-channel batch statistics and element-wise terms):
+    ``TRAIN_C (P + 8) 2^-24`` times the magnitudes, with the conditioning of the variance / norm differences as a factor;
+  * a tensor-core layer (weights read from the TF32 shadow) whose activation operand is stored off the TF32 grid has that
+    operand truncated by the tensor core: its bound is widened by 2^-10 of the magnitudes and the op is listed in
+    ``off_grid`` (this contradicts the intent of the engine's rounding flags; today: convolutions fed by a max-pool);
+  * a stored tensor whose every element lies on the TF32 grid (13 low mantissa bits zero) was rounded on store: half a
+    TF32 ulp of the reference (per accumulation for deltas summed over several consumers) is added.
+
+``delta[t]`` / ``tangent_delta[t]`` are checked as the sum over *all* consumers of ``t`` (residual branches included), which
+judges the accumulation flags; such a failure is reported at the consumer that runs last in the reverse sweep (the one with
+the lowest op index), where the buffer becomes final.
+
+A buffer source provides ``tensor(which, tid)`` (``which`` in val / delta / tangent / tangent_delta, NCHW, ``None`` where a
+tensor has no such buffer), ``param(which, index)`` (G / v_operand / W_operand, torch layout), ``unwritten`` (tensor ids whose
+tangent is not stored because the BN op reading it ran in the producing GEMM's epilogue; that pair is then checked as one)
+and ``rounds_operands(op_index)``.
+"""
+import torch
+import torch.nn.functional as F
+
+from breaching_b200 import compiler as C
+from oracle.program_interp import objective_direction
+from oracle import restate
+
+U = 2.0 ** -24          # fp32 unit roundoff
+U2 = 2.0 ** -23         # 2u per accumulation step
+TF32_HALF = 2.0 ** -11  # half a TF32 ulp, relative
+TINY = 1e-30
+TRAIN_C = 8.0           # stated constant of the composite train-mode BN / DeepInversion bounds
+
+
+def rna(t):
+    """float64 tensor -> its fp32 value rounded to the TF32 grid, ties away from zero (``cvt.rna.tf32.f32``)."""
+    f = t.to(torch.float32).contiguous()
+    r = torch.bitwise_and(f.view(torch.int32) + 0x1000, -0x2000).view(torch.float32)
+    return r.to(torch.float64)
+
+
+def on_grid(t):
+    """True if every element of ``t`` (fp32 values) has its 13 low mantissa bits zero."""
+    f = t.to(torch.float32).contiguous()
+    return bool((torch.bitwise_and(f.view(torch.int32), 0x1FFF) == 0).all())
+
+
+class Finding:
+    def __init__(self, op, kind, sweep, what, index, value, ref, err, bound):
+        self.op, self.kind, self.sweep, self.what = op, kind, sweep, what
+        self.index, self.value, self.ref, self.err, self.bound = index, value, ref, err, bound
+
+    def __repr__(self):
+        return (f"op {self.op} ({self.kind}), sweep {self.sweep}, {self.what}: worst element {self.index} = {self.value:.9g}, "
+                f"reference {self.ref:.9g}, error {self.err:.3g} > bound {self.bound:.3g}")
+
+
+class SweepCheckError(AssertionError):
+    pass
+
+
+class SweepChecker:
+    """``params``: float64 parameters in ``model.parameters()`` order (what the engine loaded); ``bn``: per op (rm, rv) or None;
+    ``g``: target gradients; ``objective``: dict(kind, scale, task_regularization, tv=dict(scale, inner_exp, outer_exp, eps,
+    double_opponents) | None, norm=dict(scale, p) | None, di=dict(scale, first_bn_multiplier) | None,
+    features=dict(scale, measured) | None)."""
+
+    def __init__(self, prog, params, bn, g, labels, objective, source):
+        self.prog, self.src = prog, source
+        self.P = [p.detach().double() for p in params]
+        self.bn = bn
+        self.g = [t.detach().double() for t in g]
+        self.labels = labels
+        self.obj = dict(scale=1.0, task_regularization=0.0, tv=None, norm=None, di=None, features=None)
+        self.obj.update(objective)
+        self.findings, self.ratios, self.off_grid = [], {}, set()
+        ops = prog.ops
+        self.first_consumer = {}
+        for i, op in enumerate(ops):
+            for t in (op.tin, op.res):
+                if t >= 0 and t not in self.first_consumer:
+                    self.first_consumer[t] = i
+        self._cache = {}
+
+    # ------------------------------------------------------------------ buffers
+    def T(self, which, tid):
+        key = (which, tid)
+        if key not in self._cache:
+            v = self.src.tensor(which, tid)
+            self._cache[key] = None if v is None else v.double()
+        return self._cache[key]
+
+    def Pm(self, which, idx):
+        key = ("p", which, idx)
+        if key not in self._cache:
+            self._cache[key] = self.src.param(which, idx).double()
+        return self._cache[key]
+
+    # ------------------------------------------------------------------ comparison
+    def _cmp(self, i, sweep, what, y, ref, bound):
+        kind = "objective" if i < 0 else C.OP_NAMES[self.prog.ops[i].kind]
+        err = (y - ref).abs()
+        ratio = err / bound.clamp_min(TINY) if torch.is_tensor(bound) else err / max(bound, TINY)
+        ratio = torch.where(err == 0, torch.zeros_like(ratio), ratio)
+        worst = float(ratio.max()) if ratio.numel() else 0.0
+        key = (kind, sweep)
+        self.ratios[key] = max(self.ratios.get(key, 0.0), worst)
+        if not worst <= 1.0:   # also catches NaN
+            j = int(torch.nan_to_num(ratio, nan=float("inf")).flatten().argmax())
+            idx = tuple(int(v) for v in torch.unravel_index(torch.tensor(j), y.shape)) if y.dim() else ()
+            b = bound.expand_as(ref).flatten()[j] if torch.is_tensor(bound) else torch.tensor(bound)
+            self.findings.append(Finding(i, kind, sweep, what, idx, float(y.flatten()[j]), float(ref.flatten()[j]),
+                                         float(err.flatten()[j]), float(b)))
+
+    @staticmethod
+    def _rounded(y, ref):
+        """Half a TF32 ulp of the reference where the engine stored ``y`` on the TF32 grid."""
+        return TF32_HALF * ref.abs() if on_grid(y) else 0.0
+
+    # ------------------------------------------------------------------ GEMM helpers
+    def _gemm_fwd(self, op, act, wgt):
+        if op.kind == C.OP_CONV:
+            return F.conv2d(act, wgt, None, stride=op.stride, padding=op.pad)
+        return F.linear(act.reshape(act.shape[0], -1), wgt).view(act.shape[0], -1, 1, 1)
+
+    def _gemm_dgrad(self, op, shape, wgt, dout):
+        if op.kind == C.OP_CONV:
+            return torch.nn.grad.conv2d_input(shape, wgt, dout, stride=op.stride, padding=op.pad)
+        return (dout.reshape(dout.shape[0], -1) @ wgt).view(shape)
+
+    def _gemm_wgrad(self, op, act, shape, dout):
+        if op.kind == C.OP_CONV:
+            return torch.nn.grad.conv2d_weight(act, shape, dout, stride=op.stride, padding=op.pad)
+        return dout.reshape(dout.shape[0], -1).t() @ act.reshape(act.shape[0], -1)
+
+    def _K(self, op, mode):
+        ti, to = self.prog.tensors[op.tin], self.prog.tensors[op.tout]
+        if op.kind == C.OP_LINEAR:
+            return {"fprop": ti.C * ti.H * ti.W, "dgrad": to.C, "wgrad": ti.N}[mode]
+        return {"fprop": ti.C * op.R * op.S, "dgrad": to.C * op.R * op.S + op.R * op.S, "wgrad": to.N * to.H * to.W}[mode]
+
+    def _operands(self, i, op):
+        """(activation, W, v) as the kernels of op i read them."""
+        a = self.T("val", op.tin)
+        W, V = self.Pm("W_operand", op.w), self.Pm("v_operand", op.w)
+        if self.src.rounds_operands(i):
+            a, W, V = rna(a), rna(W), rna(V)
+        return a, W, V
+
+    def _truncation(self, i, op, a):
+        """Relative widening for a tensor-core layer (its weights are read from the TF32 shadow) whose activation operand is
+        stored off the TF32 grid: the tensor core truncates it (up to 2^-10 relative).  Recorded in ``off_grid``."""
+        if self.src.rounds_operands(i) or not on_grid(self.Pm("W_operand", op.w)) or on_grid(a) or on_grid(self.P[op.w]):
+            return 0.0
+        self.off_grid.add(i)
+        return 2.0 ** -10
+
+    # ------------------------------------------------------------------ BN helpers
+    def _bn_eval(self, i, op):
+        rm, rv = self.bn[i]
+        inv = 1.0 / torch.sqrt(rv + op.eps)
+        gam, bet = self.P[op.gamma], self.P[op.beta]
+        v = lambda t: t.view(1, -1, 1, 1)  # noqa: E731
+        return v(rm), v(inv), v(gam), v(bet)
+
+    @staticmethod
+    def _m(t):
+        return t.mean(dim=(0, 2, 3), keepdim=True)
+
+    def _bn_train(self, op, x):
+        mean = self._m(x)
+        var = ((x - mean) ** 2).mean(dim=(0, 2, 3), keepdim=True)
+        inv = 1.0 / torch.sqrt(var + op.eps)
+        xh = (x - mean) * inv
+        # conditioning of the fp32 batch statistics: E[x^2] / var (variance by differences) and the pixel count
+        Pch = x.shape[0] * x.shape[2] * x.shape[3]
+        cond = 1.0 + self._m(x * x) / var.clamp_min(TINY)
+        return mean, var, inv, xh, TRAIN_C * (Pch + 8) * U * cond
+
+    # ------------------------------------------------------------------ sweeps
+    def check(self, raise_on_failure=True):
+        self.forward()
+        self.backward()
+        self.direction()
+        self.tangent_forward()
+        self.tangent_backward()
+        if raise_on_failure and self.findings:
+            raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
+        return self.findings
+
+    def forward(self):
+        prog = self.prog
+        for i, op in enumerate(prog.ops):
+            y = self.T("val", op.tout)
+            x = self.T("val", op.tin)
+            if op.kind in (C.OP_CONV, C.OP_LINEAR):
+                a, W, _ = self._operands(i, op)
+                ref = self._gemm_fwd(op, a, W)
+                mag = self._gemm_fwd(op, a.abs(), W.abs())
+                if op.b >= 0:
+                    b = self.P[op.b].view(1, -1, 1, 1)
+                    ref, mag = ref + b, mag + b.abs()
+                bound = ((self._K(op, "fprop") + 2) * U2 + self._truncation(i, op, a)) * mag
+                self._cmp(i, "F", f"val[t{op.tout}]", y, ref, bound + self._rounded(y, ref))
+            elif op.kind == C.OP_BNACT:
+                u, mag = x, x.abs()
+                if op.has_bn and op.bn_train:
+                    mean, var, inv, xh, c = self._bn_train(op, x)
+                    gam, bet = self.P[op.gamma].view(1, -1, 1, 1), self.P[op.beta].view(1, -1, 1, 1)
+                    u = gam * xh + bet
+                    mag = c * (gam.abs() * inv * (x.abs() + mean.abs())) / U + bet.abs()
+                elif op.has_bn:
+                    rm, inv, gam, bet = self._bn_eval(i, op)
+                    u = gam * inv * x + (bet - gam * rm * inv)
+                    mag = (gam * inv * x).abs() + bet.abs() + (gam * rm * inv).abs()
+                if op.res >= 0:
+                    r = self.T("val", op.res)
+                    u, mag = u + r, mag + r.abs()
+                ref = torch.relu(u) if op.relu else u
+                self._cmp(i, "F", f"val[t{op.tout}]", y, ref, 8 * U * mag + self._rounded(y, ref))
+            elif op.kind == C.OP_MAXPOOL:
+                ref = F.max_pool2d(x, op.R, op.stride, op.pad)
+                self._cmp(i, "F", f"val[t{op.tout}]", y, ref, 0.0)
+            elif op.kind == C.OP_AVGPOOL:
+                hw = x.shape[2] * x.shape[3]
+                ref = x.mean(dim=(2, 3), keepdim=True)
+                self._cmp(i, "F", f"val[t{op.tout}]", y, ref, (hw + 2) * U2 * x.abs().mean(dim=(2, 3), keepdim=True))
+        # cross-entropy seed of sweep B
+        z = self.T("val", prog.logits).flatten(1)
+        n = z.shape[0]
+        p = torch.softmax(z, dim=1)
+        onehot = F.one_hot(self.labels.view(-1).long(), z.shape[1]).double()
+        ref = (p - onehot) / n
+        rng = (z - z.max(dim=1, keepdim=True).values).abs()
+        bound = (16 + 2 * rng) * U * (p + onehot) / n
+        d = self.T("delta", prog.logits).flatten(1)
+        self._cmp(len(prog.ops) - 1, "F", f"delta[t{prog.logits}] (cross-entropy seed)", d, ref, bound)
+        self.p = p
+
+    def _reverse(self, sweep):
+        """Contributions of every op to the deltas (B) or tangent deltas (TB) of its inputs; returns {tid: [(i, ref, bound, mag)]}."""
+        prog = self.prog
+        tang = sweep == "TB"
+        dn = "tangent_delta" if tang else "delta"
+        contrib = {}
+
+        def add(tid, i, ref, bound, mag):
+            contrib.setdefault(tid, []).append((i, ref, bound, mag))
+
+        for i in reversed(range(len(prog.ops))):
+            op = prog.ops[i]
+            x = self.T("val", op.tin)
+            dout = self.T(dn, op.tout)
+            if op.kind in (C.OP_CONV, C.OP_LINEAR):
+                a, W, V = self._operands(i, op)
+                want_in = op.tin != 0 or tang or self.obj["task_regularization"] != 0
+                if want_in:
+                    K = self._K(op, "dgrad")
+                    ref = self._gemm_dgrad(op, x.shape, W, dout)
+                    mag = self._gemm_dgrad(op, x.shape, W.abs(), dout.abs())
+                    if tang:
+                        dB = self.T("delta", op.tout)
+                        ref = ref + self._gemm_dgrad(op, x.shape, V, dB)
+                        mag = mag + self._gemm_dgrad(op, x.shape, V.abs(), dB.abs())
+                        K = 2 * K
+                    add(op.tin, i, ref, (K + 2) * U2 * mag, mag)
+                if tang and self.obj["features"] is not None and op.kind == C.OP_LINEAR and \
+                        i == max(j for j, o in enumerate(prog.ops) if o.kind == C.OP_LINEAR):
+                    fs = self.obj["features"]
+                    diff = x.reshape(x.shape[0], -1) - fs["measured"].double().reshape(x.shape[0], -1)
+                    adj = (2.0 * fs["scale"] / diff.numel() * diff).view_as(x)
+                    add(op.tin, i, adj, 8 * U * (adj.abs() + 2.0 * fs["scale"] / diff.numel() * fs["measured"].double().abs().view_as(x)), adj.abs())
+                if not tang:   # parameter gradients
+                    Gw = self.Pm("G", op.w)
+                    ref = self._gemm_wgrad(op, a, Gw.shape, dout)
+                    mag = self._gemm_wgrad(op, a.abs(), Gw.shape, dout.abs())
+                    self._cmp(i, "B", f"G[{op.w}] (weight gradient)", Gw, ref,
+                              ((self._K(op, "wgrad") + 2) * U2 + self._truncation(i, op, a)) * mag)
+                    if op.b >= 0:
+                        Gb = self.Pm("G", op.b)
+                        P_ = dout.shape[0] * dout.shape[2] * dout.shape[3]
+                        self._cmp(i, "B", f"G[{op.b}] (bias gradient)", Gb, dout.sum(dim=(0, 2, 3)),
+                                  (P_ + 4) * U2 * dout.abs().sum(dim=(0, 2, 3)))
+            elif op.kind == C.OP_BNACT:
+                y = self.T("val", op.tout)
+                mask = (y > 0).double() if op.relu else torch.ones_like(y)
+                du = dout * mask
+                if op.res >= 0:
+                    add(op.res, i, du, 0.0, du.abs())
+                if op.has_bn and op.bn_train:
+                    mean, var, inv, xh, c = self._bn_train(op, x)
+                    gam = self.P[op.gamma].view(1, -1, 1, 1)
+                    m = self._m
+                    duB = self.T("delta", op.tout) * mask
+                    if not tang:
+                        ref = gam * inv * (du - m(du) - xh * m(du * xh))
+                        mag = gam.abs() * inv * (du.abs() + m(du.abs()) + xh.abs() * m((du * xh).abs()))
+                        self._bn_param_grads(i, op, du, xh, xh.abs())
+                    else:
+                        xd = self.T("tangent", op.tin) if op.tin not in self.src.unwritten else self._tf_override[op.tin]
+                        xhd = inv * (xd - m(xd) - xh * m(xh * xd))
+                        vg = self.Pm("v_operand", op.gamma).view(1, -1, 1, 1)
+                        invd = -inv * inv * m(xh * xd)
+                        w = duB - m(duB) - xh * m(duB * xh)
+                        wd = du - m(du) - xhd * m(duB * xh) - xh * m(du * xh + duB * xhd)
+                        ref = (vg * inv + gam * invd) * w + gam * inv * wd
+                        A = lambda t: t.abs()  # noqa: E731
+                        wm = A(duB) + m(A(duB)) + A(xh) * m(A(duB * xh))
+                        xhdm = inv * (A(xd) + m(A(xd)) + A(xh) * m(A(xh * xd)))
+                        wdm = A(du) + m(A(du)) + xhdm * m(A(duB * xh)) + A(xh) * m(A(du * xh) + A(duB) * xhdm)
+                        mag = (A(vg) * inv + A(gam) * inv * inv * m(A(xh * xd))) * wm + A(gam) * inv * wdm
+                    add(op.tin, i, ref, c * mag, mag)
+                elif op.has_bn:
+                    rm, inv, gam, bet = self._bn_eval(i, op)
+                    xh = (x - rm) * inv
+                    xhm = (x * inv).abs() + (rm * inv).abs()
+                    ref, mag = gam * inv * du, (gam * inv * du).abs()
+                    if tang:
+                        vg = self.Pm("v_operand", op.gamma).view(1, -1, 1, 1)
+                        duB = self.T("delta", op.tout) * mask
+                        ref, mag = ref + vg * inv * duB, mag + (vg * inv * duB).abs()
+                    else:
+                        self._bn_param_grads(i, op, du, xh, xhm)
+                    add(op.tin, i, ref, 8 * U * mag, mag)
+                    if tang and self.obj["di"] is not None:
+                        adj, bnd = self._di_adjoint(i, op, x)
+                        add(op.tin, i, adj, bnd, adj.abs())
+                else:
+                    add(op.tin, i, du, 0.0, du.abs())
+            elif op.kind == C.OP_MAXPOOL:
+                _, idx = F.max_pool2d(x, op.R, op.stride, op.pad, return_indices=True)
+                N_, Cc, H, W_ = x.shape
+                ref = torch.zeros(N_, Cc, H * W_, dtype=torch.float64).scatter_add_(2, idx.flatten(2), dout.flatten(2)).view_as(x)
+                mag = torch.zeros(N_, Cc, H * W_, dtype=torch.float64).scatter_add_(2, idx.flatten(2), dout.abs().flatten(2)).view_as(x)
+                add(op.tin, i, ref, op.R * op.R * U * mag, mag)
+            elif op.kind == C.OP_AVGPOOL:
+                hw = x.shape[2] * x.shape[3]
+                ref = (dout / hw).expand_as(x)
+                add(op.tin, i, ref, 2 * U * ref.abs(), ref.abs())
+        return contrib
+
+    def _bn_param_grads(self, i, op, du, xh, xhm):
+        Pch = du.shape[0] * du.shape[2] * du.shape[3]
+        s = (du.abs() * xhm).sum(dim=(0, 2, 3))
+        bound = (Pch + 4) * U2 * s
+        if op.bn_train:   # xh itself comes from the fp32 batch statistics
+            bound = bound + self._bn_train(op, self.T("val", op.tin))[4].view(-1) * s
+        self._cmp(i, "B", f"G[{op.gamma}] (BN gamma gradient)", self.Pm("G", op.gamma), (du * xh).sum(dim=(0, 2, 3)), bound)
+        self._cmp(i, "B", f"G[{op.beta}] (BN beta gradient)", self.Pm("G", op.beta), du.sum(dim=(0, 2, 3)),
+                  (Pch + 4) * U2 * du.abs().sum(dim=(0, 2, 3)))
+
+    def _di_adjoint(self, i, op, z):
+        """DeepInversion adjoint at the input of BN op i (program_interp.deep_inversion, engine statistics of ``z``)."""
+        di = self.obj["di"]
+        first = min(j for j, o in enumerate(self.prog.ops) if o.kind == C.OP_BNACT and o.has_bn)
+        mult = di["scale"] * (di.get("first_bn_multiplier", 10.0) if i == first else 1.0)
+        rm, rv = self.bn[i]
+        M = z.shape[0] * z.shape[2] * z.shape[3]
+        mean = z.mean(dim=(0, 2, 3))
+        var = z.var(dim=(0, 2, 3), unbiased=False)
+        nv, nm = torch.norm(rv - var, 2), torch.norm(rm - mean, 2)
+        cm = (mean - rm) / nm / M
+        cv = (var - rv) / nv * 2.0 / M
+        v = lambda t: t.view(1, -1, 1, 1)  # noqa: E731
+        adj = mult * (v(cm) + v(cv) * (z - v(mean)))
+        # fp32 batch statistics (P = M terms) and the norms of their differences to the running statistics
+        kap_m = 1.0 + (mean.abs().norm() + rm.norm()) / nm
+        kap_v = 1.0 + ((z * z).mean(dim=(0, 2, 3)).norm() + rv.norm()) / nv
+        mag = abs(mult) * (v(cm.abs()) * kap_m + v(cv.abs()) * kap_v * ((z - v(mean)).abs() + v(mean.abs()) + z.abs()))
+        return adj, TRAIN_C * (M + 8) * U * mag
+
+    def _check_deltas(self, sweep, contrib):
+        dn = "tangent_delta" if sweep == "TB" else "delta"
+        for tid, parts in contrib.items():
+            if tid == 0:
+                continue
+            y = self.T(dn, tid)
+            ref = sum(p[1] for p in parts)
+            mag = sum(p[3] for p in parts)
+            bound = sum(p[2] for p in parts) + len(parts) * U * mag
+            if on_grid(y):
+                bound = bound + len(parts) * TF32_HALF * mag
+            self._cmp(self.first_consumer[tid], sweep, f"{dn}[t{tid}] (sum over {len(parts)} consumer(s))", y, ref, bound)
+        return contrib
+
+    def backward(self):
+        contrib = self._check_deltas("B", self._reverse("B"))
+        if self.obj["task_regularization"] != 0 and 0 in contrib:
+            parts = contrib[0]
+            ref, mag = sum(p[1] for p in parts), sum(p[3] for p in parts)
+            self._cmp(self.first_consumer[0], "B", "delta[t0] (task-loss gradient)", self.T("delta", 0), ref,
+                      sum(p[2] for p in parts) + U * mag)
+
+    def direction(self):
+        o = self.obj
+        n = len(self.P)
+        G = [self.Pm("G", j) for j in range(n)]
+        kw = {k: o[k] for k in ("tag_scale", "scale_scheme") if k in o}
+        _, v = objective_direction(o["kind"], G, self.g, scale=o["scale"], **kw)
+        s = abs(o["scale"])
+        if o["kind"] in ("cosine-similarity", "angular", "fast-cosine-similarity", "masked-cosine-similarity"):
+            nG = sum(a.pow(2).sum() for a in G).sqrt()
+            ng = sum(b.pow(2).sum() for b in self.g).sqrt()
+            al, be = 1.0 / (nG * ng), abs(sum((a * b).sum() for a, b in zip(G, self.g))) / (nG.pow(3) * ng)
+            if o["kind"] == "angular":   # chain factor d acos(c) / dc
+                c = float(sum((a * b).sum() for a, b in zip(G, self.g)) / (nG * ng))
+                al, be = al / (torch.pi * max(1.0 - c * c, 1e-14) ** 0.5), be / (torch.pi * max(1.0 - c * c, 1e-14) ** 0.5)
+            mags = [s * (al * b.abs() + be * a.abs()) for a, b in zip(G, self.g)]
+        elif o["kind"] == "l1":    # 0.5 s sign(G - g): exact in fp32
+            mags = [0.5 * s * torch.ones_like(a) for a in G]
+        else:
+            # euclidean s (G - g) and tag-euclidean s ((G - g) + tag_scale / 2 w_l sign(G - g)): one rounded difference, one product
+            # (and one fma), each relative to the magnitudes of its terms
+            L = len(G)
+            w = [0.0] * L
+            if o["kind"] == "tag-euclidean":
+                scheme = o.get("scale_scheme", "linear")
+                if scheme == "linear":
+                    w = (torch.arange(L, 0, -1, dtype=torch.float64) / L).tolist()
+                elif scheme == "exp":
+                    e = torch.arange(L, 0, -1, dtype=torch.float64).softmax(dim=0)
+                    w = (e / e[0]).tolist()
+                else:
+                    w = [1.0] * L
+                w = [0.5 * o.get("tag_scale", 0.1) * wl for wl in w]
+            mags = [s * ((a - b).abs() + wl) for a, b, wl in zip(G, self.g, w)]
+        for j in range(n):
+            y = self.Pm("v_operand", j)
+            bound = 16 * U * mags[j] + (TF32_HALF * v[j].abs() if on_grid(y) else 0.0)
+            self._cmp(-1, "V", f"v[{j}] (direction, operand form)", y, v[j], bound)
+
+    def tangent_forward(self):
+        self._tf_override = {}
+        prog = self.prog
+        for i, op in enumerate(prog.ops):
+            x = self.T("val", op.tin)
+            tin, tin_bound = None, 0.0
+            if op.tin != 0:
+                if op.tin in self.src.unwritten:
+                    tin, tin_bound = self._tf_override[op.tin]
+                else:
+                    tin = self.T("tangent", op.tin)
+            if op.kind in (C.OP_CONV, C.OP_LINEAR):
+                a, W, V = self._operands(i, op)
+                ref, mag = self._gemm_fwd(op, a, V), self._gemm_fwd(op, a.abs(), V.abs())
+                K = self._K(op, "fprop")
+                if tin is not None:
+                    ref = ref + self._gemm_fwd(op, tin, W)
+                    mag = mag + self._gemm_fwd(op, tin.abs(), W.abs())
+                    K = 2 * K
+                if op.b >= 0:
+                    vb = self.Pm("v_operand", op.b).view(1, -1, 1, 1)
+                    ref, mag = ref + vb, mag + vb.abs()
+                bound = ((K + 2) * U2 + self._truncation(i, op, a)) * mag
+                if op.tout in self.src.unwritten:
+                    self._tf_override[op.tout] = (ref, bound)
+                    continue
+                y = self.T("tangent", op.tout)
+                self._cmp(i, "TF", f"tangent[t{op.tout}]", y, ref, bound + self._rounded(y, ref))
+                continue
+            y = self.T("tangent", op.tout)
+            if op.kind == C.OP_BNACT:
+                u = tin if tin is not None else torch.zeros_like(x)
+                mag, extra = u.abs(), tin_bound
+                if op.has_bn and op.bn_train:
+                    mean, var, inv, xh, c = self._bn_train(op, x)
+                    m = self._m
+                    gam = self.P[op.gamma].view(1, -1, 1, 1)
+                    vg, vb = (self.Pm("v_operand", k).view(1, -1, 1, 1) for k in (op.gamma, op.beta))
+                    xhd = inv * (u - m(u) - xh * m(xh * u))
+                    u = vg * xh + gam * xhd + vb
+                    mag = c / U * (vg.abs() * xh.abs() + gam.abs() * inv * (mag + m(mag) + xh.abs() * m((xh * mag).abs()))) + vb.abs()
+                    extra = gam.abs() * inv * 3 * (tin_bound if torch.is_tensor(tin_bound) else torch.tensor(tin_bound)).amax() \
+                        if tin is not None else 0.0
+                elif op.has_bn:
+                    rm, inv, gam, bet = self._bn_eval(i, op)
+                    vg, vb = (self.Pm("v_operand", k).view(1, -1, 1, 1) for k in (op.gamma, op.beta))
+                    xh = (x - rm) * inv
+                    u = gam * inv * u + vg * xh + vb
+                    mag = (gam * inv).abs() * mag + vg.abs() * ((x * inv).abs() + (rm * inv).abs()) + vb.abs()
+                    extra = (gam * inv).abs() * tin_bound
+                if op.res >= 0:
+                    r = self.T("tangent", op.res)
+                    u, mag = u + r, mag + r.abs()
+                if op.relu:
+                    mask = (self.T("val", op.tout) > 0).double()
+                    u, mag, extra = u * mask, mag * mask, extra * mask
+                self._cmp(i, "TF", f"tangent[t{op.tout}]", y, u, 8 * U * mag + extra + self._rounded(y, u))
+            elif op.kind == C.OP_MAXPOOL:
+                _, idx = F.max_pool2d(x, op.R, op.stride, op.pad, return_indices=True)
+                ref = tin.flatten(2).gather(2, idx.flatten(2)).view_as(idx)
+                self._cmp(i, "TF", f"tangent[t{op.tout}]", y, ref, 0.0)
+            elif op.kind == C.OP_AVGPOOL:
+                hw = tin.shape[2] * tin.shape[3]
+                self._cmp(i, "TF", f"tangent[t{op.tout}]", y, tin.mean(dim=(2, 3), keepdim=True),
+                          (hw + 2) * U2 * tin.abs().mean(dim=(2, 3), keepdim=True))
+
+    def tangent_backward(self):
+        prog = self.prog
+        # seed: tangent of the cross-entropy delta
+        z = self.T("val", prog.logits).flatten(1)
+        zd = self.T("tangent", prog.logits).flatten(1)
+        n = z.shape[0]
+        p = torch.softmax(z, dim=1)
+        ref = (p * zd - p * (p * zd).sum(dim=1, keepdim=True)) / n
+        rng = (z - z.max(dim=1, keepdim=True).values).abs()
+        mag = (p * zd.abs() + p * (p * zd.abs()).sum(dim=1, keepdim=True)) / n
+        y = self.T("tangent_delta", prog.logits).flatten(1)
+        self._cmp(len(prog.ops) - 1, "TB", f"tangent_delta[t{prog.logits}] (cross-entropy seed)", y, ref, (16 + 2 * rng) * U * mag)
+        contrib = self._check_deltas("TB", self._reverse("TB"))
+        # the candidate gradient: first op's contribution + image priors + task term
+        parts = contrib.get(0, [])
+        x = self.T("val", 0)
+        ref = sum(p_[1] for p_ in parts)
+        mag = sum(p_[3] for p_ in parts)
+        bound = sum(p_[2] for p_ in parts) + 2 * U * mag
+        o = self.obj
+        xd = x.clone().requires_grad_(True)
+        prior = torch.zeros((), dtype=torch.float64)
+        if o["tv"] is not None:
+            tv = o["tv"]
+            prior = prior + restate.total_variation(xd, scale=tv["scale"], inner_exp=tv.get("inner_exp", 1), outer_exp=tv.get("outer_exp", 1),
+                                                    double_opponents=tv.get("double_opponents", False), eps=tv.get("eps", 1e-8))
+        if o["norm"] is not None:
+            prior = prior + restate.norm_regularization(xd, scale=o["norm"]["scale"], pnorm=o["norm"].get("p", 2.0))
+        if prior.requires_grad:
+            (gp,) = torch.autograd.grad(prior, xd)
+            ref = ref + gp
+            tvs = o["tv"]["scale"] if o["tv"] is not None else 0.0
+            bound = bound + 64 * U * (gp.abs() + 4 * tvs / x.numel())
+        if o["task_regularization"] != 0:
+            dt = self.T("delta", 0)
+            ref = ref + o["task_regularization"] * dt
+            bound = bound + 2 * U * abs(o["task_regularization"]) * dt.abs()
+        self._cmp(self.first_consumer[0], "TB", "tangent_delta[t0] (candidate gradient)", self.T("tangent_delta", 0), ref, bound)
+
+
+class InterpreterSource:
+    """Buffers of a float64 ``ProgramInterpreter.matching_gradient`` run; ``grad_x``: the full candidate gradient (priors and
+    task term included, as the engine stores it in ``tangent_delta[0]``)."""
+
+    def __init__(self, it, grad_x):
+        self.it, self.V, self.grad_x = it, it.V, grad_x
+        self.unwritten = set()
+
+    def rounds_operands(self, i):
+        return False
+
+    def tensor(self, which, tid):
+        it = self.it
+        if which == "val":
+            return it.a[tid]
+        if which == "delta":
+            return it.d_B.get(tid)
+        if which == "tangent":
+            return it.ta.get(tid)
+        if tid == 0:
+            return self.grad_x
+        return it.d_T[tid] + it.inject.get(tid, 0)   # the engine adds the prior adjoints into the stored tangent delta
+
+    def param(self, which, idx):
+        return {"G": self.it.G, "v_operand": self.V, "W_operand": self.it.P}[which][idx]

@@ -118,3 +118,74 @@ def multi_query_oracle_for_fixture(fx):
         m.eval()
         oracles.append(restate.TrialOracle(m, loss_fn, cfg if i == 0 else no_priors, sh["gradients"], labels, dm, ds))
     return restate.MultiQueryOracle(oracles), cfg, labels
+
+
+class OddNet(torch.nn.Module):
+    """A network that reaches the scalar (non-float4) element-wise and pooling kernels and the accumulation paths of the BN / ReLU /
+    residual kernels.  A 6-channel branch (C % 4 != 0: scalar kernels) with a conv without bias, BN without ReLU, ReLU without
+    BN and residual adds without BN; maxpool 3/2/1 on odd sizes; a 10-channel conv + BN + ReLU; an 8-channel branch (float4
+    kernels) with the same shapes of reuse; a linear head on a spatial map.  In both branches a BN / ReLU / add op reads a tensor
+    that a later op also reads (``acc_in``) and takes as residual a tensor that a later op also reads (``acc_res``).  Meant for
+    15 x 13 inputs."""
+
+    def __init__(self, classes=5):
+        super().__init__()
+        self.conv1 = torch.nn.Conv2d(3, 6, 3, padding=1)
+        self.bn1 = torch.nn.BatchNorm2d(6)
+        self.conv2 = torch.nn.Conv2d(6, 6, 3, padding=1, bias=False)
+        self.relu = torch.nn.ReLU()
+        self.pool = torch.nn.MaxPool2d(3, 2, 1)
+        self.conv3 = torch.nn.Conv2d(6, 10, 3, padding=1, bias=False)
+        self.bn3 = torch.nn.BatchNorm2d(10)
+        self.conv5 = torch.nn.Conv2d(10, 8, 3, padding=1)
+        self.bn5 = torch.nn.BatchNorm2d(8)
+        self.conv6 = torch.nn.Conv2d(8, 8, 3, padding=1, bias=False)
+        self.conv7 = torch.nn.Conv2d(8, 8, 1)
+        self.fc = torch.nn.Linear(8 * 8 * 7, classes)
+
+    def forward(self, x):
+        a = self.bn1(self.conv1(x))          # BN without ReLU
+        r = self.relu(a)                     # ReLU without BN; conv2 reads `a` later -> acc_in
+        b = self.relu(self.conv2(a))
+        s = r + b                            # residual add without BN; the next add reads `b` later -> acc_res
+        c = self.pool(s + b)
+        d = self.relu(self.bn3(self.conv3(c)))
+        e = self.bn5(self.conv5(d))
+        g = self.relu(e)                     # 8 channels: conv6 reads `e` later -> acc_in (float4)
+        h = self.conv6(e)
+        k = g + h                            # conv7 reads `h` later -> acc_res (float4)
+        u = self.conv7(h) + k
+        return self.fc(torch.flatten(u, 1))
+
+
+def odd_case(seed=5, batch=3):
+    """(model in eval mode with random BN, input shape, labels, target gradients) for :class:`OddNet`."""
+    torch.manual_seed(seed)
+    model = synthetic.randomize_bn(OddNet(), seed + 1).eval()
+    gen = torch.Generator().manual_seed(seed + 7)
+    x = torch.randn(batch, 3, 15, 13, generator=gen)
+    y = torch.randint(0, 5, (batch,), generator=gen)
+    grads = torch.autograd.grad(torch.nn.functional.cross_entropy(model(x), y), list(model.parameters()))
+    return model, (batch, 3, 15, 13), y, [g.detach() for g in grads]
+
+
+def sweep_objective(cfg, features=None):
+    """The objective dict of ``oracle.sweep_check.SweepChecker`` for an attack config."""
+    reg = cfg.get("regularization") or {}
+
+    def on(key):
+        return key in reg and reg[key]["scale"] > 0
+
+    obj = dict(kind=cfg.objective.type, scale=float(cfg.objective.get("scale", 1.0)),
+               task_regularization=float(cfg.objective.get("task_regularization", 0.0) or 0.0))
+    if on("total_variation"):
+        r = reg["total_variation"]
+        obj["tv"] = dict(scale=r["scale"], inner_exp=r.get("inner_exp", 1), outer_exp=r.get("outer_exp", 1), eps=r.get("eps", 1e-8),
+                         double_opponents=bool(r.get("double_opponents", False)))
+    if on("norm"):
+        obj["norm"] = dict(scale=reg["norm"]["scale"], p=reg["norm"].get("pnorm", 2.0))
+    if on("deep_inversion"):
+        obj["di"] = dict(scale=reg["deep_inversion"]["scale"], first_bn_multiplier=reg["deep_inversion"].get("first_bn_multiplier", 10))
+    if on("features") and features is not None:
+        obj["features"] = dict(scale=reg["features"]["scale"], measured=features)
+    return obj
