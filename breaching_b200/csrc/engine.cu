@@ -495,15 +495,15 @@ struct bre_engine {
           break;
         }
         case BRE_OP_POSADD:
-          BRE_LAUNCH(launch_token_posadd(t[op.tin].val, Wp(op.w), t[op.tout].val, to.N, to.C, op.S, stream));
+          BRE_LAUNCH(launch_token_posadd(t[op.tin].val, Wp(op.w), t[op.tout].val, to.N, to.C, op.S, round_val(op.tout), stream));
           break;
         case BRE_OP_LAYERNORM:
           BRE_LAUNCH(launch_token_layernorm(0, t[op.tin].val, nullptr, nullptr, nullptr, Wp(op.gamma), Wp(op.beta), nullptr, nullptr, op.eps,
-                                            to.N, to.C, tok_a[i], t[op.tout].val, 0, stream));
+                                            to.N, to.C, tok_a[i], t[op.tout].val, 0, round_val(op.tout), stream));
           break;
         case BRE_OP_ATTENTION:
           BRE_LAUNCH(launch_token_attention(0, t[op.tin].val, nullptr, nullptr, nullptr, to.N / op.S, op.S, op.R, to.C / op.R, tok_a[i], tok_b[i],
-                                            t[op.tout].val, 0, stream));
+                                            t[op.tout].val, 0, round_val(op.tout), stream));
           break;
         default: set_error("unknown op kind"); return BRE_ERR_INVALID;
       }
@@ -511,7 +511,7 @@ struct bre_engine {
     const bre_tensor_desc& lt = td(logits);
     if (seq_len > 0) {   // next-token loss over rows with class-probability targets (joint attacker on a causal language model)
       if (soft_q == nullptr) { set_error("token programs need soft labels (bre_engine_load_soft_labels)"); return BRE_ERR_STATE; }
-      BRE_LAUNCH(launch_token_ce_fwd(t[logits].val, soft_q, lt.N, classes(), lt.C, seq_len, p, loss_n, t[logits].d, stream));
+      BRE_LAUNCH(launch_token_ce_fwd(t[logits].val, soft_q, lt.N, classes(), lt.C, seq_len, p, loss_n, t[logits].d, round_d(logits), stream));
       BRE_LAUNCH(launch_loss_mean(loss_n, lt.N, sc, stream));
       return 0;
     }
@@ -591,17 +591,19 @@ struct bre_engine {
           BRE_LAUNCH(launch_avgpool_bwd(t[op.tout].d, t[op.tin].d, op.acc_in != 0, ti.N, ti.H * ti.W, ti.C, stream));
           break;
         }
-        case BRE_OP_POSADD:      // gradient of the positional table (the candidate's own first-backward delta is not needed)
+        case BRE_OP_POSADD:      // gradient of the positional table; the candidate's own delta only for the task-loss term
           BRE_LAUNCH(launch_token_pos_grad(t[op.tout].d, Gp(op.w), to.N, to.C, op.S, stream));
+          if (need_task_grad())
+            BRE_CUDA_CHECK(cudaMemcpyAsync(t[0].d, t[op.tout].d, (size_t)to.N * to.C * sizeof(float), cudaMemcpyDeviceToDevice, stream));
           break;
         case BRE_OP_LAYERNORM:
           BRE_LAUNCH(launch_token_ln_param_grad(t[op.tin].val, t[op.tout].d, tok_a[i], to.N, to.C, Gp(op.gamma), Gp(op.beta), stream));
           BRE_LAUNCH(launch_token_layernorm(1, t[op.tin].val, t[op.tout].d, nullptr, nullptr, Wp(op.gamma), Wp(op.beta), nullptr, nullptr, op.eps,
-                                            to.N, to.C, tok_a[i], t[op.tin].d, op.acc_in != 0, stream));
+                                            to.N, to.C, tok_a[i], t[op.tin].d, op.acc_in != 0, round_d(op.tin), stream));
           break;
         case BRE_OP_ATTENTION:
           BRE_LAUNCH(launch_token_attention(1, t[op.tin].val, t[op.tout].d, nullptr, nullptr, to.N / op.S, op.S, op.R, to.C / op.R, tok_a[i],
-                                            tok_b[i], t[op.tin].d, op.acc_in != 0, stream));
+                                            tok_b[i], t[op.tin].d, op.acc_in != 0, round_d(op.tin), stream));
           break;
         default: break;
       }
@@ -691,15 +693,15 @@ struct bre_engine {
           break;
         }
         case BRE_OP_POSADD:      // the candidate's tangent is zero: only the direction component of the positional table
-          BRE_LAUNCH(launch_token_posadd(nullptr, Vp(op.w), t[op.tout].tval, to.N, to.C, op.S, stream));
+          BRE_LAUNCH(launch_token_posadd(nullptr, Vp(op.w), t[op.tout].tval, to.N, to.C, op.S, round_val(op.tout), stream));
           break;
         case BRE_OP_LAYERNORM:
           BRE_LAUNCH(launch_token_layernorm(2, t[op.tin].val, t[op.tin].tval, nullptr, nullptr, Wp(op.gamma), Wp(op.beta), Vp(op.gamma),
-                                            Vp(op.beta), op.eps, to.N, to.C, tok_a[i], t[op.tout].tval, 0, stream));
+                                            Vp(op.beta), op.eps, to.N, to.C, tok_a[i], t[op.tout].tval, 0, round_val(op.tout), stream));
           break;
         case BRE_OP_ATTENTION:
           BRE_LAUNCH(launch_token_attention(2, t[op.tin].val, t[op.tin].tval, nullptr, nullptr, to.N / op.S, op.S, op.R, to.C / op.R, tok_a[i],
-                                            tok_b[i], t[op.tout].tval, 0, stream));
+                                            tok_b[i], t[op.tout].tval, 0, round_val(op.tout), stream));
           break;
         default: break;
       }
@@ -768,7 +770,7 @@ struct bre_engine {
   int sweep_tangent_backward() {
     bool forked = false;
     const bre_tensor_desc& lt = td(logits);
-    if (seq_len > 0) BRE_LAUNCH(launch_token_ce_tan_bwd(p, t[logits].tval, lt.N, classes(), lt.C, seq_len, t[logits].td, stream));
+    if (seq_len > 0) BRE_LAUNCH(launch_token_ce_tan_bwd(p, t[logits].tval, lt.N, classes(), lt.C, seq_len, t[logits].td, round_d(logits), stream));
     else BRE_LAUNCH(launch_ce_tan_bwd(p, t[logits].tval, lt.N, lt.C, t[logits].td, stream));
     const bool di = cfg.di_scale > 0.f && n_di > 0;
     for (int i = (int)ops.size() - 1; i >= 0; --i) {
@@ -849,11 +851,11 @@ struct bre_engine {
           break;
         case BRE_OP_LAYERNORM:
           BRE_LAUNCH(launch_token_layernorm(3, t[op.tin].val, t[op.tout].td, t[op.tout].d, t[op.tin].tval, Wp(op.gamma), Wp(op.beta),
-                                            Vp(op.gamma), nullptr, op.eps, to.N, to.C, tok_a[i], t[op.tin].td, op.acc_in != 0, stream));
+                                            Vp(op.gamma), nullptr, op.eps, to.N, to.C, tok_a[i], t[op.tin].td, op.acc_in != 0, round_d(op.tin), stream));
           break;
         case BRE_OP_ATTENTION:
           BRE_LAUNCH(launch_token_attention(3, t[op.tin].val, t[op.tout].td, t[op.tout].d, t[op.tin].tval, to.N / op.S, op.S, op.R, to.C / op.R,
-                                            tok_a[i], tok_b[i], t[op.tin].td, op.acc_in != 0, stream));
+                                            tok_a[i], tok_b[i], t[op.tin].td, op.acc_in != 0, round_d(op.tin), stream));
           break;
         default: break;
       }

@@ -24,10 +24,13 @@ namespace {
 // sweep 3 (TB): dx' = inv u' - u mean(xh x') inv^2                              [in1 = dy', in2 = dy, in3 = x']
 //               t' = dy' gamma + dy v_gamma, u = t - mean(t) - xh mean(t xh),
 //               u' = t' - mean(t') - xh' mean(t xh) - xh mean(t' xh + t xh')
+// kRound: store `out` on the TF32 grid (a template parameter so that the unrounded kernel is the plain one)
+template <bool kRound>
 __global__ void layernorm_kernel(int sweep, const float* __restrict__ x, const float* __restrict__ in1, const float* __restrict__ in2,
                                  const float* __restrict__ in3, const float* __restrict__ gamma, const float* __restrict__ beta,
                                  const float* __restrict__ v_gamma, const float* __restrict__ v_beta, float eps, int rows, int C,
                                  float* __restrict__ stats, float* __restrict__ out, int accumulate) {
+  constexpr bool round_out = kRound;
   pdl_prologue();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -43,7 +46,10 @@ __global__ void layernorm_kernel(int sweep, const float* __restrict__ x, const f
     for (int c = lane; c < C; c += 32) { const float dlt = xr[c] - mean; q = fmaf(dlt, dlt, q); }
     inv = 1.0f / sqrtf(warp_sum(q) * invC + eps);
     if (lane == 0) { stats[2 * row] = mean; stats[2 * row + 1] = inv; }
-    for (int c = lane; c < C; c += 32) out[(long long)row * C + c] = fmaf(gamma[c], (xr[c] - mean) * inv, beta[c]);
+    for (int c = lane; c < C; c += 32) {
+      const float y = fmaf(gamma[c], (xr[c] - mean) * inv, beta[c]);
+      out[(long long)row * C + c] = round_out ? tf32_rna(y) : y;
+    }
     return;
   }
   mean = stats[2 * row];
@@ -60,7 +66,8 @@ __global__ void layernorm_kernel(int sweep, const float* __restrict__ x, const f
     for (int c = lane; c < C; c += 32) {
       const float xh = (xr[c] - mean) * inv;
       const float v = inv * (a1[c] * gamma[c] - m0 - xh * m1);
-      o[c] = accumulate ? o[c] + v : v;
+      const float r = accumulate ? o[c] + v : v;
+      o[c] = round_out ? tf32_rna(r) : r;
     }
   } else if (sweep == 2) {
     float s0 = 0.f, s1 = 0.f;
@@ -69,7 +76,8 @@ __global__ void layernorm_kernel(int sweep, const float* __restrict__ x, const f
     for (int c = lane; c < C; c += 32) {
       const float xh = (xr[c] - mean) * inv;
       const float xhd = inv * (a1[c] - m0 - xh * m1);
-      o[c] = fmaf(v_gamma[c], xh, fmaf(gamma[c], xhd, v_beta[c]));
+      const float yd = fmaf(v_gamma[c], xh, fmaf(gamma[c], xhd, v_beta[c]));
+      o[c] = round_out ? tf32_rna(yd) : yd;
     }
   } else {
     const float* dyB = in2 + (long long)row * C;
@@ -96,7 +104,8 @@ __global__ void layernorm_kernel(int sweep, const float* __restrict__ x, const f
       const float u = t - mt - xh * mtxh;
       const float ud = td - mtd - xhd * mtxh - xh * mmix;
       const float v = inv * ud - u * mxhxd * inv * inv;
-      o[c] = accumulate ? o[c] + v : v;
+      const float r = accumulate ? o[c] + v : v;
+      o[c] = round_out ? tf32_rna(r) : r;
     }
   }
 }
@@ -141,10 +150,13 @@ __global__ void __launch_bounds__(256) layernorm_param_grad_kernel(const float* 
 //   sweep 2 (TF): O' from (qkv)' (= in1 [rows, 3 d])        writes out [rows, d], P'
 //   sweep 3 (TB): d(qkv)' from dO' (= in1), dO (= in2), (qkv)' (= in3), P, P'     writes out [rows, 3 d]
 constexpr int ATT_THREADS = 256;
+constexpr size_t kAttSmemLimit = 200 * 1024;   // dynamic shared memory the attention kernel opts in to
+template <bool kRound>
 __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(int sweep, const float* __restrict__ qkv, const float* __restrict__ in1,
                                                               const float* __restrict__ in2, const float* __restrict__ in3, int T, int heads,
                                                               int dh, float* __restrict__ P, float* __restrict__ Pd, float* __restrict__ out,
                                                               int accumulate) {
+  constexpr bool round_out = kRound;
   pdl_prologue();
   extern __shared__ float sm[];
   const int b = blockIdx.x / heads, h = blockIdx.x % heads;
@@ -186,9 +198,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(int sweep, const
   auto store_qkv_grad = [&](int i, int c, float dq, float dk, float dv) {
     float* o = out + (row0 + i) * 3 * d + h * dh + c;
     const float vq = dq * scale, vk = dk * scale;
-    o[0] = accumulate ? o[0] + vq : vq;
-    o[d] = accumulate ? o[d] + vk : vk;
-    o[2 * d] = accumulate ? o[2 * d] + dv : dv;
+    const float rq = accumulate ? o[0] + vq : vq, rk = accumulate ? o[d] + vk : vk, rv = accumulate ? o[2 * d] + dv : dv;
+    o[0] = round_out ? tf32_rna(rq) : rq;
+    o[d] = round_out ? tf32_rna(rk) : rk;
+    o[2 * d] = round_out ? tf32_rna(rv) : rv;
   };
   load_qkv(qkv, sQ, sK, sV);
   if (sweep == 0) {
@@ -208,7 +221,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(int sweep, const
       const int i = e / dh, c = e - i * dh;
       float o = 0.f;
       for (int j = 0; j < T; ++j) o = fmaf(sP[i * T + j], sV[j * dh + c], o);
-      out[(row0 + i) * d + h * dh + c] = o;
+      out[(row0 + i) * d + h * dh + c] = round_out ? tf32_rna(o) : o;
     }
     return;
   }
@@ -253,7 +266,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(int sweep, const
       const int i = e / dh, c = e - i * dh;
       float o = 0.f;
       for (int j = 0; j < T; ++j) o += sM[i * T + j] * sV[j * dh + c] + sP[i * T + j] * sC[j * dh + c];
-      out[(row0 + i) * d + h * dh + c] = o;
+      out[(row0 + i) * d + h * dh + c] = round_out ? tf32_rna(o) : o;
     }
     return;
   }
@@ -297,13 +310,16 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(int sweep, const
 }
 
 // ---- positional embedding ------------------------------------------------------------------------------------------
+template <bool kRound>
 __global__ void posadd_kernel(const float* __restrict__ x, const float* __restrict__ pos, float* __restrict__ out, long long total, int C, int T) {
+  constexpr bool round_out = kRound;
   pdl_prologue();
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long row = i / C;
     const int c = (int)(i - row * C);
     const float v = pos[(row % T) * C + c];
-    out[i] = x != nullptr ? x[i] + v : v;
+    const float y = x != nullptr ? x[i] + v : v;
+    out[i] = round_out ? tf32_rna(y) : y;
   }
 }
 
@@ -353,8 +369,10 @@ __device__ __forceinline__ void cluster_softmax_stats(const float* z, int c0, in
   mx_out = mx;
 }
 
+template <bool kRound>
 __global__ void __launch_bounds__(kRowThreads, 2) token_ce_fwd_kernel(const float* __restrict__ logits, const float* __restrict__ q, int rows, int V,
                                                                   int Vs, int T, float* p, float* loss_n, float* dlogits) {
+  constexpr bool round_out = kRound;
   pdl_prologue();
   __shared__ RowReduce ws;
   const int row = blockIdx.x;
@@ -381,7 +399,8 @@ __global__ void __launch_bounds__(kRowThreads, 2) token_ce_fwd_kernel(const floa
       const float pc = expf(zc.v[k] - m) / fsum;
       p[(long long)row * Vs + c] = pc;
       if (scored) {
-        dlogits[(long long)row * Vs + c] = (pc - qc.v[k]) * invM;
+        const float g = (pc - qc.v[k]) * invM;
+        dlogits[(long long)row * Vs + c] = round_out ? tf32_rna(g) : g;
         lp -= (double)qc.v[k] * (double)(zc.v[k] - lse_c);
       } else {
         dlogits[(long long)row * Vs + c] = 0.f;
@@ -401,7 +420,8 @@ __global__ void __launch_bounds__(kRowThreads, 2) token_ce_fwd_kernel(const floa
     p[(long long)row * Vs + c] = pc;
     if (scored) {
       const float qc = qn[c];
-      dlogits[(long long)row * Vs + c] = (pc - qc) * invM;
+      const float g = (pc - qc) * invM;
+      dlogits[(long long)row * Vs + c] = round_out ? tf32_rna(g) : g;
       lpart -= (double)qc * (double)(z[c] - lse);
     } else {
       dlogits[(long long)row * Vs + c] = 0.f;
@@ -412,8 +432,10 @@ __global__ void __launch_bounds__(kRowThreads, 2) token_ce_fwd_kernel(const floa
   cluster_exit();
 }
 
+template <bool kRound>
 __global__ void __launch_bounds__(kRowThreads, 2) token_ce_tan_bwd_kernel(const float* __restrict__ p, const float* __restrict__ zdot, int rows, int V,
                                                                       int Vs, int T, float* tdl) {
+  constexpr bool round_out = kRound;
   pdl_prologue();
   __shared__ RowReduce ws;
   const int row = blockIdx.x;
@@ -434,7 +456,9 @@ __global__ void __launch_bounds__(kRowThreads, 2) token_ce_tan_bwd_kernel(const 
 #pragma unroll
     for (int k = 0; k < kSegCache; ++k) {
       const int c = c0 + k * kRowThreads + (int)threadIdx.x;
-      if (c < c1) tdl[(long long)row * Vs + c] = scored ? pc.v[k] * (zc.v[k] - dt) * invM : 0.f;
+      if (c >= c1) continue;
+      const float g = scored ? pc.v[k] * (zc.v[k] - dt) * invM : 0.f;
+      tdl[(long long)row * Vs + c] = round_out ? tf32_rna(g) : g;
     }
     cluster_exit();
     return;
@@ -442,7 +466,10 @@ __global__ void __launch_bounds__(kRowThreads, 2) token_ce_tan_bwd_kernel(const 
   double part = 0.0;
   for (int c = c0 + threadIdx.x; c < c1; c += kRowThreads) part += (double)pp[c] * (double)zz[c];
   const float dot = (float)row_allreduce<ROW_SUM>(part, ws, 0);
-  for (int c = c0 + threadIdx.x; c < c1; c += kRowThreads) tdl[(long long)row * Vs + c] = scored ? pp[c] * (zz[c] - dot) * invM : 0.f;
+  for (int c = c0 + threadIdx.x; c < c1; c += kRowThreads) {
+    const float g = scored ? pp[c] * (zz[c] - dot) * invM : 0.f;
+    tdl[(long long)row * Vs + c] = round_out ? tf32_rna(g) : g;
+  }
   cluster_exit();
 }
 
@@ -512,10 +539,10 @@ static int check_launch(const char* what) {
 
 int launch_token_layernorm(int sweep, const float* x, const float* in1, const float* in2, const float* in3, const float* gamma,
                            const float* beta, const float* v_gamma, const float* v_beta, float eps, int rows, int C, float* stats, float* out,
-                           int accumulate, cudaStream_t s) {
+                           int accumulate, bool round_out, cudaStream_t s) {
   const int warps = 4;
-  const cudaError_t lerr = launch_kernel(layernorm_kernel, dim3((rows + warps - 1) / warps), dim3(warps * 32), 0, s, 1, sweep, x, in1, in2, in3, gamma, beta,
-                                         v_gamma, v_beta, eps, rows, C, stats, out, accumulate);
+  const cudaError_t lerr = launch_kernel(round_out ? layernorm_kernel<true> : layernorm_kernel<false>, dim3((rows + warps - 1) / warps), dim3(warps * 32), 0, s,
+                                         1, sweep, x, in1, in2, in3, gamma, beta, v_gamma, v_beta, eps, rows, C, stats, out, accumulate);
   if (lerr != cudaSuccess) { set_error(std::string("token layernorm: ") + cudaGetErrorString(lerr)); return -2; }
   return check_launch("token layernorm");
 }
@@ -526,26 +553,32 @@ int launch_token_ln_param_grad(const float* x, const float* dy, const float* sta
   return check_launch("token layernorm parameter gradient");
 }
 int launch_token_attention(int sweep, const float* qkv, const float* in1, const float* in2, const float* in3, int B, int T, int heads, int dh,
-                           float* P, float* Pd, float* out, int accumulate, cudaStream_t s) {
-  if (T > 128) { set_error("token attention: seq_len > 128 needs the tiled kernel (not written yet)"); return -4; }
-  const size_t smem = (size_t)(8 * T * dh + 4 * T * T) * sizeof(float);
-  if (smem > 200 * 1024) { set_error("token attention: head too large for the resident-head kernel"); return -4; }
+                           float* P, float* Pd, float* out, int accumulate, bool round_out, cudaStream_t s) {
+  // the whole head stays resident in shared memory (8 T dh + 4 T^2 floats) under the 200 KB opt-in; longer sequences need a tiled kernel
+  const size_t smem = (size_t)(8LL * T * dh + 4LL * T * T) * sizeof(float);
+  if (smem > kAttSmemLimit) {
+    set_error("token attention: seq_len " + std::to_string(T) + " with head size " + std::to_string(dh) + " needs " + std::to_string(smem) +
+              " B of shared memory, over the " + std::to_string(kAttSmemLimit) + " B opt-in limit of the resident-head kernel");
+    return -4;
+  }
   static bool attr_done = false;
   if (!attr_done) {
-    if (cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) {
+    if (cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmemLimit) != cudaSuccess ||
+        cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmemLimit) != cudaSuccess) {
       set_error("token attention: shared memory opt-in failed");
       return -2;
     }
     attr_done = true;
   }
-  const cudaError_t lerr = launch_kernel(attention_kernel, dim3(B * heads), dim3(ATT_THREADS), smem, s, 1, sweep, qkv, in1, in2, in3, T, heads, dh, P, Pd, out,
-                                         accumulate);
+  const cudaError_t lerr = launch_kernel(round_out ? attention_kernel<true> : attention_kernel<false>, dim3(B * heads), dim3(ATT_THREADS), smem, s, 1, sweep,
+                                         qkv, in1, in2, in3, T, heads, dh, P, Pd, out, accumulate);
   if (lerr != cudaSuccess) { set_error(std::string("token attention: ") + cudaGetErrorString(lerr)); return -2; }
   return check_launch("token attention");
 }
-int launch_token_posadd(const float* x, const float* pos, float* out, int rows, int C, int T, cudaStream_t s) {
+int launch_token_posadd(const float* x, const float* pos, float* out, int rows, int C, int T, bool round_out, cudaStream_t s) {
   const long long total = (long long)rows * C;
-  const cudaError_t lerr = launch_kernel(posadd_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, s, 1, x, pos, out, total, C, T);
+  const cudaError_t lerr = launch_kernel(round_out ? posadd_kernel<true> : posadd_kernel<false>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, s, 1, x,
+                                         pos, out, total, C, T);
   if (lerr != cudaSuccess) { set_error(std::string("token posadd: ") + cudaGetErrorString(lerr)); return -2; }
   return check_launch("token posadd");
 }
@@ -554,12 +587,15 @@ int launch_token_pos_grad(const float* d, float* g_pos, int rows, int C, int T, 
   if (lerr != cudaSuccess) { set_error(std::string("token positional gradient: ") + cudaGetErrorString(lerr)); return -2; }
   return check_launch("token positional gradient");
 }
-int launch_token_ce_fwd(const float* logits, const float* q, int rows, int V, int Vs, int T, float* p, float* loss_n, float* dlogits, cudaStream_t s) {
-  if (launch_row_kernel(token_ce_fwd_kernel, rows, V, s, logits, q, rows, V, Vs, T, p, loss_n, dlogits) != cudaSuccess) { set_error("token cross-entropy: launch failed"); return -2; }
+int launch_token_ce_fwd(const float* logits, const float* q, int rows, int V, int Vs, int T, float* p, float* loss_n, float* dlogits, bool round_out,
+                        cudaStream_t s) {
+  if (launch_row_kernel(round_out ? token_ce_fwd_kernel<true> : token_ce_fwd_kernel<false>, rows, V, s, logits, q, rows, V, Vs, T, p, loss_n, dlogits) !=
+      cudaSuccess) { set_error("token cross-entropy: launch failed"); return -2; }
   return check_launch("token cross-entropy");
 }
-int launch_token_ce_tan_bwd(const float* p, const float* zdot, int rows, int V, int Vs, int T, float* tdlogits, cudaStream_t s) {
-  if (launch_row_kernel(token_ce_tan_bwd_kernel, rows, V, s, p, zdot, rows, V, Vs, T, tdlogits) != cudaSuccess) { set_error("token cross-entropy tangent: launch failed"); return -2; }
+int launch_token_ce_tan_bwd(const float* p, const float* zdot, int rows, int V, int Vs, int T, float* tdlogits, bool round_out, cudaStream_t s) {
+  if (launch_row_kernel(round_out ? token_ce_tan_bwd_kernel<true> : token_ce_tan_bwd_kernel<false>, rows, V, s, p, zdot, rows, V, Vs, T, tdlogits) !=
+      cudaSuccess) { set_error("token cross-entropy tangent: launch failed"); return -2; }
   return check_launch("token cross-entropy tangent");
 }
 int launch_token_label_grad(const float* logits, const float* p, const float* zdot, int rows, int V, int Vs, int T, float task_reg,
@@ -702,24 +738,24 @@ int bre_token_match(const float* rec, const float* emb, const int64_t* subset, i
 // sweep 1 additionally writes the parameter gradients when g_gamma / g_beta are non-null.
 int bre_token_layernorm(int32_t sweep, const float* x, const float* in1, const float* in2, const float* in3, const float* gamma,
                         const float* beta, const float* v_gamma, const float* v_beta, float eps, int32_t rows, int32_t C, float* stats,
-                        float* out, float* g_gamma, float* g_beta, void* stream) {
+                        float* out, float* g_gamma, float* g_beta, int32_t round_out, void* stream) {
   using namespace bre;
   if (!x || !out || !stats || !gamma || rows < 1 || C < 1 || sweep < 0 || sweep > 3) { set_error("bre_token_layernorm: bad arguments"); return -1; }
   cudaStream_t s = (cudaStream_t)stream;
-  int rc = launch_token_layernorm(sweep, x, in1, in2, in3, gamma, beta, v_gamma, v_beta, eps, rows, C, stats, out, 0, s);
+  int rc = launch_token_layernorm(sweep, x, in1, in2, in3, gamma, beta, v_gamma, v_beta, eps, rows, C, stats, out, 0, round_out != 0, s);
   if (rc == 0 && sweep == 1 && g_gamma && g_beta) rc = launch_token_ln_param_grad(x, in1, stats, rows, C, g_gamma, g_beta, s);
   return rc;
 }
 
 // Stand-alone attention sweeps: qkv [B*T, 3 d], P / Pd [B, heads, T, T] scratch kept by the caller between sweeps.
 int bre_token_attention(int32_t sweep, const float* qkv, const float* in1, const float* in2, const float* in3, int32_t B, int32_t T,
-                        int32_t heads, int32_t dh, float* P, float* Pd, float* out, void* stream) {
+                        int32_t heads, int32_t dh, float* P, float* Pd, float* out, int32_t round_out, void* stream) {
   using namespace bre;
-  if (!qkv || !out || !P || B < 1 || T < 1 || T > 128 || heads < 1 || dh < 1 || sweep < 0 || sweep > 3) {
-    set_error("bre_token_attention: bad arguments (T <= 128)");
+  if (!qkv || !out || !P || B < 1 || T < 1 || heads < 1 || dh < 1 || sweep < 0 || sweep > 3) {
+    set_error("bre_token_attention: bad arguments");
     return -1;
   }
-  return launch_token_attention(sweep, qkv, in1, in2, in3, B, T, heads, dh, P, Pd, out, 0, (cudaStream_t)stream);
+  return launch_token_attention(sweep, qkv, in1, in2, in3, B, T, heads, dh, P, Pd, out, 0, round_out != 0, (cudaStream_t)stream);
 }
 
 }  // extern "C"

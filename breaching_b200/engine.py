@@ -132,8 +132,8 @@ def load_library(path=None):
     lib.bre_match_reduce.argtypes = [vp, vp, vp, i64, f32, P(ctypes.c_double), vp]
     lib.bre_total_variation.argtypes = [vp, vp, i32, i32, i32, f32, f32, f32, f32, i32, i32, P(ctypes.c_double), vp]
     lib.bre_conv_gemm.argtypes = [i32, i32, vp, vp, vp, vp, vp] + [i32] * 9 + [vp]
-    lib.bre_token_layernorm.argtypes = [i32, vp, vp, vp, vp, vp, vp, vp, vp, f32, i32, i32, vp, vp, vp, vp, vp]
-    lib.bre_token_attention.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp]
+    lib.bre_token_layernorm.argtypes = [i32, vp, vp, vp, vp, vp, vp, vp, vp, f32, i32, i32, vp, vp, vp, vp, i32, vp]
+    lib.bre_token_attention.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, i32, vp]
     lib.bre_token_match.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp]
     lib.bre_engine_begin_joint_trial.argtypes = [vp, vp, vp, i64, vp, i32]
     lib.bre_engine_get_joint_labels.argtypes = [vp, i32, vp]
@@ -644,9 +644,11 @@ def conv_gemm(mode, a, w, out, N, H, W, Ci, Co, R, S, stride, pad, a2=None, w2=N
     return out
 
 
-def token_layernorm(sweep, x, gamma, beta, stats, in1=None, in2=None, in3=None, v_gamma=None, v_beta=None, eps=1e-5, want_param_grad=False):
+def token_layernorm(sweep, x, gamma, beta, stats, in1=None, in2=None, in3=None, v_gamma=None, v_beta=None, eps=1e-5, want_param_grad=False,
+                    round_out=False):
     """Stand-alone LayerNorm sweep (csrc/tokens.cu) on [rows, C] device tensors; returns ``out`` (and the gamma / beta
-    gradients for sweep 1 with ``want_param_grad``)."""
+    gradients for sweep 1 with ``want_param_grad``).  ``round_out``: store ``out`` on the TF32 grid (as the engine does for
+    tensor-core GEMM operands)."""
     lib = load_library()
     rows, C = x.shape
     out = torch.empty_like(x)
@@ -655,7 +657,7 @@ def token_layernorm(sweep, x, gamma, beta, stats, in1=None, in2=None, in3=None, 
     stream = torch.cuda.current_stream(x.device).cuda_stream
     with torch.cuda.device(x.device):
         rc = lib.bre_token_layernorm(sweep, _ptr(x), _ptr(in1), _ptr(in2), _ptr(in3), _ptr(gamma), _ptr(beta), _ptr(v_gamma), _ptr(v_beta),
-                                     float(eps), rows, C, _ptr(stats), _ptr(out), _ptr(gg), _ptr(gb), ctypes.c_void_p(stream))
+                                     float(eps), rows, C, _ptr(stats), _ptr(out), _ptr(gg), _ptr(gb), int(bool(round_out)), ctypes.c_void_p(stream))
     _check(lib, rc, "bre_token_layernorm")
     return (out, gg, gb) if want_param_grad else out
 
@@ -677,14 +679,15 @@ def token_match(rec, emb, subset=None):
     return out
 
 
-def token_attention(sweep, qkv, B, T, heads, P, Pd, in1=None, in2=None, in3=None):
-    """Stand-alone multi-head self-attention sweep (csrc/tokens.cu); qkv [B*T, 3 d]."""
+def token_attention(sweep, qkv, B, T, heads, P, Pd, in1=None, in2=None, in3=None, round_out=False):
+    """Stand-alone multi-head self-attention sweep (csrc/tokens.cu); qkv [B*T, 3 d].  ``round_out``: store ``out`` on the TF32
+    grid.  A head that does not fit the kernel's shared memory (8 T dh + 4 T^2 floats over 200 KB) raises."""
     lib = load_library()
     d = qkv.shape[1] // 3
     out = torch.empty(qkv.shape[0], d if sweep in (0, 2) else 3 * d, device=qkv.device)
     stream = torch.cuda.current_stream(qkv.device).cuda_stream
     with torch.cuda.device(qkv.device):
         rc = lib.bre_token_attention(sweep, _ptr(qkv), _ptr(in1), _ptr(in2), _ptr(in3), B, T, heads, d // heads, _ptr(P), _ptr(Pd), _ptr(out),
-                                     ctypes.c_void_p(stream))
+                                     int(bool(round_out)), ctypes.c_void_p(stream))
     _check(lib, rc, "bre_token_attention")
     return out

@@ -255,12 +255,13 @@ int bre_total_variation(const float* x, float* grad, int32_t N, int32_t H, int32
  *              sweep 0 and read by the others; sweep 1 also writes g_gamma / g_beta when non-NULL.
  *   attention: qkv [rows, 3 d] = (q | k | v) projections, heads x dh = d, no mask; in1..in3 per sweep: (1) dO [rows, d] |
  *              (2) (qkv)' | (3) dO', dO, (qkv)'; P / Pd [B, heads, T, T] are written by sweeps 0 / 2 and read later.
- * The engine's sweeps do not dispatch to these kernels yet (the transformer model family is the next row to be built). */
+ * round_out != 0 stores `out` on the TF32 grid (cvt.rna), as the engine does for the operands of tensor-core GEMMs.  The attention
+ * kernel keeps a whole head in shared memory: 8 T dh + 4 T^2 floats must fit in 200 KB, otherwise the call fails (-4). */
 int bre_token_layernorm(int32_t sweep, const float* x, const float* in1, const float* in2, const float* in3, const float* gamma,
                         const float* beta, const float* v_gamma, const float* v_beta, float eps, int32_t rows, int32_t C, float* stats,
-                        float* out, float* g_gamma, float* g_beta, void* stream);
+                        float* out, float* g_gamma, float* g_beta, int32_t round_out, void* stream);
 int bre_token_attention(int32_t sweep, const float* qkv, const float* in1, const float* in2, const float* in3, int32_t B, int32_t T,
-                        int32_t heads, int32_t dh, float* P, float* Pd, float* out, void* stream);
+                        int32_t heads, int32_t dh, float* P, float* Pd, float* out, int32_t round_out, void* stream);
 
 /* Token recovery of the text attacks (replaces `_postprocess_text_data._max_similarity`, breaching/attacks/base_attack.py:126-133):
  * tokens[n] = argmax_v <r_n - mean, e_v - mean> / |r_n - mean|^2 / |e_v - mean|^2 over the V rows of emb [*, d] (rows picked through

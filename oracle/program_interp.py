@@ -412,6 +412,7 @@ class ProgramInterpreter:
             dq = torch.zeros_like(centred)
             dq[1:] = -centred[:-1] / self.M
             self.dq = dq.view(n // T, T, -1)
+            self.d_T, self.inject = d, inject or {}
             return d[0].flatten(1).view(n // T, T, -1)
         seed = (p * zdot - p * (p * zdot).sum(dim=1, keepdim=True)) / n
         d, _, _ = self._reverse(seed, V=V, d_prev=self.d_B, inject=inject)
@@ -463,7 +464,7 @@ class ProgramInterpreter:
         dx = self.tangent_backward(V, inject)
         if task_regularization != 0:
             val = val + task_regularization * loss
-            dx = dx + task_regularization * self.d_B[0]
+            dx = dx + task_regularization * self.d_B[0].reshape(dx.shape)
         return val, dx, loss, G
 
 

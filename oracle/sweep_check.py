@@ -22,9 +22,32 @@ rounding-error bound derived for that element:
   * a stored tensor whose every element lies on the TF32 grid (13 low mantissa bits zero) was rounded on store: half a
     TF32 ulp of the reference (per accumulation for deltas summed over several consumers) is added.
 
+Token programs (``compiler.compile_transformer``: tensors are [rows = B x T, C, 1, 1]):
+
+  * ``posadd``: F and TF are one fp32 add / a copy (``2u`` of the magnitudes; the tangent is ``v_pos`` of row mod T exactly); the
+    positional-table gradient of B is a sum over the B sequences, ``(B + 4) 2^-23 sum |terms|``, its rows >= T exactly zero; the
+    delta passes to the candidate unchanged (task-loss gradient in B, candidate gradient in TB);
+  * ``layernorm`` (statistics over the C features of a row): composite bounds as for train-mode BN, ``TRAIN_C (C + 8) 2^-24``
+    times the magnitudes with the conditioning ``1 + mean(x^2) / var`` of the row as a factor; in those magnitudes ``xh`` counts
+    as ``|xh| + inv (|x| + |mean|)`` (the error of ``x - mean``); gamma / beta gradients are sums over rows, ``(rows + 4) 2^-23``
+    plus the composite term of ``xh``;
+  * ``attention``, per (sequence, head), recomputed in float64 from the stored ``qkv`` (and its tangent, the output delta and
+    tangent delta): a first-order running error bound.  Dot products over dh (scores) or T (P V, dS K, ...) cost
+    ``(n + 2) 2^-23`` of their magnitudes; the softmax adds ``(T + 2) 2^-23 + 3u + u |S - max S|`` relative to P plus the
+    P-weighted mean of the score errors; each product / difference one more ``u``; these errors are propagated through P V,
+    dS K / Q and their tangents (the kernel's stored P / P' carry exactly these errors);
+  * the next-token loss seed (sweep B) and its tangent (TB): row (b, t) is scored against the target row (b, t + 1) of the soft
+    targets, each sequence's last row is exactly zero, the mean runs over ``M = rows - rows / T``; only the first
+    ``logits_valid`` columns are real: the padded columns of the logits value, delta, tangent and tangent delta must be exactly
+    zero (the decoder's tangent dgrad would read a nonzero one through v);
+  * ``check_label_gradient``: d objective / d target probabilities, ``-(zdot - <p, zdot>) / M - tau (z - lse) / M`` of the
+    source row (row (b, t - 1) for tokens, 0 at t = 0), bounded like the seeds.
+
 ``delta[t]`` / ``tangent_delta[t]`` are checked as the sum over *all* consumers of ``t`` (residual branches included), which
 judges the accumulation flags; such a failure is reported at the consumer that runs last in the reverse sweep (the one with
 the lowest op index), where the buffer becomes final.
+
+The vision cross-entropy seed takes soft targets (a float ``labels`` tensor [N, classes]) as well as class indices.
 
 A buffer source provides ``tensor(which, tid)`` (``which`` in val / delta / tangent / tangent_delta, NCHW, ``None`` where a
 tensor has no such buffer), ``param(which, index)`` (G / v_operand / W_operand, torch layout), ``unwritten`` (tensor ids whose
@@ -87,6 +110,8 @@ class SweepChecker:
         self.obj = dict(scale=1.0, task_regularization=0.0, tv=None, norm=None, di=None, features=None)
         self.obj.update(objective)
         self.findings, self.ratios, self.off_grid = [], {}, set()
+        self.seq = getattr(prog, "seq_len", 0)
+        self.Vv = getattr(prog, "logits_valid", 0) or prog.tensors[prog.logits].C   # real classes
         ops = prog.ops
         self.first_consumer = {}
         for i, op in enumerate(ops):
@@ -97,11 +122,21 @@ class SweepChecker:
 
     # ------------------------------------------------------------------ buffers
     def T(self, which, tid):
+        """Buffer ``which`` of tensor ``tid`` in float64; logits-shaped tensors without their padded columns."""
         key = (which, tid)
         if key not in self._cache:
             v = self.src.tensor(which, tid)
+            if v is not None and tid == self.prog.logits and v.shape[1] > self.Vv:
+                v = v[:, :self.Vv]
             self._cache[key] = None if v is None else v.double()
         return self._cache[key]
+
+    def _padding(self, which, op, sweep):
+        """The padded logit columns of buffer ``which`` must be exactly zero."""
+        v = self.src.tensor(which, self.prog.logits)
+        if v is not None and v.shape[1] > self.Vv:
+            pad = v[:, self.Vv:].double()
+            self._cmp(op, sweep, f"{which}[t{self.prog.logits}] padded columns", pad, torch.zeros_like(pad), 0.0)
 
     def Pm(self, which, idx):
         key = ("p", which, idx)
@@ -110,8 +145,8 @@ class SweepChecker:
         return self._cache[key]
 
     # ------------------------------------------------------------------ comparison
-    def _cmp(self, i, sweep, what, y, ref, bound):
-        kind = "objective" if i < 0 else C.OP_NAMES[self.prog.ops[i].kind]
+    def _cmp(self, i, sweep, what, y, ref, bound, kind=None):
+        kind = kind or ("objective" if i < 0 else C.OP_NAMES[self.prog.ops[i].kind])
         err = (y - ref).abs()
         ratio = err / bound.clamp_min(TINY) if torch.is_tensor(bound) else err / max(bound, TINY)
         ratio = torch.where(err == 0, torch.zeros_like(ratio), ratio)
@@ -190,6 +225,85 @@ class SweepChecker:
         cond = 1.0 + self._m(x * x) / var.clamp_min(TINY)
         return mean, var, inv, xh, TRAIN_C * (Pch + 8) * U * cond
 
+    # ------------------------------------------------------------------ token helpers
+    @staticmethod
+    def _mc(t):
+        return t.mean(dim=1, keepdim=True)
+
+    def _ln(self, op, x):
+        """Row statistics of a LayerNorm input [rows, C]: mean, inv, xh, A (magnitude of xh with the error of x - mean), c."""
+        x = x.flatten(1)
+        mean = self._mc(x)
+        var = self._mc((x - mean) ** 2)
+        inv = 1.0 / torch.sqrt(var + op.eps)
+        xh = (x - mean) * inv
+        cond = 1.0 + self._mc(x * x) / var.clamp_min(TINY)
+        return mean, inv, xh, xh.abs() + inv * (x.abs() + mean.abs()), TRAIN_C * (x.shape[1] + 8) * U * cond
+
+    def _heads(self, t, op, width):
+        """[rows, width * d] -> ``width`` tensors [B, heads, T, dh]."""
+        rows = t.shape[0]
+        T_ = self.seq
+        parts = t.flatten(1).split(t.shape[1] // width, dim=1)
+        return [p.reshape(rows // T_, T_, op.R, -1).transpose(1, 2) for p in parts]
+
+    @staticmethod
+    def _merge(*ts):
+        return torch.cat([t.transpose(1, 2).reshape(t.shape[0] * t.shape[2], -1) for t in ts], dim=1)
+
+    @staticmethod
+    def _mm(pairs, n):
+        """sum of products A @ B over ``pairs`` = [(A, eA, B, eB)] (e: absolute error bound or None) with n terms in all:
+        (value, error bound)."""
+        val, err = 0.0, 0.0
+        mag = 0.0
+        for A, eA, B, eB in pairs:
+            val = val + A @ B
+            mag = mag + A.abs() @ B.abs()
+            if eA is not None:
+                err = err + eA @ B.abs()
+            if eB is not None:
+                err = err + A.abs() @ eB
+        return val, err + (n + 2) * U2 * mag
+
+    def _attention(self, op, qkv):
+        """Scores and probabilities of every (sequence, head) with their error bounds."""
+        Q, K, Vv = self._heads(qkv, op, 3)
+        dh, T_ = Q.shape[-1], self.seq
+        s = 1.0 / dh ** 0.5
+        S0, eS0 = self._mm([(Q, None, K.transpose(-1, -2), None)], dh)
+        S = S0 * s
+        eS = eS0 * s + 3 * U * S.abs()
+        P = torch.softmax(S, dim=-1)
+        rho = eS + U * (S - S.amax(dim=-1, keepdim=True)).abs() + 2 * U
+        eP = P * (rho + (P * rho).sum(dim=-1, keepdim=True) + (T_ + 2) * U2 + 2 * U)
+        return Q, K, Vv, s, P, eP
+
+    def _att_tangent_probs(self, op, Q, K, s, P, eP):
+        """Tangent of the probabilities from the stored tangent of qkv: (Q', K', V', P', error of P')."""
+        Qd, Kd, Vd = self._heads(self.T("tangent", op.tin), op, 3)
+        dh, T_ = Q.shape[-1], self.seq
+        Sd0, eSd0 = self._mm([(Qd, None, K.transpose(-1, -2), None), (Q, None, Kd.transpose(-1, -2), None)], 2 * dh)
+        Sd = Sd0 * s
+        eSd = eSd0 * s + 3 * U * Sd.abs()
+        acc = (P * Sd).sum(dim=-1, keepdim=True)
+        eacc = (T_ + 2) * U2 * (P * Sd.abs()).sum(dim=-1, keepdim=True) + (eP * Sd.abs() + P * eSd).sum(dim=-1, keepdim=True)
+        diff = Sd - acc
+        Pd = P * diff
+        ePd = eP * diff.abs() + P * (eSd + eacc + U * diff.abs()) + U * Pd.abs()
+        return Qd, Kd, Vd, Pd, ePd
+
+    def _seed_rows(self, rows):
+        """Token programs: (scored-row mask [rows, 1], M)."""
+        keep = ((torch.arange(rows) % self.seq) != self.seq - 1).double().view(-1, 1)
+        return keep, rows - rows // self.seq
+
+    def _targets(self, n):
+        """Soft targets [n, classes] (float64) or the one-hot of class-index labels."""
+        if self.labels.is_floating_point():
+            return self.labels.double().reshape(n, -1)
+        return F.one_hot(self.labels.view(-1).long(), self.Vv).double()
+
     # ------------------------------------------------------------------ sweeps
     def check(self, raise_on_failure=True):
         self.forward()
@@ -238,17 +352,57 @@ class SweepChecker:
                 hw = x.shape[2] * x.shape[3]
                 ref = x.mean(dim=(2, 3), keepdim=True)
                 self._cmp(i, "F", f"val[t{op.tout}]", y, ref, (hw + 2) * U2 * x.abs().mean(dim=(2, 3), keepdim=True))
-        # cross-entropy seed of sweep B
+            elif op.kind == C.OP_POSADD:
+                pos = self._pos_rows(self.P[op.w], x)
+                ref = x + pos
+                self._cmp(i, "F", f"val[t{op.tout}]", y, ref, 2 * U * (x.abs() + pos.abs()) + self._rounded(y, ref))
+            elif op.kind == C.OP_LAYERNORM:
+                mean, inv, xh, A, c = self._ln(op, x)
+                gam, bet = self.P[op.gamma].view(1, -1), self.P[op.beta].view(1, -1)
+                ref = (gam * xh + bet).view_as(y)
+                bound = (c * gam.abs() * inv * (x.flatten(1).abs() + mean.abs()) + 4 * U * (gam * xh).abs() + 4 * U * bet.abs()).view_as(y)
+                self._cmp(i, "F", f"val[t{op.tout}]", y, ref, bound + self._rounded(y, ref))
+            elif op.kind == C.OP_ATTENTION:
+                _, _, Vv, _, P, eP = self._attention(op, x)
+                O, eO = self._mm([(P, eP, Vv, None)], self.seq)
+                ref, bound = self._merge(O).view_as(y), self._merge(eO).view_as(y)
+                self._cmp(i, "F", f"val[t{op.tout}]", y, ref, bound + self._rounded(y, ref))
         z = self.T("val", prog.logits).flatten(1)
+        self.p = torch.softmax(z, dim=1)
+        self._padding("val", len(prog.ops) - 1, "F")
+        if self.seq:   # the next-token seed is checked with sweep B
+            return
+        # cross-entropy seed of sweep B (class indices or soft targets)
         n = z.shape[0]
-        p = torch.softmax(z, dim=1)
-        onehot = F.one_hot(self.labels.view(-1).long(), z.shape[1]).double()
-        ref = (p - onehot) / n
+        p = self.p
+        q = self._targets(n)
+        ref = (p - q) / n
         rng = (z - z.max(dim=1, keepdim=True).values).abs()
-        bound = (16 + 2 * rng) * U * (p + onehot) / n
+        bound = (16 + 2 * rng) * U * (p + q.abs()) / n
         d = self.T("delta", prog.logits).flatten(1)
         self._cmp(len(prog.ops) - 1, "F", f"delta[t{prog.logits}] (cross-entropy seed)", d, ref, bound)
-        self.p = p
+
+    def _pos_rows(self, pos, like):
+        rows = like.shape[0]
+        return pos[:self.seq].repeat(rows // self.seq, 1).view_as(like)
+
+    def _token_seed(self):
+        """Next-token loss seed of sweep B: (p - q of the next row) / M on scored rows, exactly 0 on each sequence's last row."""
+        prog = self.prog
+        z = self.T("val", prog.logits).flatten(1)
+        rows = z.shape[0]
+        keep, M = self._seed_rows(rows)
+        p = self.p
+        q = self._targets(rows)
+        qn = torch.zeros_like(q)
+        qn[:-1] = q[1:]
+        qn = qn * keep
+        ref = (p - qn) * keep / M
+        rng = (z - z.max(dim=1, keepdim=True).values).abs()
+        bound = (16 + 2 * rng) * U * (p + qn) * keep / M
+        d = self.T("delta", prog.logits).flatten(1)
+        self._cmp(len(prog.ops) - 1, "B", f"delta[t{prog.logits}] (next-token loss seed)", d, ref, bound + self._rounded(d, ref))
+        self._padding("delta", len(prog.ops) - 1, "B")
 
     def _reverse(self, sweep):
         """Contributions of every op to the deltas (B) or tangent deltas (TB) of its inputs; returns {tid: [(i, ref, bound, mag)]}."""
@@ -350,7 +504,89 @@ class SweepChecker:
                 hw = x.shape[2] * x.shape[3]
                 ref = (dout / hw).expand_as(x)
                 add(op.tin, i, ref, 2 * U * ref.abs(), ref.abs())
+            elif op.kind == C.OP_POSADD:
+                add(op.tin, i, dout, 0.0, dout.abs())
+                if not tang:   # positional-table gradient: sum over the sequences, rows >= T untouched
+                    d2 = dout.flatten(1).reshape(-1, self.seq, dout.shape[1])
+                    Gp = self.Pm("G", op.w)
+                    ref, mag = torch.zeros_like(Gp), torch.zeros_like(Gp)
+                    ref[:self.seq], mag[:self.seq] = d2.sum(dim=0), d2.abs().sum(dim=0)
+                    self._cmp(i, "B", f"G[{op.w}] (positional table gradient)", Gp, ref, (d2.shape[0] + 4) * U2 * mag)
+            elif op.kind == C.OP_LAYERNORM:
+                ref, bound, mag = self._ln_reverse(i, op, x, dout, tang)
+                add(op.tin, i, ref.view_as(x), bound.view_as(x), mag.view_as(x))
+            elif op.kind == C.OP_ATTENTION:
+                ref, bound = self._att_reverse(op, x, dout, tang)
+                add(op.tin, i, ref.view_as(x), bound.view_as(x), (ref.abs() + bound).view_as(x))
         return contrib
+
+    def _ln_reverse(self, i, op, x, dout, tang):
+        """LayerNorm input delta (B) or tangent delta (TB): (reference, bound, magnitude) as [rows, C]; B also checks gamma / beta."""
+        m = self._mc
+        mean, inv, xh, A, c = self._ln(op, x)
+        gam = self.P[op.gamma].view(1, -1)
+        dy = dout.flatten(1)
+        if not tang:
+            t = dy * gam
+            ref = inv * (t - m(t) - xh * m(t * xh))
+            mag = inv * (t.abs() + m(t.abs()) + A * m(t.abs() * A))
+            rows = dy.shape[0]
+            s = (dy.abs() * xh.abs()).sum(dim=0)
+            bound = (rows + 4) * U2 * s + (c * dy.abs() * inv * (x.flatten(1).abs() + mean.abs())).sum(dim=0)
+            self._cmp(i, "B", f"G[{op.gamma}] (LayerNorm gamma gradient)", self.Pm("G", op.gamma), (dy * xh).sum(dim=0), bound)
+            self._cmp(i, "B", f"G[{op.beta}] (LayerNorm beta gradient)", self.Pm("G", op.beta), dy.sum(dim=0),
+                      (rows + 4) * U2 * dy.abs().sum(dim=0))
+            return ref, c * mag, mag
+        dyB = self.T("delta", op.tout).flatten(1)
+        xd = self.T("tangent", op.tin).flatten(1)
+        vg = self.Pm("v_operand", op.gamma).view(1, -1)
+        xhd = inv * (xd - m(xd) - xh * m(xh * xd))
+        t, td = dyB * gam, dy * gam + dyB * vg
+        u = t - m(t) - xh * m(t * xh)
+        ud = td - m(td) - xhd * m(t * xh) - xh * m(td * xh + t * xhd)
+        ref = inv * ud - u * m(xh * xd) * inv * inv
+        At, Atd = t.abs(), dy.abs() * gam.abs() + dyB.abs() * vg.abs()
+        Axhd = inv * (xd.abs() + m(xd.abs()) + A * m(A * xd.abs()))
+        Au = At + m(At) + A * m(At * A)
+        Aud = Atd + m(Atd) + Axhd * m(At * A) + A * m(Atd * A + At * Axhd)
+        mag = inv * Aud + Au * m(A * xd.abs()) * inv * inv
+        return ref, c * mag, mag
+
+    def _att_reverse(self, op, qkv, dout, tang):
+        """Attention: delta (B) or tangent delta (TB) of qkv, (reference, bound) as [rows, 3 d]."""
+        T_ = self.seq
+        Q, K, Vv, s, P, eP = self._attention(op, qkv)
+        dh = Q.shape[-1]
+        tr = lambda t: t.transpose(-1, -2)  # noqa: E731
+        (dO,) = self._heads(self.T("delta", op.tout), op, 1)
+        dP, edP = self._mm([(dO, None, tr(Vv), None)], dh)
+        r = (dP * P).sum(dim=-1, keepdim=True)
+        er = (T_ + 2) * U2 * (dP.abs() * P).sum(dim=-1, keepdim=True) + (edP * P + dP.abs() * eP).sum(dim=-1, keepdim=True)
+        diff = dP - r
+        ediff = edP + er + U * diff.abs()
+        dS = P * diff
+        edS = eP * diff.abs() + P * ediff + U * dS.abs()
+        if not tang:
+            dQ, edQ = self._mm([(dS, edS, K, None)], T_)
+            dK, edK = self._mm([(tr(dS), tr(edS), Q, None)], T_)
+            dV, edV = self._mm([(tr(P), tr(eP), dO, None)], T_)
+            grads = [(dQ * s, edQ * s + 3 * U * (dQ * s).abs()), (dK * s, edK * s + 3 * U * (dK * s).abs()), (dV, edV)]
+        else:
+            (dOd,) = self._heads(dout, op, 1)
+            Qd, Kd, Vd, Pd, ePd = self._att_tangent_probs(op, Q, K, s, P, eP)
+            dPd, edPd = self._mm([(dOd, None, tr(Vv), None), (dO, None, tr(Vd), None)], 2 * dh)
+            rd = (dPd * P + dP * Pd).sum(dim=-1, keepdim=True)
+            erd = (2 * T_ + 2) * U2 * (dPd.abs() * P + dP.abs() * Pd.abs()).sum(dim=-1, keepdim=True) + \
+                (edPd * P + dPd.abs() * eP + edP * Pd.abs() + dP.abs() * ePd).sum(dim=-1, keepdim=True)
+            diff2 = dPd - rd
+            ediff2 = edPd + erd + U * diff2.abs()
+            dSd = Pd * diff + P * diff2
+            edSd = ePd * diff.abs() + Pd.abs() * ediff + eP * diff2.abs() + P * ediff2 + 2 * U * ((Pd * diff).abs() + (P * diff2).abs())
+            dQ, edQ = self._mm([(dSd, edSd, K, None), (dS, edS, Kd, None)], 2 * T_)
+            dK, edK = self._mm([(tr(dSd), tr(edSd), Q, None), (tr(dS), tr(edS), Qd, None)], 2 * T_)
+            dV, edV = self._mm([(tr(Pd), tr(ePd), dO, None), (tr(P), tr(eP), dOd, None)], 2 * T_)
+            grads = [(dQ * s, edQ * s + 3 * U * (dQ * s).abs()), (dK * s, edK * s + 3 * U * (dK * s).abs()), (dV, edV)]
+        return self._merge(*[g for g, _ in grads]), self._merge(*[e for _, e in grads])
 
     def _bn_param_grads(self, i, op, du, xh, xhm):
         Pch = du.shape[0] * du.shape[2] * du.shape[3]
@@ -397,6 +633,8 @@ class SweepChecker:
         return contrib
 
     def backward(self):
+        if self.seq:
+            self._token_seed()
         contrib = self._check_deltas("B", self._reverse("B"))
         if self.obj["task_regularization"] != 0 and 0 in contrib:
             parts = contrib[0]
@@ -507,19 +745,43 @@ class SweepChecker:
                 hw = tin.shape[2] * tin.shape[3]
                 self._cmp(i, "TF", f"tangent[t{op.tout}]", y, tin.mean(dim=(2, 3), keepdim=True),
                           (hw + 2) * U2 * tin.abs().mean(dim=(2, 3), keepdim=True))
+            elif op.kind == C.OP_POSADD:   # the candidate's tangent is zero: v of the positional table, copied
+                ref = self._pos_rows(self.Pm("v_operand", op.w), y)
+                self._cmp(i, "TF", f"tangent[t{op.tout}]", y, ref, self._rounded(y, ref))
+            elif op.kind == C.OP_LAYERNORM:
+                m = self._mc
+                mean, inv, xh, A, c = self._ln(op, x)
+                gam = self.P[op.gamma].view(1, -1)
+                vg, vb = (self.Pm("v_operand", k).view(1, -1) for k in (op.gamma, op.beta))
+                xd = tin.flatten(1)
+                xhd = inv * (xd - m(xd) - xh * m(xh * xd))
+                ref = (vg * xh + gam * xhd + vb).view_as(y)
+                Axhd = inv * (xd.abs() + m(xd.abs()) + A * m(A * xd.abs()))
+                bound = (c * (vg.abs() * A + gam.abs() * Axhd) + 4 * U * vb.abs()).view_as(y)
+                self._cmp(i, "TF", f"tangent[t{op.tout}]", y, ref, bound + self._rounded(y, ref))
+            elif op.kind == C.OP_ATTENTION:
+                Q, K, Vv, s, P, eP = self._attention(op, x)
+                _, _, Vd, Pd, ePd = self._att_tangent_probs(op, Q, K, s, P, eP)
+                Od, eOd = self._mm([(Pd, ePd, Vv, None), (P, eP, Vd, None)], 2 * self.seq)
+                ref, bound = self._merge(Od).view_as(y), self._merge(eOd).view_as(y)
+                self._cmp(i, "TF", f"tangent[t{op.tout}]", y, ref, bound + self._rounded(y, ref))
+        self._padding("tangent", len(prog.ops) - 1, "TF")
 
     def tangent_backward(self):
         prog = self.prog
-        # seed: tangent of the cross-entropy delta
+        # seed: tangent of the cross-entropy delta (token programs: scored rows, mean over M)
         z = self.T("val", prog.logits).flatten(1)
         zd = self.T("tangent", prog.logits).flatten(1)
         n = z.shape[0]
+        keep, M = self._seed_rows(n) if self.seq else (1.0, n)
         p = torch.softmax(z, dim=1)
-        ref = (p * zd - p * (p * zd).sum(dim=1, keepdim=True)) / n
+        ref = (p * zd - p * (p * zd).sum(dim=1, keepdim=True)) * keep / M
         rng = (z - z.max(dim=1, keepdim=True).values).abs()
-        mag = (p * zd.abs() + p * (p * zd.abs()).sum(dim=1, keepdim=True)) / n
+        mag = (p * zd.abs() + p * (p * zd.abs()).sum(dim=1, keepdim=True)) * keep / M
         y = self.T("tangent_delta", prog.logits).flatten(1)
-        self._cmp(len(prog.ops) - 1, "TB", f"tangent_delta[t{prog.logits}] (cross-entropy seed)", y, ref, (16 + 2 * rng) * U * mag)
+        self._cmp(len(prog.ops) - 1, "TB", f"tangent_delta[t{prog.logits}] (cross-entropy seed)", y, ref,
+                  (16 + 2 * rng) * U * mag + self._rounded(y, ref))
+        self._padding("tangent_delta", len(prog.ops) - 1, "TB")
         contrib = self._check_deltas("TB", self._reverse("TB"))
         # the candidate gradient: first op's contribution + image priors + task term
         parts = contrib.get(0, [])
@@ -547,6 +809,33 @@ class SweepChecker:
             bound = bound + 2 * U * abs(o["task_regularization"]) * dt.abs()
         self._cmp(self.first_consumer[0], "TB", "tangent_delta[t0] (candidate gradient)", self.T("tangent_delta", 0), ref, bound)
 
+    def check_label_gradient(self, lg, raise_on_failure=True):
+        """d objective / d (target probabilities) as ``bre_engine_label_gradient`` returns it ([rows or N, classes]):
+        ``-(zdot - <p, zdot>) / M - tau (z - lse) / M`` of the source row -- the row itself for vision programs (M = N), row
+        (b, t - 1) for token programs (exactly 0 at t = 0).  Run after ``check()`` (or ``forward()``)."""
+        z = self.T("val", self.prog.logits).flatten(1)
+        zd = self.T("tangent", self.prog.logits).flatten(1)
+        n = z.shape[0]
+        tau = self.obj["task_regularization"]
+        p = torch.softmax(z, dim=1)
+        lse = torch.logsumexp(z, dim=1, keepdim=True)
+        rng = (z - z.max(dim=1, keepdim=True).values).abs()
+        M = n - n // self.seq if self.seq else n
+        dot = (p * zd).sum(dim=1, keepdim=True)
+        ref = -(zd - dot) / M - tau * (z - lse) / M
+        # <p, zdot> from the stored fp32 p (softmax bound) in double; lse in fp32 from a double sum of expf; a few roundings each
+        bound = (4 * U * (zd.abs() + (p * zd.abs()).sum(dim=1, keepdim=True)) + ((16 + 2 * rng) * U * p * zd.abs()).sum(dim=1, keepdim=True)
+                 + abs(tau) * (8 * U * (z.abs() + lse.abs()) + (4 + 2 * rng.amax(dim=1, keepdim=True)) * U)) / M + U * ref.abs()
+        if self.seq:
+            first = (torch.arange(n) % self.seq == 0).view(-1, 1)
+            ref = torch.cat([torch.zeros_like(ref[:1]), ref[:-1]]).masked_fill(first, 0.0)
+            bound = torch.cat([torch.zeros_like(bound[:1]), bound[:-1]]).masked_fill(first, 0.0)
+        y = lg.double().reshape(n, -1)
+        self._cmp(len(self.prog.ops) - 1, "L", "label gradient", y, ref, bound, kind="label")
+        if raise_on_failure and self.findings:
+            raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
+        return self.findings
+
 
 class InterpreterSource:
     """Buffers of a float64 ``ProgramInterpreter.matching_gradient`` run; ``grad_x``: the full candidate gradient (priors and
@@ -568,7 +857,7 @@ class InterpreterSource:
         if which == "tangent":
             return it.ta.get(tid)
         if tid == 0:
-            return self.grad_x
+            return self.grad_x.reshape(it.a[0].shape)
         return it.d_T[tid] + it.inject.get(tid, 0)   # the engine adds the prior adjoints into the stored tangent delta
 
     def param(self, which, idx):

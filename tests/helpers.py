@@ -178,6 +178,8 @@ def sweep_objective(cfg, features=None):
 
     obj = dict(kind=cfg.objective.type, scale=float(cfg.objective.get("scale", 1.0)),
                task_regularization=float(cfg.objective.get("task_regularization", 0.0) or 0.0))
+    if cfg.objective.type == "tag-euclidean":
+        obj.update(tag_scale=float(cfg.objective.get("tag_scale", 0.1)), scale_scheme=cfg.objective.get("scale_scheme", "linear"))
     if on("total_variation"):
         r = reg["total_variation"]
         obj["tv"] = dict(scale=r["scale"], inner_exp=r.get("inner_exp", 1), outer_exp=r.get("outer_exp", 1), eps=r.get("eps", 1e-8),
@@ -189,3 +191,30 @@ def sweep_objective(cfg, features=None):
     if on("features") and features is not None:
         obj["features"] = dict(scale=reg["features"]["scale"], measured=features)
     return obj
+
+
+def unwritten_tangents(eng):
+    """Tensors whose tangent the last evaluation did not store (fuse_bnact: a conv output whose only consumer is the BN op that ran
+    in the conv's epilogue), as the engine reports them."""
+    return {op.tin for i, op in enumerate(eng.prog.ops) if eng.debug_op(i)["tangent_in_unwritten"]}
+
+
+class EngineSource:
+    """The sweep checker's buffer source (oracle/sweep_check.py): the engine's debug read-back (NCHW / torch layout).  Build it
+    after the evaluation."""
+
+    def __init__(self, eng):
+        self.eng = eng
+        self.unwritten = unwritten_tangents(eng)
+        self.stem = {i for i in range(len(eng.prog.ops)) if eng.debug_op(i)["stem_columns"]}
+
+    def rounds_operands(self, i):
+        return i in self.stem   # the candidate-fed conv on the tensor-core column path rounds x, W and v itself
+
+    def tensor(self, which, tid):
+        if tid == 0 and which == "tangent":
+            return None
+        return self.eng.debug_tensor(which, tid).double()
+
+    def param(self, which, idx):
+        return self.eng.debug_param(which, idx).double()

@@ -13,7 +13,8 @@ from breaching_b200 import compiler as C  # noqa: E402
 from breaching_b200 import get_attack_config, synthetic  # noqa: E402
 from breaching_b200.engine import Engine  # noqa: E402
 from breaching_b200.schedule import lr_table  # noqa: E402
-from test_sweep_local_gpu import build_case, candidate, make_engine, unwritten_tangents  # noqa: E402
+from helpers import unwritten_tangents  # noqa: E402
+from test_sweep_local_gpu import build_case, candidate, make_engine  # noqa: E402
 
 DEV = torch.device("cuda:0")
 

@@ -13,36 +13,10 @@ pytestmark = pytest.mark.gpu
 from breaching_b200 import compiler as C  # noqa: E402
 from breaching_b200 import get_attack_config, synthetic  # noqa: E402
 from breaching_b200.engine import Engine  # noqa: E402
-from helpers import odd_case, sweep_objective  # noqa: E402
+from helpers import EngineSource, odd_case, sweep_objective  # noqa: E402
 from oracle.sweep_check import SweepChecker  # noqa: E402
 
 DEV = torch.device("cuda:0")
-
-
-def unwritten_tangents(eng):
-    """Tensors whose tangent the last evaluation did not store (fuse_bnact: a conv output whose only consumer is the BN op that ran
-    in the conv's epilogue), as the engine reports them."""
-    return {op.tin for i, op in enumerate(eng.prog.ops) if eng.debug_op(i)["tangent_in_unwritten"]}
-
-
-class EngineSource:
-    """The checker's buffer source: the engine's debug read-back (NCHW / torch layout).  Build it after the evaluation."""
-
-    def __init__(self, eng):
-        self.eng = eng
-        self.unwritten = unwritten_tangents(eng)
-        self.stem = {i for i in range(len(eng.prog.ops)) if eng.debug_op(i)["stem_columns"]}
-
-    def rounds_operands(self, i):
-        return i in self.stem   # the candidate-fed conv on the tensor-core column path rounds x, W and v itself
-
-    def tensor(self, which, tid):
-        if tid == 0 and which == "tangent":
-            return None
-        return self.eng.debug_tensor(which, tid).double()
-
-    def param(self, which, idx):
-        return self.eng.debug_param(which, idx).double()
 
 
 def build_case(name):

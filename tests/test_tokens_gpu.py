@@ -39,7 +39,9 @@ def test_layernorm_four_sweeps(rows, C):
     assert _relerr(out3, dxd) < 5e-5
 
 
-@pytest.mark.parametrize("B,T,heads,dh", [(1, 32, 8, 12), (2, 8, 4, 4), (3, 5, 2, 7)])
+# (1, 33, 2, 8): one row past a lane stride; (2, 64, 4, 16): two full strides; (1, 100, 2, 12): 198 400 B of shared memory, just
+# under the kernel's 200 KB opt-in
+@pytest.mark.parametrize("B,T,heads,dh", [(1, 32, 8, 12), (2, 8, 4, 4), (3, 5, 2, 7), (1, 33, 2, 8), (2, 64, 4, 16), (1, 100, 2, 12)])
 def test_attention_four_sweeps(B, T, heads, dh):
     gen = torch.Generator().manual_seed(B * 100 + T)
     d = heads * dh
@@ -82,6 +84,41 @@ def test_attention_four_sweeps(B, T, heads, dh):
     assert _relerr(out2, Od) < 2e-5 and _relerr(Pdg, Pd) < 2e-5
     out3 = E.token_attention(3, f(qkv), B, T, heads, Pg, Pdg, in1=f(dOd), in2=f(dO), in3=f(qkvd))
     assert _relerr(out3, dqkvd) < 5e-5
+
+
+def test_attention_head_over_the_shared_memory_limit_is_rejected():
+    """T = 128, dh = 12 needs 8 T dh + 4 T^2 floats = 311 296 B: an error naming the limit, not a launch."""
+    B, T, heads, dh = 1, 128, 2, 12
+    qkv = torch.randn(B * T, 3 * heads * dh, device=DEV)
+    P, Pd = torch.empty(B, heads, T, T, device=DEV), torch.empty(B, heads, T, T, device=DEV)
+    with pytest.raises(E.EngineError, match="311296 B of shared memory"):
+        E.token_attention(0, qkv, B, T, heads, P, Pd)
+
+
+@pytest.mark.parametrize("sweep", [0, 1, 2, 3])
+def test_token_kernels_round_their_output_on_request(sweep):
+    """``round_out`` stores exactly the TF32 rounding (cvt.rna) of what the kernel stores without it."""
+    from oracle.sweep_check import on_grid, rna
+
+    gen = torch.Generator().manual_seed(41 + sweep)
+    rows, C, B, T, heads = 24, 48, 2, 12, 4
+    r = lambda *s: torch.randn(*s, generator=gen).to(DEV)  # noqa: E731
+    x, a1, a2, a3, g, b, vg, vb = r(rows, C), r(rows, C), r(rows, C), r(rows, C), 1 + 0.1 * r(C), r(C), r(C), r(C)
+    stats = torch.empty(rows, 2, device=DEV)
+    E.token_layernorm(0, x, g, b, stats)
+    kw = dict(in1=a1, in2=a2, in3=a3, v_gamma=vg, v_beta=vb)
+    plain = E.token_layernorm(sweep, x, g, b, stats, **kw)
+    rounded = E.token_layernorm(sweep, x, g, b, stats, round_out=True, **kw)
+    assert not on_grid(plain.cpu()) and torch.equal(rounded.cpu().double(), rna(plain.cpu().double()))
+    qkv, qkvd, dO, dOd = r(B * T, 3 * C), r(B * T, 3 * C), r(B * T, C), r(B * T, C)
+    P, Pd = torch.empty(B, heads, T, T, device=DEV), torch.empty(B, heads, T, T, device=DEV)
+    E.token_attention(0, qkv, B, T, heads, P, Pd)
+    E.token_attention(2, qkv, B, T, heads, P, Pd, in1=qkvd)
+    ins = {0: {}, 1: dict(in1=dO), 2: dict(in1=qkvd), 3: dict(in1=dOd, in2=dO, in3=qkvd)}[sweep]
+    Pk, Pdk = P.clone(), Pd.clone()   # sweeps 0 / 2 rewrite P / P'; the same values either way
+    plain = E.token_attention(sweep, qkv, B, T, heads, P, Pd, **ins)
+    rounded = E.token_attention(sweep, qkv, B, T, heads, Pk, Pdk, round_out=True, **ins)
+    assert not on_grid(plain.cpu()) and torch.equal(rounded.cpu().double(), rna(plain.cpu().double()))
 
 
 @pytest.mark.parametrize("backend", ["simt", "tc"])
