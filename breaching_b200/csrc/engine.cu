@@ -172,6 +172,10 @@ struct bre_engine {
   std::vector<BnPrep*> ms_bnprep_dev;  // per step (k >= 1): device table for the batched BN-constant refresh
   int n_bn_layers = 0;
   bool want_tangent_G = false;
+  // option "debug_multistep_stop" (tests): 0 = off; s in 1..K = the evaluation returns after step s-1's forward and backward
+  // sweeps and its W / D updates; s = K + 1 + k = it returns after step k's tangent sweeps, before its candidate-gradient axpy
+  // and the adjoint update.  A host-side branch only: the captured iteration is the same.
+  int debug_ms_stop = 0;
   // column path of the candidate-fed convolution on the tensor-core back end (stem_cols.cu)
   int stem_op = -1, stem_Kp = 0;
   float *xcol = nullptr, *dcol = nullptr, *Wcol = nullptr, *Vcol = nullptr, *Gcol = nullptr;
@@ -880,7 +884,7 @@ struct bre_engine {
   }
   int refresh_bn_constants(int k);   // defined below (needs a kernel)
 
-  int multistep_forward() {
+  int multistep_forward(int stop = 0) {   // stop = s in 1..K: return after step s - 1
     for (int k = 0; k < ms_steps; ++k) {
       bind_step(k);
       if (k > 0) BRE_TRY(refresh_bn_constants(k));
@@ -892,13 +896,15 @@ struct bre_engine {
       if (tc_round()) BRE_LAUNCH(launch_round_tf32(ms_W[k + 1], ms_Wt[k + 1], P_pad, stream));
       if (k == 0) BRE_CUDA_CHECK(cudaMemsetAsync(ms_D, 0, P_pad * sizeof(float), stream));
       BRE_LAUNCH(launch_axpby(ms_D, G, -ms_lr, ms_D, P_pad, stream));
+      if (stop == k + 1) return 0;
     }
     return 0;
   }
 
   int evaluate_multistep() {
     BRE_CUDA_CHECK(cudaMemsetAsync(gradx, 0, nx * sizeof(float), stream));
-    BRE_TRY(multistep_forward());
+    BRE_TRY(multistep_forward(debug_ms_stop));
+    if (debug_ms_stop >= 1 && debug_ms_stop <= ms_steps) return 0;
     const float mv = cfg.objective == BRE_OBJ_MASKED_COSINE ? cfg.mask_value : -1.f;
     BRE_LAUNCH(launch_match_reduce(ms_D, g, chunk_w, P_pad, mv, cfg.objective, cfg.obj_scale, cfg.tag_scale, cfg.angular_fudge, true, sc,
                                    dpartials, dcounter, stream));
@@ -912,6 +918,7 @@ struct bre_engine {
       const int rc = sweep_tangent_backward();
       want_tangent_G = false;
       if (rc != 0) return rc;
+      if (debug_ms_stop == ms_steps + 1 + k) return 0;
       // d Phi / d x_k = -lr * d/d eps grad_x L(x_k, W_{k-1} + eps u_k)
       BRE_LAUNCH(launch_axpy(gradx_step, gradx + ms_offset[k], -ms_lr, nstep, stream));
       if (k > 0) {
@@ -1499,6 +1506,7 @@ int bre_engine_get_joint_labels(bre_engine* e, int32_t best, float* out) {
 int bre_engine_run(bre_engine* e, int32_t n_iters) {
   if (!e || n_iters < 0) { set_error("bre_engine_run: bad arguments"); return BRE_ERR_INVALID; }
   if (!e->trial_begun) { set_error("bre_engine_begin_trial must be called first"); return BRE_ERR_STATE; }
+  if (e->debug_ms_stop != 0) { set_error("bre_engine_run: debug_multistep_stop is set"); return BRE_ERR_STATE; }
   BRE_CUDA_CHECK(cudaSetDevice(e->device));
   if (!e->use_graph) {
     BRE_TRY(e->build_chunk_modes());
@@ -1758,18 +1766,17 @@ int bre_engine_last_terms(bre_engine* e, double* terms6) {
   return BRE_OK;
 }
 
-int bre_engine_debug_param(bre_engine* e, int32_t which, int32_t index, float* out_host) {
-  if (!e || !out_host || index < 0 || index >= (int)e->params.size() || which < 0 || which > 5) return BRE_ERR_INVALID;
-  BRE_CUDA_CHECK(cudaSetDevice(e->device));
-  // 4 / 5: the direction / weights as the GEMMs read them -- the TF32 shadow for the weight of a layer that Vg / Wg route to it
-  bool shadow = false;
-  if (which >= 4)
-    for (const bre_op_desc& op : e->ops)
-      if ((op.kind == BRE_OP_CONV || op.kind == BRE_OP_LINEAR) && op.w == index && e->round_val(op.tin) && !e->is_precise(e->op_index(op)))
-        shadow = true;
-  const float* arenas[6] = {e->G, e->V, e->W, e->g, shadow ? e->Vt : e->V, shadow ? e->Wt : e->W};
+// parameter `index` is the weight of a layer whose GEMMs read the TF32 shadows (Vg / Wg route to them)
+static bool param_is_shadowed(bre_engine* e, int32_t index) {
+  for (const bre_op_desc& op : e->ops)
+    if ((op.kind == BRE_OP_CONV || op.kind == BRE_OP_LINEAR) && op.w == index && e->round_val(op.tin) && !e->is_precise(e->op_index(op)))
+      return true;
+  return false;
+}
+
+static int copy_param_out(bre_engine* e, const float* arena, int32_t index, float* out_host) {
   const ParamInfo& pi = e->params[index];
-  const float* src = arenas[which] + pi.off;
+  const float* src = arena + pi.off;
   if (pi.desc.perm != BRE_PERM_NONE) {
     BRE_TRY(launch_permute(src, e->stage, pi.desc.d0, pi.desc.d1, pi.desc.d2, true, e->stream));
     src = e->stage;
@@ -1777,6 +1784,24 @@ int bre_engine_debug_param(bre_engine* e, int32_t which, int32_t index, float* o
   BRE_CUDA_CHECK(cudaMemcpyAsync(out_host, src, pi.desc.numel * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
   BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
   return BRE_OK;
+}
+
+int bre_engine_debug_step_param(bre_engine* e, int32_t which, int32_t step, int32_t index, float* out_host) {
+  if (!e || !out_host || index < 0 || index >= (int)e->params.size() || which < 0 || which > 2) return BRE_ERR_INVALID;
+  if (e->ms_steps == 0 || step < 0 || step > e->ms_steps) { set_error("bre_engine_debug_step_param: no such local step"); return BRE_ERR_INVALID; }
+  BRE_CUDA_CHECK(cudaSetDevice(e->device));
+  const bool shadow = which == 1 && param_is_shadowed(e, index);
+  const float* arena = which == 2 ? e->ms_D : shadow ? e->ms_Wt[step] : e->ms_W[step];
+  return copy_param_out(e, arena, index, out_host);
+}
+
+int bre_engine_debug_param(bre_engine* e, int32_t which, int32_t index, float* out_host) {
+  if (!e || !out_host || index < 0 || index >= (int)e->params.size() || which < 0 || which > 5) return BRE_ERR_INVALID;
+  BRE_CUDA_CHECK(cudaSetDevice(e->device));
+  // 4 / 5: the direction / weights as the GEMMs read them -- the TF32 shadow for the weight of a layer that Vg / Wg route to it
+  const bool shadow = which >= 4 && param_is_shadowed(e, index);
+  const float* arenas[6] = {e->G, e->V, e->W, e->g, shadow ? e->Vt : e->V, shadow ? e->Wt : e->W};
+  return copy_param_out(e, arenas[which], index, out_host);
 }
 
 int bre_engine_debug_tensor(bre_engine* e, int32_t which, int32_t tensor, float* out_host) {
@@ -1815,6 +1840,10 @@ int bre_engine_set_option(bre_engine* e, const char* name, int64_t value) {
   if (n == "pdl") { bre::set_pdl(value != 0); e->graph_ready = false; return BRE_OK; }
   if (n == "overlap_wgrad") { e->overlap_wgrad = value != 0; e->graph_ready = false; return BRE_OK; }
   if (n == "fuse_bnact") { e->fuse_bnact = value != 0; e->graph_ready = false; return BRE_OK; }
+  if (n == "debug_multistep_stop") {
+    if (value < 0 || value > 2LL * e->ms_steps) { set_error("debug_multistep_stop must be in [0, 2 * local steps]"); return BRE_ERR_INVALID; }
+    e->debug_ms_stop = (int)value; return BRE_OK;
+  }
   if (n == "precise_first" || n == "precise_last") {
     (n == "precise_first" ? e->precise_first : e->precise_last) = (int)value;
     e->precise_op.clear(); e->rnd_val.clear(); e->rnd_d.clear(); e->chunk_mode_ready = false; e->graph_ready = false;

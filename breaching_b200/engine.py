@@ -78,7 +78,7 @@ EXPORTS = [
     "bre_engine_load_feature_targets", "bre_engine_set_local_steps", "bre_engine_begin_trial", "bre_engine_run", "bre_engine_run_timed", "bre_engine_sync",
     "bre_engine_status", "bre_engine_read_history", "bre_engine_get_best", "bre_engine_get_candidate",
     "bre_engine_score", "bre_engine_objective_and_gradient", "bre_engine_last_terms", "bre_engine_debug_param",
-    "bre_engine_debug_tensor", "bre_engine_debug_op", "bre_engine_launches_per_iteration", "bre_engine_set_option", "bre_match_reduce",
+    "bre_engine_debug_step_param", "bre_engine_debug_tensor", "bre_engine_debug_op", "bre_engine_launches_per_iteration", "bre_engine_set_option", "bre_match_reduce",
     "bre_total_variation", "bre_conv_gemm", "bre_last_error", "bre_version",
     "bre_engine_load_soft_labels", "bre_engine_label_gradient", "bre_engine_set_labels",
     "bre_token_layernorm", "bre_token_attention", "bre_token_match",
@@ -125,6 +125,7 @@ def load_library(path=None):
     lib.bre_engine_objective_and_gradient.argtypes = [vp, vp, P(ctypes.c_double), vp]
     lib.bre_engine_last_terms.argtypes = [vp, P(ctypes.c_double)]
     lib.bre_engine_debug_param.argtypes = [vp, i32, i32, vp]
+    lib.bre_engine_debug_step_param.argtypes = [vp, i32, i32, i32, vp]
     lib.bre_engine_debug_tensor.argtypes = [vp, i32, i32, vp]
     lib.bre_engine_debug_op.argtypes = [vp, i32, P(i32)]
     lib.bre_engine_launches_per_iteration.argtypes = [vp, P(i32)]
@@ -452,6 +453,8 @@ class Engine:
         return out.value
 
     def objective_and_gradient(self, candidate):
+        """(objective, d objective / d candidate) of one evaluation without an optimiser step.  With the option
+        ``debug_multistep_stop`` set the evaluation stops part-way and neither return value is meaningful."""
         cand = _f32c(candidate)
         if cand.is_cuda:
             torch.cuda.synchronize(self.device)
@@ -523,6 +526,15 @@ class Engine:
         # "v_operand" / "W_operand": what the GEMMs read (the TF32 shadow for tensor-core layers; "v" is stale for those)
         code = {"G": 0, "v": 1, "W": 2, "g": 3, "v_operand": 4, "W_operand": 5}[which]
         _check(self.lib, self.lib.bre_engine_debug_param(self.h, code, index, _ptr(out)), "bre_engine_debug_param")
+        return out
+
+    def debug_step_param(self, which, step, index):
+        """Multi-step engines: "W" = W_step, "W_operand" = W_step as the GEMMs read it, "D" = the accumulated W_K - W_0 (``step``
+        ignored); which of them are valid at which ``debug_multistep_stop`` is listed in include/breaching_b200.h."""
+        p = self.prog.params[index]
+        out = torch.empty(p.shape, dtype=torch.float32)
+        code = {"W": 0, "W_operand": 1, "D": 2}[which]
+        _check(self.lib, self.lib.bre_engine_debug_step_param(self.h, code, int(step), index, _ptr(out)), "bre_engine_debug_step_param")
         return out
 
     def debug_tensor(self, which, tid):

@@ -175,6 +175,19 @@ int bre_engine_last_terms(bre_engine* e, double* terms6);
  * only, so which = 1 returns stale memory for them; which = 4 / 5 return the TF32 shadow for those weights and the fp32
  * arena for every other parameter. */
 int bre_engine_debug_param(bre_engine* e, int32_t which, int32_t index, float* out_host);
+/* Multi-step engines: the local weights W_k of step `step` (0..K), torch layout like bre_engine_debug_param; which: 0 = W_k (fp32),
+ * 1 = W_k as the GEMMs read it (its TF32 shadow for the weights of tensor-core layers), 2 = D = W_K - W_0 as accumulated
+ * (`step` ignored).  W_0 is always valid.  W_{k+1}, its shadow and D_{k+1} are written by step k's update: valid after a full
+ * evaluation, or after one stopped at debug_multistep_stop >= k + 1 (for D: exactly k + 1, or any reverse stop for D_K).
+ *
+ * Option "debug_multistep_stop" (bre_engine_set_option, default 0 = off) stops bre_engine_objective_and_gradient inside a
+ * multi-step evaluation.  s = k + 1 (1 <= s <= K): after step k's forward and backward sweeps and its W_{k+1} / D updates;
+ * step k stays bound: activations, deltas, probabilities, labels, W = W_k and G = G_k (bre_engine_debug_tensor / debug_param).
+ * s = K + 1 + k: after step k's tangent-forward and tangent-backward sweeps, before its candidate-gradient axpy and adjoint
+ * update; v and its TF32 shadow hold the direction u_{k+1} that step k used, G holds the tangent weight gradient H_k u_{k+1}
+ * (k > 0 only) and the tangent delta of tensor 0 is the step's input gradient.  The value and gradient returned by a stopped
+ * evaluation are not meaningful.  bre_engine_run refuses while a stop is set. */
+int bre_engine_debug_step_param(bre_engine* e, int32_t which, int32_t step, int32_t index, float* out_host);
 /* which: 0 = activation, 1 = delta (sweep B), 2 = tangent, 3 = tangent delta; NCHW fp32 to host.  Tensor 0 (the candidate)
  * has no tangent; its delta is the task-loss gradient and its tangent delta the candidate gradient.  With fuse_bnact, the
  * tangent of a conv output whose only consumer is the BN op fused into the conv's epilogue is not written in single-step

@@ -199,7 +199,9 @@ class ProgramInterpreter:
         * ``V is None``: ordinary backward (sweep B): returns parameter gradients ``G``, saves deltas.
         * ``V`` given (sweep TB): propagates tangent deltas; the additional ``v``-terms use the deltas
           ``d_prev`` saved by sweep B;  ``inject[tid]`` tensors (regulariser adjoints) are added to the
-          stream when that tensor's delta is consumed.
+          stream when that tensor's delta is consumed.  With ``want_G`` it also returns the tangent of every parameter gradient
+          (the Hessian-vector product ``H v`` of the multi-step adjoint, sweep "TG"): conv / linear ``wgrad(a, d_T) + wgrad(a', d_B)``
+          (``a' = 0`` for the candidate), bias ``sum d_T``, eval-mode BN gamma ``sum (du_T xh + du_B x' inv)`` and beta ``sum du_T``.
         """
         prog = self.prog
         d = {prog.logits: seed.view(seed.shape[0], -1, 1, 1)}
@@ -213,12 +215,17 @@ class ProgramInterpreter:
             if self.tamper is not None:
                 d[tid] = self.tamper("B" if V is None else "TB", i, tid, d[tid], contribution=val)
 
+        def put_tg(idx, val):
+            G[idx] = val if self.tamper is None else self.tamper("TG", i, idx, val)
+
         for i in reversed(range(len(prog.ops))):
             op = prog.ops[i]
             dout = d[op.tout]
             if inject is not None and op.tout in inject:
                 dout = dout + inject[op.tout]
             xin = self.a[op.tin]
+            if V is not None and want_G:
+                self._tangent_param_grads(i, op, dout, d_prev, put_tg)
             if op.kind == C.OP_CONV:
                 if V is None:
                     if want_G:
@@ -331,6 +338,36 @@ class ProgramInterpreter:
                     add(op.tin, (do2 @ self.P[op.w] + dprev2 @ V[op.w]).view_as(xin))
         return d, G, du_saved
 
+    def _tangent_param_grads(self, i, op, dout, d_prev, put):
+        """Tangent of op ``i``'s parameter gradients (see ``_reverse``); ``dout`` is the tangent delta of its output."""
+        xin, xd = self.a[op.tin], self.ta.get(op.tin)
+        if op.kind == C.OP_CONV:
+            Gw = torch.nn.grad.conv2d_weight(xin, self.P[op.w].shape, dout, stride=op.stride, padding=op.pad)
+            if xd is not None:
+                Gw = Gw + torch.nn.grad.conv2d_weight(xd, self.P[op.w].shape, d_prev[op.tout], stride=op.stride, padding=op.pad)
+            put(op.w, Gw)
+            if op.b >= 0:
+                put(op.b, dout.sum(dim=(0, 2, 3)))
+        elif op.kind == C.OP_LINEAR:
+            do2 = dout.view(dout.shape[0], -1)
+            Gw = do2.t() @ self._flat_in(op, xin)
+            if xd is not None:
+                Gw = Gw + d_prev[op.tout].view(dout.shape[0], -1).t() @ self._flat_in(op, xd)
+            put(op.w, Gw)
+            if op.b >= 0:
+                put(op.b, do2.sum(dim=0))
+        elif op.kind == C.OP_BNACT and op.has_bn:
+            if getattr(op, "bn_train", False):
+                raise NotImplementedError("tangent parameter gradients of train-mode BN")
+            mask = (self.a[op.tout] > 0).to(self.dtype) if op.relu else 1.0
+            _, inv = self._bn_consts(i, op)
+            duT, duB = dout * mask, self.du_B[i]
+            xdot = xd if xd is not None else torch.zeros_like(xin)
+            put(op.gamma, (duT * self.aux[i] + duB * xdot * inv).sum(dim=(0, 2, 3)))
+            put(op.beta, duT.sum(dim=(0, 2, 3)))
+        elif op.kind in (C.OP_POSADD, C.OP_LAYERNORM):
+            raise NotImplementedError("tangent parameter gradients of token ops")
+
     def backward(self, want_dx=False):
         n = self.p.shape[0]
         if getattr(self.prog, "seq_len", 0):
@@ -399,7 +436,8 @@ class ProgramInterpreter:
         self.ta = ta
         return ta
 
-    def tangent_backward(self, V, inject=None):
+    def tangent_backward(self, V, inject=None, want_G=False):
+        """Tangent delta of the candidate; with ``want_G`` the pair (that, tangent parameter gradients), also kept as ``TG``."""
         n = self.p.shape[0]
         zdot = self.ta[self.prog.logits].view(n, -1)
         p = self.p
@@ -407,7 +445,7 @@ class ProgramInterpreter:
             T = self.prog.seq_len
             centred = (zdot - (p * zdot).sum(dim=1, keepdim=True)) * self.row_keep
             seed = p * centred / self.M
-            d, _, _ = self._reverse(seed, V=V, d_prev=self.d_B, inject=inject)
+            d, _, _ = self._reverse(seed, V=V, d_prev=self.d_B, inject=inject, want_G=False)
             # d objective / d (target probabilities): row (b, t) receives the term of the logits row (b, t - 1)
             dq = torch.zeros_like(centred)
             dq[1:] = -centred[:-1] / self.M
@@ -415,8 +453,11 @@ class ProgramInterpreter:
             self.d_T, self.inject = d, inject or {}
             return d[0].flatten(1).view(n // T, T, -1)
         seed = (p * zdot - p * (p * zdot).sum(dim=1, keepdim=True)) / n
-        d, _, _ = self._reverse(seed, V=V, d_prev=self.d_B, inject=inject)
+        d, TG, _ = self._reverse(seed, V=V, d_prev=self.d_B, inject=inject, want_G=want_G)
         self.d_T, self.inject = d, inject or {}
+        if want_G:
+            self.TG = TG
+            return d[0], TG
         return d[0]
 
     # ------------------------------------------------------------------ regulariser adjoints
@@ -466,6 +507,89 @@ class ProgramInterpreter:
             val = val + task_regularization * loss
             dx = dx + task_regularization * self.d_B[0].reshape(dx.shape)
         return val, dx, loss, G
+
+
+def image_prior(x, obj):
+    """(value, d value / d x) of the TV / norm priors of a sweep-checker objective dict (``tests/helpers.sweep_objective``)."""
+    from oracle import restate
+
+    xd = x.detach().clone().requires_grad_(True)
+    val = xd.sum() * 0
+    if obj.get("tv") is not None:
+        tv = obj["tv"]
+        val = val + restate.total_variation(xd, scale=tv["scale"], inner_exp=tv.get("inner_exp", 1), outer_exp=tv.get("outer_exp", 1),
+                                            double_opponents=tv.get("double_opponents", False), eps=tv.get("eps", 1e-8))
+    if obj.get("norm") is not None:
+        val = val + restate.norm_regularization(xd, scale=obj["norm"]["scale"], pnorm=obj["norm"].get("p", 2.0))
+    (gp,) = torch.autograd.grad(val, xd)
+    return val.detach(), gp
+
+
+class MultiStepInterpreter:
+    """The multi-step (FedAvg) evaluation as the engine computes it (``evaluate_multistep``; reference
+    ``_grad_fn_multi_step``, objectives.py:48-72): K forward / backward passes, step k on the candidate slice starting at image
+    ``k * dps mod N`` with weights W_k and labels ``labels[k]``; ``W_{k+1} = W_k - lr G_k`` and ``D_{k+1} = D_k - lr G_k``
+    accumulated directly; ``v = objective_direction(D_K, g)``; then the reverse loop ``u_K = v``, ``gradx[slice k] += -lr
+    TB_k(u_{k+1})``, ``u_k = u_{k+1} - lr H_k u_{k+1}`` (the tangent parameter gradients of step k, k > 0); the priors act on the
+    whole candidate.  Every step keeps its ``ProgramInterpreter`` (``steps[k]``, with ``U`` = the direction it used, ``gx`` =
+    its tangent input gradient and ``TG`` for k > 0).
+
+    ``tamper(step, sweep, op_index, key, stored, contribution=None)`` sees every sweep's stores as in ``ProgramInterpreter``
+    (including "TG") and the glue: "W" (``stored`` = W_{k+1}, ``contribution`` = G_k), "U" (u_k, contribution = the tangent
+    parameter gradients used) and "GX" (the candidate-gradient slice after step k's accumulation, contribution = step k's term);
+    it returns what is stored instead."""
+
+    tamper = None
+
+    def __init__(self, model, prog, lr, dtype=torch.float64):
+        self.model, self.prog, self.lr, self.dtype = model, prog, lr, dtype
+
+    def _hook(self, k):
+        if self.tamper is None:
+            return None
+        return lambda *a, **kw: self.tamper(k, *a, **kw)
+
+    def _glue(self, k, sweep, key, stored, contribution):
+        return stored if self.tamper is None else self.tamper(k, sweep, -1, key, stored, contribution=contribution)
+
+    def run(self, x, labels, g, obj):
+        """``x``: the whole candidate; ``labels``: one label tensor per step; ``obj``: sweep-checker objective dict (kind, scale,
+        tv, norm).  Returns (objective value, candidate gradient)."""
+        lr, K = self.lr, len(labels)
+        x = x.to(self.dtype)
+        dps, N = self.prog.tensors[0].N, x.shape[0]
+        self.steps, self.offsets, seen = [], [], 0
+        W = [p.detach().to(self.dtype) for p in self.model.parameters()]
+        self.W, self.D = [W], [[torch.zeros_like(w) for w in W]]
+        for k in range(K):
+            it = ProgramInterpreter(self.model, self.prog, self.dtype)
+            it.P, it.tamper = self.W[k], self._hook(k)
+            self.offsets.append(seen)
+            it.forward(x[seen:seen + dps], labels[k])
+            seen = (seen + dps) % N
+            G = it.backward()
+            self.W.append(self._glue(k, "W", None, [w - lr * gk for w, gk in zip(self.W[k], G)], G))
+            self.D.append([d - lr * gk for d, gk in zip(self.D[k], G)])
+            self.steps.append(it)
+        gg = [t.to(self.dtype) for t in g]
+        kw = {k_: obj[k_] for k_ in ("tag_scale", "scale_scheme") if k_ in obj}
+        val, u = objective_direction(obj["kind"], self.D[K], gg, scale=obj.get("scale", 1.0), **kw)
+        self.V = u
+        grad = torch.zeros_like(x)
+        for k in reversed(range(K)):
+            it, o = self.steps[k], self.offsets[k]
+            it.U = u
+            it.tangent_forward(u)
+            if k > 0:
+                it.gx, TG = it.tangent_backward(u, want_G=True)
+            else:
+                it.gx = it.tangent_backward(u)
+            term = -lr * it.gx
+            grad[o:o + dps] = self._glue(k, "GX", o, grad[o:o + dps] + term, term)
+            if k > 0:
+                u = self._glue(k, "U", None, [a - lr * b for a, b in zip(u, TG)], TG)
+        pv, gp = image_prior(x, obj)
+        return val + pv, grad + gp
 
 
 def _maxpool_scatter(dout, idx, in_shape):

@@ -43,6 +43,25 @@ Token programs (``compiler.compile_transformer``: tensors are [rows = B x T, C, 
   * ``check_label_gradient``: d objective / d target probabilities, ``-(zdot - <p, zdot>) / M - tau (z - lse) / M`` of the
     source row (row (b, t - 1) for tokens, 0 at t = 0), bounded like the seeds.
 
+Multi-step (FedAvg) evaluations (``MultiStepChecker``; the engine's ``evaluate_multistep``, ``MultiStepInterpreter``): every
+local step k is checked as a single step, with W_k as the parameters (the BN constants follow from it), step k's labels, the
+direction u_{k+1} that step k used as ``v``, and no priors or task term in its candidate-gradient relation (that buffer is the
+step's own input gradient).  In addition:
+
+  * sweep ``TG`` (steps k > 0): the tangent parameter gradients ``H_k u_{k+1}``.  Conv / linear weights
+    ``wgrad(a, d_T) + wgrad(a', d_B)`` (one source for the candidate-fed layer) with the GEMM bound ``(K_total + 2) 2^-23`` of
+    ``|A| * |B|`` summed over both sources, on the operands the kernel read (stored values; the candidate rounded to TF32 on the
+    stem column path; an off-grid activation or tangent of a tensor-core layer widened as for sweep B); biases ``sum d_T`` and the
+    eval-mode BN tangents (gamma ``sum (du_T xh + du_B x' inv)``, beta ``sum du_T``, ``du`` the ReLU-masked deltas, ``x'`` the
+    pre-BN tangent) with the reduction bound ``(P + 4) 2^-23 sum |terms|`` (2P terms for gamma);
+  * the glue, each one rounding of an fp32 axpby with the step size the engine applied (its fp32 value):
+    ``W_{k+1} = W_k - lr G_k``, ``D_{k+1} = D_k - lr G_k`` and the adjoint update ``u_k = u_{k+1} - lr TG_k``, each within
+    ``2u (|a| + |lr b|)``; the TF32 operand forms of W_k and u_k equal ``rna`` of their fp32 values exactly (shadowed weights) or
+    the values themselves; ``v = make_v(D_K, g)`` is the direction relation above with ``G := D_K``;
+  * the final candidate gradient: ``sum_k -lr gradx_step_k`` scattered onto step k's slice (the slices of steps that wrap
+    around the images accumulate), ``(n + 2) 2^-23 sum |terms|`` for n contributions to an element, plus the TV / norm priors on
+    the whole candidate with the prior bound of the single-step relation.
+
 ``delta[t]`` / ``tangent_delta[t]`` are checked as the sum over *all* consumers of ``t`` (residual branches included), which
 judges the accumulation flags; such a failure is reported at the consumer that runs last in the reverse sweep (the one with
 the lowest op index), where the buffer becomes final.
@@ -50,7 +69,7 @@ the lowest op index), where the buffer becomes final.
 The vision cross-entropy seed takes soft targets (a float ``labels`` tensor [N, classes]) as well as class indices.
 
 A buffer source provides ``tensor(which, tid)`` (``which`` in val / delta / tangent / tangent_delta, NCHW, ``None`` where a
-tensor has no such buffer), ``param(which, index)`` (G / v_operand / W_operand, torch layout), ``unwritten`` (tensor ids whose
+tensor has no such buffer), ``param(which, index)`` (G / v_operand / W_operand, torch layout; multi-step steps also v and TG), ``unwritten`` (tensor ids whose
 tangent is not stored because the BN op reading it ran in the producing GEMM's epilogue; that pair is then checked as one)
 and ``rounds_operands(op_index)``.
 """
@@ -82,12 +101,14 @@ def on_grid(t):
 
 
 class Finding:
-    def __init__(self, op, kind, sweep, what, index, value, ref, err, bound):
+    def __init__(self, op, kind, sweep, what, index, value, ref, err, bound, step=None):
         self.op, self.kind, self.sweep, self.what = op, kind, sweep, what
         self.index, self.value, self.ref, self.err, self.bound = index, value, ref, err, bound
+        self.step = step   # local step of a multi-step evaluation (None: single step, or a relation over all steps)
 
     def __repr__(self):
-        return (f"op {self.op} ({self.kind}), sweep {self.sweep}, {self.what}: worst element {self.index} = {self.value:.9g}, "
+        at = "" if self.step is None else f"step {self.step}, "
+        return (f"{at}op {self.op} ({self.kind}), sweep {self.sweep}, {self.what}: worst element {self.index} = {self.value:.9g}, "
                 f"reference {self.ref:.9g}, error {self.err:.3g} > bound {self.bound:.3g}")
 
 
@@ -311,9 +332,56 @@ class SweepChecker:
         self.direction()
         self.tangent_forward()
         self.tangent_backward()
+        if getattr(self.src, "has_tangent_G", False):
+            self.tangent_G()
         if raise_on_failure and self.findings:
             raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
         return self.findings
+
+    def tangent_G(self):
+        """Sweep TG: the tangent parameter gradients ``param("TG", j)`` of a multi-step step k > 0 (see module docstring).
+        Run after ``tangent_forward`` (a tangent the engine did not store is taken from its reference)."""
+        for i, op in enumerate(self.prog.ops):
+            dT = self.T("tangent_delta", op.tout)
+            if op.kind in (C.OP_CONV, C.OP_LINEAR):
+                a, _, _ = self._operands(i, op)
+                TGw = self.Pm("TG", op.w)
+                ref, mag = self._gemm_wgrad(op, a, TGw.shape, dT), self._gemm_wgrad(op, a.abs(), TGw.shape, dT.abs())
+                K, trunc = self._K(op, "wgrad"), self._truncation(i, op, a)
+                if op.tin != 0:
+                    ad = self._tangent_in(op)
+                    if self.src.rounds_operands(i):
+                        ad = rna(ad)
+                    dB = self.T("delta", op.tout)
+                    ref = ref + self._gemm_wgrad(op, ad, TGw.shape, dB)
+                    mag = mag + self._gemm_wgrad(op, ad.abs(), TGw.shape, dB.abs())
+                    K, trunc = 2 * K, max(trunc, self._truncation(i, op, ad))
+                self._cmp(i, "TG", f"TG[{op.w}] (tangent weight gradient)", TGw, ref, ((K + 2) * U2 + trunc) * mag)
+                if op.b >= 0:
+                    P_ = dT.shape[0] * dT.shape[2] * dT.shape[3]
+                    self._cmp(i, "TG", f"TG[{op.b}] (tangent bias gradient)", self.Pm("TG", op.b), dT.sum(dim=(0, 2, 3)),
+                              (P_ + 4) * U2 * dT.abs().sum(dim=(0, 2, 3)))
+            elif op.kind == C.OP_BNACT and op.has_bn:
+                if op.bn_train:
+                    raise NotImplementedError("tangent parameter gradients of train-mode BN")
+                x = self.T("val", op.tin)
+                mask = (self.T("val", op.tout) > 0).double() if op.relu else torch.ones_like(dT)
+                duT, duB = dT * mask, self.T("delta", op.tout) * mask
+                rm, inv, _, _ = self._bn_eval(i, op)
+                xh, xhm = (x - rm) * inv, (x * inv).abs() + (rm * inv).abs()
+                xd = self._tangent_in(op)
+                Pch = x.shape[0] * x.shape[2] * x.shape[3]
+                s = (duT.abs() * xhm + duB.abs() * xd.abs() * inv).sum(dim=(0, 2, 3))
+                self._cmp(i, "TG", f"TG[{op.gamma}] (BN gamma tangent)", self.Pm("TG", op.gamma),
+                          (duT * xh + duB * xd * inv).sum(dim=(0, 2, 3)), (2 * Pch + 4) * U2 * s)
+                self._cmp(i, "TG", f"TG[{op.beta}] (BN beta tangent)", self.Pm("TG", op.beta), duT.sum(dim=(0, 2, 3)),
+                          (Pch + 4) * U2 * duT.abs().sum(dim=(0, 2, 3)))
+
+    def _tangent_in(self, op):
+        """The stored tangent of op's input (its reference where the engine did not store it)."""
+        if op.tin in self.src.unwritten:
+            return self._tf_override[op.tin][0]
+        return self.T("tangent", op.tin)
 
     def forward(self):
         prog = self.prog
@@ -862,3 +930,160 @@ class InterpreterSource:
 
     def param(self, which, idx):
         return {"G": self.it.G, "v_operand": self.V, "W_operand": self.it.P}[which][idx]
+
+
+class InterpreterStepSource:
+    """Buffers of step k of a float64 ``program_interp.MultiStepInterpreter`` run, as the multi-step checker reads them."""
+
+    def __init__(self, mi, k):
+        self.it = mi.steps[k]
+        self.has_tangent_G = k > 0
+        self.unwritten = set()
+
+    def rounds_operands(self, i):
+        return False
+
+    def tensor(self, which, tid):
+        it = self.it
+        if which == "tangent_delta":
+            return it.gx if tid == 0 else it.d_T[tid]
+        return InterpreterSource.tensor(self, which, tid)
+
+    def param(self, which, idx):
+        it = self.it
+        return {"G": it.G, "v": it.U, "v_operand": it.U, "W_operand": it.P, "TG": getattr(it, "TG", None)}[which][idx]
+
+
+class InterpreterGlue:
+    """What the multi-step checker reads outside the steps, from a ``MultiStepInterpreter`` run: W_k / their operands (k = 0..K),
+    D_k (k = 1..K), the whole candidate and its final gradient."""
+
+    def __init__(self, mi, x, grad):
+        self.x, self.grad, self.offsets, self.lr = x, grad, mi.offsets, mi.lr
+        self.W, self.W_operand, self.D = mi.W, mi.W, {k: mi.D[k] for k in range(1, len(mi.D))}
+
+    def shadowed(self, j):
+        return False
+
+
+class MultiStepChecker:
+    """Layer-local check of every local step of a multi-step (FedAvg) evaluation, plus the glue between the steps.
+
+    ``sources[k]`` is step k's buffer source: its forward / backward buffers (``val``, ``delta``, ``G`` = G_k) and those of its
+    tangent sweeps (``tangent``, ``tangent_delta`` with the step's input gradient at tensor 0, ``v`` / ``v_operand`` = u_{k+1}, the
+    direction step k used, ``TG`` = H_k u_{k+1} for k > 0).  ``glue`` provides ``W[k]`` / ``W_operand[k]`` (k = 0..K, lists in
+    parameter order), ``D[k]`` (k = 1..K; missing entries are not checked), ``shadowed(j)`` (parameter j has a TF32 operand
+    form), ``x`` (the whole candidate), ``grad`` (its final gradient), ``offsets`` (first image of each step's slice) and ``lr``
+    (the step size as the source applied it: the engine's is the fp32 value).
+    ``labels[k]``: step k's labels; ``objective``: as for ``SweepChecker`` (the priors act on the final assembly only)."""
+
+    def __init__(self, prog, bn, g, labels, objective, sources, glue):
+        self.prog, self.bn, self.g, self.labels = prog, bn, [t.detach().double() for t in g], labels
+        self.obj, self.src, self.glue = objective, sources, glue
+        self.K = len(sources)
+        self.findings, self.ratios, self.off_grid = [], {}, set()
+
+    def _step_objective(self):
+        o = dict(self.obj)
+        o.update(tv=None, norm=None, di=None, features=None, task_regularization=0.0)
+        return o
+
+    def _absorb(self, chk, step):
+        for f in chk.findings:
+            f.step = step if f.step is None else f.step
+            self.findings.append(f)
+        for key, r in chk.ratios.items():
+            self.ratios[key] = max(self.ratios.get(key, 0.0), r)
+        chk.findings, chk.ratios = [], {}
+
+    def check(self, raise_on_failure=True):
+        n = len(self.g)
+        self.steps = []
+        for k in range(self.K):
+            W = [w.double() for w in self.glue.W[k]]
+            chk = SweepChecker(self.prog, W, self.bn, self.g, self.labels[k], self._step_objective(), self.src[k])
+            chk.forward()
+            chk.backward()
+            chk.tangent_forward()
+            chk.tangent_backward()
+            if k > 0:
+                chk.tangent_G()
+            self.off_grid.update({(k, i) for i in chk.off_grid})
+            self._absorb(chk, k)
+            self.steps.append(chk)
+        self.glue_relations(n)
+        if raise_on_failure and self.findings:
+            raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
+        return self.findings
+
+    def _cmp(self, step, sweep, what, y, ref, bound):
+        chk = self.steps[0]
+        chk._cmp(-1, sweep, what, y.double(), ref, bound, kind="glue")
+        self._absorb(chk, step)
+
+    def glue_relations(self, n):
+        lr, K, gl = self.glue.lr, self.K, self.glue
+        G = [[self.src[k].param("G", j).double() for j in range(n)] for k in range(K)]
+        for k in range(K):
+            for j in range(n):
+                # W_{k+1} = fl(W_k - lr G_k) (fp32 lr; one product, one sum); its TF32 operand form is rna(W_{k+1}) exactly
+                Wk, Wn = gl.W[k][j].double(), gl.W[k + 1][j].double()
+                step = lr * G[k][j]
+                self._cmp(k, "W", f"W_{k + 1}[{j}] = W_{k} - lr G_{k}", Wn, Wk - step, 2 * U * (Wk.abs() + step.abs()))
+                Wo = gl.W_operand[k + 1][j].double()
+                self._cmp(k, "Wt", f"W_operand_{k + 1}[{j}] (TF32 shadow)", Wo, rna(Wn) if gl.shadowed(j) else Wn, 0.0)
+                if k + 1 in gl.D and (k == 0 or k in gl.D):
+                    Dk = gl.D[k][j].double() if k > 0 else torch.zeros_like(Wk)
+                    Dn = gl.D[k + 1][j].double()
+                    self._cmp(k, "D", f"D_{k + 1}[{j}] = D_{k} - lr G_{k}", Dn, Dk - step, 2 * U * (Dk.abs() + step.abs()))
+        # the direction of the last step: make_v(D_K, g), the direction relation of the single-step check with G := D_K
+        last = self.K - 1
+
+        class _DirSource:
+            def __init__(s, base):
+                s.base = base
+
+            def param(s, which, idx):
+                return gl.D[K][idx] if which == "G" else s.base.param(which, idx)
+
+        d = SweepChecker(self.prog, [w.double() for w in gl.W[0]], self.bn, self.g, self.labels[0], self.obj, _DirSource(self.src[last]))
+        d.direction()
+        for f in d.findings:
+            f.step = last
+        self.findings += d.findings
+        for key, r in d.ratios.items():
+            self.ratios[key] = max(self.ratios.get(key, 0.0), r)
+        for k in range(K):
+            u = [self.src[k].param("v", j).double() for j in range(n)]
+            for j in range(n):   # the TF32 shadow of the direction step k used
+                uo = self.src[k].param("v_operand", j).double()
+                self._cmp(k, "Ut", f"v_operand[{j}] (TF32 shadow of u_{k + 1})", uo, rna(u[j]) if gl.shadowed(j) else u[j], 0.0)
+            if k == 0:
+                continue
+            # u_k = fl(u_{k+1} - lr H_k u_{k+1}): the direction step k - 1 used
+            un = [self.src[k - 1].param("v", j).double() for j in range(n)]
+            for j in range(n):
+                step = lr * self.src[k].param("TG", j).double()
+                self._cmp(k, "U", f"u_{k}[{j}] = u_{k + 1} - lr TG_{k}", un[j], u[j] - step, 2 * U * (u[j].abs() + step.abs()))
+        self._final_assembly()
+
+    def _final_assembly(self):
+        """gradx = sum_k -lr gradx_step_k scattered onto step k's slice (slices of wrapped steps accumulate) + the priors."""
+        gl, lr = self.glue, self.glue.lr
+        x = gl.x.double()
+        ref, mag, cnt = torch.zeros_like(x), torch.zeros_like(x), torch.zeros_like(x)
+        for k in range(self.K):
+            gs = lr * self.src[k].tensor("tangent_delta", 0).double()
+            o, b = gl.offsets[k], gs.shape[0]
+            ref[o:o + b] -= gs
+            mag[o:o + b] += gs.abs()
+            cnt[o:o + b] += 1
+        bound = (cnt + 2) * U2 * mag
+        o = self.obj
+        if o.get("tv") is not None or o.get("norm") is not None:
+            from oracle.program_interp import image_prior
+            _, gp = image_prior(x, o)
+            ref = ref + gp
+            tvs = o["tv"]["scale"] if o.get("tv") is not None else 0.0
+            bound = bound + 64 * U * (gp.abs() + 4 * tvs / x.numel())
+        self._cmp(None, "GX", "candidate gradient (sum over the local steps + priors)", gl.grad.double(), ref, bound + U * ref.abs())

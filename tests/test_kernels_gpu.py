@@ -206,8 +206,8 @@ def test_tall_linear_dgrad_matches_float64(rows, Ci, Co, dual):
 @pytest.mark.parametrize("rows,Ci,Co", [(32, 96, 288), (32, 96, 1536), (20, 96, 96), (32, 1536, 96), (1, 512, 397), (8, 2048, 397)])
 def test_small_row_linear_kernels_match_float64(rows, Ci, Co):
     """Linear layers on <= 32 rows (classification heads, token-model projections at batch 1) through the engine's dispatch rule
-    (`bre_conv_gemm` backend 2: matrix-vector kernels for short reductions, the GEMM back ends otherwise): fprop / dgrad with one and
-    two sources and wgrad against float64."""
+    (`bre_conv_gemm` backend 2: matrix-vector kernels for short reductions, the GEMM back ends otherwise): fprop / dgrad / wgrad with
+    one and two sources against float64."""
     from breaching_b200 import engine as E
 
     dev = torch.device("cuda:0")
@@ -234,3 +234,6 @@ def test_small_row_linear_kernels_match_float64(rows, Ci, Co):
         dw = torch.empty(Co, Ci, device=dev)
         E.conv_gemm(2, x, dy, dw, *geom, backend=backend)
         assert rel(dw, dy.double().T @ x.double()) < tol, ("wgrad", backend)
+        # two sources: the tangent weight gradient of a FedAvg step, wgrad(a, d_T) + wgrad(a', d_B)
+        E.conv_gemm(2, x, dy, dw, *geom, a2=x2, w2=dy2, backend=backend)
+        assert rel(dw, dy.double().T @ x.double() + dy2.double().T @ x2.double()) < tol, ("wgrad2", backend)
