@@ -1160,8 +1160,20 @@ int launch_igemm_tc(const GemmArgs& a, cudaStream_t stream) {
     memset(&cmaps, 0, sizeof(cmaps));
     if (build_cls(a, &plan, &cmaps)) return launch_tc<GEMM_DGRAD, 64, true, true>(a, d, cmaps, stream, &plan);
   }
-  if (d.Nc % 64 != 0) {   // 128 x 32 tiles (TMA producer only, see igemm_tc_supported)
-    if (!build_maps(a, 32, &maps)) { set_error("igemm_tc: tensor-map encoding failed for a narrow-tile shape"); return -4; }
+  // 128 x 32 tiles: widths that are only a multiple of 32 (TMA producer only, see igemm_tc_supported), and data / weight gradients
+  // whose 128 x 64 tiles would fill at most half the SMs even at the full 8-CTA split while every CTA walks a long k-range (batch 1:
+  // ResNet-18's layer-3 / layer-4 dgrad, 8 tiles x 8 = 64 CTAs over 9-36 k-blocks each; the stem's column wgrad, 3 tiles x 49).
+  // Their mma.sync consumer (fragments loaded with ld.shared) bounds the k-loop; halving the tile width doubles the CTAs and halves
+  // each CTA's MMA and fragment-load work per k-block, while every output element keeps the same k-blocks per split, the same MMA
+  // accumulation chain and the same fixed-order cluster reduction: the result is bitwise the one of 128 x 64 tiles.  Both grids stay
+  // <= kNumSMs, so the split-K rule picks the same 8-way split for either.  Measured per launch on the H100 (scripts/profile_gemms.py,
+  // DESIGN.md section 6): dgrad 15-44 -> 10-32 us, the stem wgrad 44 -> 34 us; the wgmma fprop of the same shapes gained 0-2 us on
+  // some and lost 2 us on layer 4's, so it keeps 128 x 64 tiles.
+  const long long wide_tiles = (long long)ceil_div(d.M, TC_BM) * (d.Nc / 64);
+  const bool underfilled = a.mode != GEMM_FPROP && d.Nc % 64 == 0 && wide_tiles * 16 <= kNumSMs && d.total_kblocks >= 64 &&
+                           narrow_tiles_ok(a);
+  if (d.Nc % 64 != 0 || (underfilled && build_maps(a, 32, &maps))) {
+    if (d.Nc % 64 != 0 && !build_maps(a, 32, &maps)) { set_error("igemm_tc: tensor-map encoding failed for a narrow-tile shape"); return -4; }
     if (a.mode == GEMM_FPROP) return launch_tc<GEMM_FPROP, 32, true>(a, d, maps, stream);
     if (a.mode == GEMM_DGRAD) return launch_tc<GEMM_DGRAD, 32, true>(a, d, maps, stream);
     return launch_tc<GEMM_WGRAD, 32, true>(a, d, maps, stream);
