@@ -134,7 +134,8 @@ class OptimizationBasedAttacker:
         local = shared_data[index]["metadata"]["local_hyperparams"]
         model = rec_models[index]
         n = shared_data[index]["metadata"]["num_data_points"]
-        # FedAvg (objectives.py:48-72): the layer program is compiled for one local step's batch
+        # FedAvg (objectives.py:48-72): the layer program is compiled for one local step's batch.  task_regularization and
+        # deep_inversion act on the last local step; the features prior is refused by Engine.set_local_steps (see its docstring)
         shape = (n if local is None else int(local["data_per_step"]), *(self.data_shape if data_shape is None else data_shape))
         seed = int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if cfg_get(self.cfg.optim, "langevin_noise", 0.0) else 0
         if self._engine is not None and index == 0 and primary:

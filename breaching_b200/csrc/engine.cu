@@ -238,7 +238,7 @@ struct bre_engine {
     return 0;
   }
   int augment_pull() {   // gradx <- view^T (gradx_aug + task_regularization * gradx_task)
-    if (need_task_grad()) BRE_LAUNCH(launch_axpy(gradx_task, gradx_aug, cfg.task_regularization, nx, stream));
+    if (task_grad_from_backward()) BRE_LAUNCH(launch_axpy(gradx_task, gradx_aug, cfg.task_regularization, nx, stream));
     BRE_LAUNCH(launch_aug_pull(gradx_aug, aug_tmp, gradx, xN, xC, xH, xW, aug, aug_draws, stream));
     return 0;
   }
@@ -444,6 +444,9 @@ struct bre_engine {
     return PoolGeom{ti.N, ti.H, ti.W, ti.C, to.H, to.W, op.R, op.stride, op.pad};
   }
   bool need_task_grad() const { return cfg.task_regularization != 0.f; }
+  // single-step evaluations take task_regularization * dL/dx from sweep B's dgrad of the candidate-fed layer (gradx_task, added
+  // by the pixel kernel); a FedAvg evaluation seeds it into the last local step's tangent backward instead (prior_seed)
+  bool task_grad_from_backward() const { return need_task_grad() && ms_steps == 0; }
   float value_task_reg() const { return cfg.objective_excludes_task ? 0.f : cfg.task_regularization; }
 
   // ---- sweeps ---------------------------------------------------------------------------------------
@@ -552,7 +555,7 @@ struct bre_engine {
             if (cols) BRE_LAUNCH(launch_stem_pad_rows(Gcol, Gp(op.w), to.C, Kraw, stem_Kp, true, false, stream));
             if (op.b >= 0) BRE_LAUNCH(launch_channel_sum(t[op.tout].d, Pout, to.C, Gp(op.b), red_partials, red_counters, stream));
           }
-          if (op.tin != 0 || need_task_grad()) {
+          if (op.tin != 0 || task_grad_from_backward()) {
             GemmArgs b = cols ? stem_geom(op) : conv_geom(op);
             b.mode = GEMM_DGRAD;
             b.act[0] = t[op.tout].d; b.wgt[0] = cols ? Wcol : Wg(op);
@@ -597,7 +600,7 @@ struct bre_engine {
         }
         case BRE_OP_POSADD:      // gradient of the positional table; the candidate's own delta only for the task-loss term
           BRE_LAUNCH(launch_token_pos_grad(t[op.tout].d, Gp(op.w), to.N, to.C, op.S, stream));
-          if (need_task_grad())
+          if (task_grad_from_backward())
             BRE_CUDA_CHECK(cudaMemcpyAsync(t[0].d, t[op.tout].d, (size_t)to.N * to.C * sizeof(float), cudaMemcpyDeviceToDevice, stream));
           break;
         case BRE_OP_LAYERNORM:
@@ -713,18 +716,20 @@ struct bre_engine {
     return 0;
   }
 
-  // DeepInversion statistics of every BN input of this forward pass: one batched launch pair (layers.cu) + per-layer finalisation
+  // DeepInversion statistics of every BN input of this forward pass: one batched launch pair (layers.cu) + per-layer finalisation.
+  // FedAvg: the statistics of the last local step's forward (its saved activations).
   StatSlot* di_stat_slots = nullptr;
   double* di_layer_values = nullptr;
   int di_stat_blocks = 0, di_stat_groups = 0;
   bool di_batched = false, di_tables_built = false;
+  const float* di_input(const bre_op_desc& op) const { return ms_steps > 0 ? ms_bufs[ms_steps - 1].val[op.tin] : t[op.tin].val; }
   int build_di_tables() {
     if (di_tables_built) return 0;
     di_tables_built = true;
     if (cfg.di_scale <= 0.f || n_di == 0) return 0;
-    BRE_TRY(alloc(&di_layer_values, n_di));
+    if (!di_layer_values) BRE_TRY(alloc(&di_layer_values, n_di));
     static const bool env = [] { const char* e = getenv("BRE_DI_BATCHED"); return e ? atoi(e) != 0 : true; }();
-    if (!env || ms_steps > 0) return 0;
+    if (!env) return 0;
     std::vector<StatSlot> table;
     int blocks = 0, groups = 0;
     // one launch covers every BN input: ~16 blocks per SM in total, dealt to the tensors in proportion to their size
@@ -741,7 +746,7 @@ struct bre_engine {
       if (target < 4) target = 4;
       if (!channel_stats_plan((long long)ti.N * ti.H * ti.W, ti.C, &sl, target)) return 0;   // odd channel count somewhere: per-layer kernels
       BnBuf& b = bn[op.bn_buffer];
-      sl.x = t[op.tin].val; sl.mean = b.di_mean; sl.var = b.di_var;
+      sl.x = di_input(op); sl.mean = b.di_mean; sl.var = b.di_var;
       BRE_TRY(alloc(&sl.partials, (long long)sl.slabs * sl.Cpad * 2));
       sl.first_block = blocks; sl.first_group = groups;
       blocks += sl.cg * sl.slabs; groups += (ti.C + 255) / 256;
@@ -763,20 +768,28 @@ struct bre_engine {
         if (op.kind != BRE_OP_BNACT || !op.has_bn) continue;
         const bre_tensor_desc& ti = td(op.tin);
         BnBuf& b = bn[op.bn_buffer];
-        BRE_LAUNCH(launch_channel_stats(t[op.tin].val, (long long)ti.N * ti.H * ti.W, ti.C, b.di_mean, b.di_var, red_partials,
+        BRE_LAUNCH(launch_channel_stats(di_input(op), (long long)ti.N * ti.H * ti.W, ti.C, b.di_mean, b.di_var, red_partials,
                                         red_counters, stream));
       }
     }
-    BRE_LAUNCH(launch_di_finalize(di_layers_dev, n_di, di_layer_values, sc, stream));
+    // FedAvg: the adjoint seeds the last local step's tangent backward, scaled by -1/lr like every seed there
+    BRE_LAUNCH(launch_di_finalize(di_layers_dev, n_di, di_layer_values, sc, stream, ms_steps > 0 ? -1.0 / (double)ms_lr : 1.0));
     return 0;
   }
 
+  // FedAvg: set while the last local step's tangent backward runs.  Task-loss regularisation and DeepInversion read that step's
+  // forward, so their adjoints enter its tangent-backward stream as seeds scaled by -1/lr: the candidate axpy (-lr) turns them into
+  // d prior / d x_last, and the tangent parameter gradients carry -1/lr d prior / d W_last into the adjoint update (DESIGN.md 3.1).
+  bool prior_seed = false;
   int sweep_tangent_backward() {
     bool forked = false;
     const bre_tensor_desc& lt = td(logits);
     if (seq_len > 0) BRE_LAUNCH(launch_token_ce_tan_bwd(p, t[logits].tval, lt.N, classes(), lt.C, seq_len, t[logits].td, round_d(logits), stream));
+    else if (prior_seed && need_task_grad())
+      BRE_LAUNCH(launch_ce_tan_bwd_seeded(p, t[logits].tval, labels, lt.N, lt.C, -cfg.task_regularization / ms_lr, t[logits].td,
+                                          round_d(logits), stream));
     else BRE_LAUNCH(launch_ce_tan_bwd(p, t[logits].tval, lt.N, lt.C, t[logits].td, stream));
-    const bool di = cfg.di_scale > 0.f && n_di > 0;
+    const bool di = cfg.di_scale > 0.f && n_di > 0 && (ms_steps == 0 || prior_seed);
     for (int i = (int)ops.size() - 1; i >= 0; --i) {
       const bre_op_desc& op = ops[i];
       const bre_tensor_desc& to = td(op.tout);
@@ -911,12 +924,16 @@ struct bre_engine {
     BRE_LAUNCH(launch_make_v(ms_D, g, chunk_w, V, P_pad, mv, sc, stream));          // adjoint of W_K
     BRE_TRY(refresh_Vt());
     const long long nstep = t[0].numel;
-    for (int k = ms_steps - 1; k >= 0; --k) {
+    const int last = ms_steps - 1;
+    for (int k = last; k >= 0; --k) {
       bind_step(k);
       want_tangent_G = k > 0;
+      prior_seed = k == last;
+      if (k == last) BRE_TRY(deep_inversion_stats());   // statistics of the last step's forward (no launch without the prior)
       BRE_TRY(sweep_tangent_forward());
       const int rc = sweep_tangent_backward();
       want_tangent_G = false;
+      prior_seed = false;
       if (rc != 0) return rc;
       if (debug_ms_stop == ms_steps + 1 + k) return 0;
       // d Phi / d x_k = -lr * d/d eps grad_x L(x_k, W_{k-1} + eps u_k)
@@ -978,7 +995,8 @@ struct bre_engine {
 
   StepArgs step_args() const {
     StepArgs a;
-    a.x = x; a.m = m; a.v = v; a.best = best; a.grad = gradx; a.grad_task = (need_task_grad() && !task_grad_folded()) ? gradx_task : nullptr;
+    a.x = x; a.m = m; a.v = v; a.best = best; a.grad = gradx;
+    a.grad_task = (task_grad_from_backward() && !task_grad_folded()) ? gradx_task : nullptr;
     a.lr_table = lr_table; a.n_lr = n_lr; a.lo = lo; a.hi = hi; a.n = nx; a.C = xC; a.HW = xH * xW; a.cfg = cfg;
     return a;
   }
@@ -1368,9 +1386,15 @@ int bre_engine_set_local_steps(bre_engine* e, int32_t total_images, int32_t step
   if (e->ms_steps > 0) { set_error("local steps already configured"); return BRE_ERR_STATE; }
   for (const bre_op_desc& o : e->ops)
     if (o.kind == BRE_OP_BNACT && o.has_bn && o.bn_train) { set_error("multi-step updates with train-mode BatchNorm are not implemented"); return BRE_ERR_UNSUPPORTED; }
-  if (e->cfg.task_regularization != 0.f || e->cfg.di_scale > 0.f || e->cfg.feat_scale > 0.f) {
-    set_error("task regularisation / DeepInversion / feature priors are not implemented for multi-step updates "
-              "(the reference crashes on the latter two, SURVEY.md section 0 fact 9)");
+  if (e->cfg.feat_scale > 0.f) {
+    set_error("the feature prior is not defined for multi-step updates: its target W_g[y] / b_g[y] is the input feature of one "
+              "forward pass only when the shared update is a single gradient; W_K - W_0 sums K local steps with different "
+              "activations, so the ratio is the feature of no forward pass");
+    return BRE_ERR_UNSUPPORTED;
+  }
+  if ((e->cfg.task_regularization != 0.f || e->cfg.di_scale > 0.f) && !(lr != 0.f)) {
+    set_error("task regularisation / DeepInversion with multi-step updates need a nonzero local learning rate: their adjoints "
+              "enter the last local step's tangent backward scaled by -1/lr");
     return BRE_ERR_UNSUPPORTED;
   }
   BRE_CUDA_CHECK(cudaSetDevice(e->device));
@@ -1433,6 +1457,8 @@ int bre_engine_set_local_steps(bre_engine* e, int32_t total_images, int32_t step
   e->ms_steps = steps;
   e->ms_lr = lr;
   e->bind_step(0);
+  e->di_tables_built = false;   // the DeepInversion statistics now read the last local step's activations
+  e->di_batched = false;
   e->graph_ready = false;
   return BRE_OK;
 }
@@ -1634,7 +1660,7 @@ int bre_engine_objective_and_gradient(bre_engine* e, const float* candidate, dou
   BRE_TRY(e->build_bn_slots());
   BRE_TRY(e->build_di_tables());
   BRE_TRY(e->evaluate());
-  if (e->need_task_grad() && !e->task_grad_folded()) BRE_TRY(launch_axpy(e->gradx_task, e->gradx, e->cfg.task_regularization, e->nx, e->stream));
+  if (e->task_grad_from_backward() && !e->task_grad_folded()) BRE_TRY(launch_axpy(e->gradx_task, e->gradx, e->cfg.task_regularization, e->nx, e->stream));
   Scalars h;
   BRE_TRY(read_scalars(e, &h));
   if (objective) {

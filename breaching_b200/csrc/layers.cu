@@ -196,6 +196,10 @@ __global__ void bnact_tan_bwd_g_kernel(BnActTanBwdArgs a, long long pps, int Cpa
   float v[2] = {0.f, 0.f};
   float inv = 0.f, nrm = 0.f, scale = 1.f, vg = 0.f;
   if (cv) { inv = __ldg(a.bn.inv + c); nrm = __ldg(a.bn.nrm + c); scale = __ldg(a.bn.scale + c); vg = __ldg(a.v_gamma + c); }
+  // DeepInversion adjoint at the BN input (the last local step of a FedAvg evaluation): not part of the parameter tangents
+  const bool di = a.di_cm != nullptr;
+  float di_m = 0.f, di_v = 0.f, di_mean = 0.f;
+  if (cv && di) { di_m = __ldg(a.di_cm + c); di_v = __ldg(a.di_cv + c); di_mean = __ldg(a.di_mean + c); }
   if (cv) {
     for (long long p = p0 + threadIdx.y; p < p1; p += 8) {
       const long long o = p * a.C + c;
@@ -206,6 +210,7 @@ __global__ void bnact_tan_bwd_g_kernel(BnActTanBwdArgs a, long long pps, int Cpa
       v[0] += fmaf(tdu, xhat, du * tz * inv);
       v[1] += tdu;
       float tdi = fmaf(scale, tdu, vg * inv * du);
+      if (di) tdi += fmaf(di_v, a.in[o] - di_mean, di_m);
       if (a.tdin != nullptr) {
         if (a.acc_in) tdi += a.tdin[o];
         a.tdin[o] = a.round_din ? tf32_rna(tdi) : tdi;
@@ -1063,6 +1068,30 @@ __global__ void ce_tan_bwd_kernel(const float* __restrict__ p, const float* __re
   for (int c = threadIdx.x; c < C; c += blockDim.x) tdl[(long long)n * C + c] = pp[c] * (zz[c] - dot) * invN;
 }
 
+// the tangent seed plus coef * (p - onehot(y)) / N: the task-loss term of the last local step of a FedAvg evaluation, which
+// enters that step's tangent-backward stream scaled by -1/lr (DESIGN.md section 3.1).  ROUND: output on the TF32 grid.
+template <bool ROUND>
+__global__ void ce_tan_bwd_seed_kernel(const float* __restrict__ p, const float* __restrict__ zdot, const long long* __restrict__ labels,
+                                       int N, int C, float coef, float* tdl) {
+  pdl_prologue();
+  __shared__ double scratch[32];
+  __shared__ float s_dot;
+  const int n = blockIdx.x;
+  const float* pp = p + (long long)n * C;
+  const float* zz = zdot + (long long)n * C;
+  double part = 0.0;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) part += (double)pp[c] * (double)zz[c];
+  const double tot = block_sum(part, scratch);
+  if (threadIdx.x == 0) s_dot = (float)tot;
+  __syncthreads();
+  const float dot = s_dot, invN = 1.0f / (float)N;
+  const int y = (int)labels[n];
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const float t = fmaf(coef, (pp[c] - (c == y ? 1.f : 0.f)) * invN, pp[c] * (zz[c] - dot) * invN);
+    tdl[(long long)n * C + c] = ROUND ? tf32_rna(t) : t;
+  }
+}
+
 // ---- layout ----------------------------------------------------------------------------------------
 __global__ void permute_kernel(const float* __restrict__ src, float* __restrict__ dst, int O, int I, int HW, bool inverse,
                                long long total) {
@@ -1324,6 +1353,13 @@ int launch_ce_fwd(const float* logits, const long long* labels, const float* q, 
 }
 int launch_ce_label_grad(const float* logits, const float* p, const float* zdot, int N, int C, float task_reg, float* out, cudaStream_t s) {
   BRE_KLAUNCH(ce_label_grad_kernel, N, 256, 0, s, logits, p, zdot, N, C, task_reg, out);
+  BRE_CHECK_LAUNCH();
+  return 0;
+}
+int launch_ce_tan_bwd_seeded(const float* p, const float* zdot, const long long* labels, int N, int C, float coef, float* tdlogits,
+                             bool round_out, cudaStream_t s) {
+  if (round_out) BRE_KLAUNCH(ce_tan_bwd_seed_kernel<true>, N, 256, 0, s, p, zdot, labels, N, C, coef, tdlogits);
+  else BRE_KLAUNCH(ce_tan_bwd_seed_kernel<false>, N, 256, 0, s, p, zdot, labels, N, C, coef, tdlogits);
   BRE_CHECK_LAUNCH();
   return 0;
 }

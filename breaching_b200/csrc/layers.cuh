@@ -134,6 +134,10 @@ int launch_ce_label_grad(const float* logits, const float* p, const float* zdot,
                          cudaStream_t s);
 // tangent of dlogits: (p*zdot - p * sum(p*zdot)) / N
 int launch_ce_tan_bwd(const float* p, const float* zdot, int N, int C, float* tdlogits, cudaStream_t s);
+// the same plus coef * (p - onehot(labels)) / N (index labels), optionally stored on the TF32 grid: the task-loss seed of the last
+// local step's tangent backward in a FedAvg evaluation (coef = -task_regularization / lr)
+int launch_ce_tan_bwd_seeded(const float* p, const float* zdot, const long long* labels, int N, int C, float coef, float* tdlogits,
+                             bool round_out, cudaStream_t s);
 
 // column path of the candidate-fed convolution (stem_cols.cu): xcol[(n,p,q)][(r,s,c)] <- NCHW candidate (K padded to Kp, optional
 // TF32 rounding); candidate gradient <- dcol by gathering; zero-padded [Co][Kp] copies of OHWI weight rows and back

@@ -562,7 +562,8 @@ __global__ void loss_mean_kernel(const float* loss_n, int N, Scalars* sc) {
 }
 
 // DeepInversion value and adjoint coefficients: one block per BN layer (not one block walking all 20-53 layers), then a one-warp sum of the per-layer values in layer order.
-__global__ void __launch_bounds__(256) di_layer_kernel(const DiLayer* layers, double* layer_values) {
+// `adjoint_scale` multiplies the adjoint coefficients only (1 in single-step evaluations, -1/lr for the seeds of a FedAvg step).
+__global__ void __launch_bounds__(256) di_layer_kernel(const DiLayer* layers, double* layer_values, double adjoint_scale) {
   pdl_prologue();
   __shared__ double scratch[32];
   __shared__ double s_n[2];
@@ -580,8 +581,8 @@ __global__ void __launch_bounds__(256) di_layer_kernel(const DiLayer* layers, do
   const double nv = s_n[0], nm = s_n[1];
   if (threadIdx.x == 0) layer_values[blockIdx.x] = (double)L.mult * (nv + nm);
   for (int c = threadIdx.x; c < L.C; c += blockDim.x) {
-    const float cm = nm > 0.0 ? (float)((double)L.mult * ((double)L.mean[c] - (double)L.rm[c]) / nm / (double)L.M) : 0.f;
-    const float cv = nv > 0.0 ? (float)((double)L.mult * ((double)L.var[c] - (double)L.rv[c]) / nv * 2.0 / (double)L.M) : 0.f;
+    const float cm = nm > 0.0 ? (float)((double)L.mult * ((double)L.mean[c] - (double)L.rm[c]) / nm / (double)L.M * adjoint_scale) : 0.f;
+    const float cv = nv > 0.0 ? (float)((double)L.mult * ((double)L.var[c] - (double)L.rv[c]) / nv * 2.0 / (double)L.M * adjoint_scale) : 0.f;
     L.cm[c] = cm; L.cv[c] = cv;
   }
 }
@@ -744,8 +745,8 @@ int launch_loss_mean(const float* loss_n, int N, Scalars* sc, cudaStream_t s) {
   BRE_CHECK_LAUNCH();
   return 0;
 }
-int launch_di_finalize(const DiLayer* layers_dev, int n_layers, double* layer_values, Scalars* sc, cudaStream_t s) {
-  BRE_KLAUNCH(di_layer_kernel, n_layers, 256, 0, s, layers_dev, layer_values);
+int launch_di_finalize(const DiLayer* layers_dev, int n_layers, double* layer_values, Scalars* sc, cudaStream_t s, double adjoint_scale) {
+  BRE_KLAUNCH(di_layer_kernel, n_layers, 256, 0, s, layers_dev, layer_values, adjoint_scale);
   BRE_KLAUNCH(di_sum_kernel, 1, 32, 0, s, (const double*)layer_values, n_layers, sc);
   BRE_CHECK_LAUNCH();
   return 0;

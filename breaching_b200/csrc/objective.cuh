@@ -57,7 +57,10 @@ int launch_loss_mean(const float* loss_n, int N, Scalars* sc, cudaStream_t s);
 struct DiLayer { const float* mean; const float* var; const float* rm; const float* rv; float* cm; float* cv; int C; float M; float mult; };
 // DeepInversion value + per-channel adjoint coefficients for all BN layers (one block, layers in order)
 // `layer_values`: device scratch of n_layers doubles (two launches: one block per layer, then the ordered sum)
-int launch_di_finalize(const DiLayer* layers_dev, int n_layers, double* layer_values, Scalars* sc, cudaStream_t s);
+// `adjoint_scale` multiplies the per-channel adjoint coefficients, not the value: -1/lr when the adjoint seeds the last local step
+// of a FedAvg evaluation (DESIGN.md section 3.1)
+int launch_di_finalize(const DiLayer* layers_dev, int n_layers, double* layer_values, Scalars* sc, cudaStream_t s,
+                       double adjoint_scale = 1.0);
 // features regulariser: value into sc->feat, adjoint accumulated into tdelta
 int launch_feature_reg(const float* feat, const float* measured, float* tdelta, long long n, float scale, Scalars* sc,
                        cudaStream_t s);

@@ -347,7 +347,12 @@ class Engine:
         _check(self.lib, self.lib.bre_engine_load_feature_targets(self.h, _ptr(m), m.numel()), "bre_engine_load_feature_targets")
 
     def set_local_steps(self, total_images, steps, lr, labels_per_step):
-        """FedAvg: ``labels_per_step`` = list of ``steps`` LongTensors of length ``data_per_step`` (the program batch)."""
+        """FedAvg: ``labels_per_step`` = list of ``steps`` LongTensors of length ``data_per_step`` (the program batch).
+
+        Supported with the matching objectives, TV / norm / orthogonality on the whole candidate, and ``task_regularization`` and
+        DeepInversion on the last local step (its task loss, the BN-input statistics of its forward; both need ``lr != 0``).  The
+        feature prior (its target is the input feature of no forward pass once the update spans several steps) and train-mode BN
+        raise ``EngineError``."""
         labels = torch.cat([l.detach().to(torch.int64).flatten().cpu() for l in labels_per_step]).contiguous()
         if labels.numel() != steps * self.input_shape[0]:
             raise EngineError("labels_per_step must hold data_per_step labels for every local step")

@@ -123,6 +123,9 @@ int bre_engine_load_targets(bre_engine* e, const float* const* grads, int32_t n_
 /* FedAvg / multi-step local updates (objectives.py:48-72, users.py:336-413): the user ran `steps` SGD steps of size `lr`,
  * step k on the candidate slice [k*B mod total_images, ... + B) (B = batch of the layer program) with labels
  * labels[k*B .. (k+1)*B); the matched quantity becomes W_K - W_0.  Re-sizes the candidate state to `total_images`.
+ * task_regularization and DeepInversion read the last local step (its task loss at W_{K-1}, the BN-input statistics of its
+ * forward) and need lr != 0 (their adjoints seed that step's tangent backward scaled by -1/lr); the feature prior, train-mode
+ * BatchNorm and lr == 0 with a prior are refused with BRE_ERR_UNSUPPORTED.
  * Call after bre_engine_load_model / load_targets and before bre_engine_begin_trial.  labels: device or host. */
 int bre_engine_set_local_steps(bre_engine* e, int32_t total_images, int32_t steps, float lr, const int64_t* labels);
 
@@ -185,8 +188,11 @@ int bre_engine_debug_param(bre_engine* e, int32_t which, int32_t index, float* o
  * step k stays bound: activations, deltas, probabilities, labels, W = W_k and G = G_k (bre_engine_debug_tensor / debug_param).
  * s = K + 1 + k: after step k's tangent-forward and tangent-backward sweeps, before its candidate-gradient axpy and adjoint
  * update; v and its TF32 shadow hold the direction u_{k+1} that step k used, G holds the tangent weight gradient H_k u_{k+1}
- * (k > 0 only) and the tangent delta of tensor 0 is the step's input gradient.  The value and gradient returned by a stopped
- * evaluation are not meaningful.  bre_engine_run refuses while a stop is set. */
+ * (k > 0 only) and the tangent delta of tensor 0 is the step's input gradient.  At the stop after the last step (s = 2K) the
+ * prior seeds are in place: the logits tangent delta holds the cross-entropy tangent plus -tau/lr (p - y)/N (tau =
+ * task_regularization), every BN input's tangent delta holds its DeepInversion adjoint scaled by -1/lr, and G and the step's input
+ * gradient carry those seeds through the sweep.  The value and gradient returned by a stopped evaluation are not meaningful.
+ * bre_engine_run refuses while a stop is set. */
 int bre_engine_debug_step_param(bre_engine* e, int32_t which, int32_t step, int32_t index, float* out_host);
 /* which: 0 = activation, 1 = delta (sweep B), 2 = tangent, 3 = tangent delta; NCHW fp32 to host.  Tensor 0 (the candidate)
  * has no tangent; its delta is the task-loss gradient and its tangent delta the candidate gradient.  With fuse_bnact, the
