@@ -148,6 +148,10 @@ class OptimizationJointAttacker(OptimizationBasedAttacker):
             if shared_data[0]["metadata"]["labels"] is not None:
                 raise ValueError("Joint optimization only makes sense if no labels are provided. Switch to attack.attack_type=optimization instead")
             return self._reconstruct_text(server_payload, shared_data, server_secrets, initial_data, dryrun)
+        from . import augment
+
+        if augment.has_view_stages(self.cfg):   # the joint loop does not run the view pipeline: refuse rather than skip
+            raise NotImplementedError("zoom / centerzoom / focus / antialias are not implemented for the joint attacker by the engine")
         rec_models, labels, stats, shared_data = self.prepare_attack(server_payload, shared_data)
         if any(True for _ in self.regularizers) and any(k in ("deep_inversion", "features") for k, _ in self.regularizers):
             raise NotImplementedError("feature / DeepInversion priors are not implemented for the joint attacker")

@@ -9,7 +9,8 @@ its body.)
 
 On the engine one stage = one trial of a layer program compiled for that resolution (the model must accept variable input sizes,
 e.g. ResNets with adaptive pooling -- otherwise the compiler refuses, as the reference's forward pass would); the resizes run in
-``bre_resize_bilinear`` (``F.interpolate(mode="bilinear", align_corners=False)`` semantics).
+``bre_resize_bilinear`` (``F.interpolate(mode="bilinear", align_corners=False)`` semantics).  Each stage's program is compiled at
+the view shape of that stage's candidate: with ``augmentations: {zoom: {out_size: H}}`` every stage runs the model at H.
 """
 import logging
 
@@ -36,13 +37,13 @@ def scale_pyramid(kind, num_stages, full):
 
 
 class MultiScaleOptimizationAttacker(OptimizationBasedAttacker):
-    def _get_engine(self, rec_models, shared_data, labels, index=0, cfg=None, data_shape=None, primary=True):
+    def _get_engine(self, rec_models, shared_data, labels, index=0, cfg=None, data_shape=None, primary=True, **kw):
         if primary and index == 0:
             self._stage_context = (rec_models, shared_data, labels)
             for eng in getattr(self, "_stage_engines", {}).values():
                 eng.close()
             self._stage_engines = {}
-        return super()._get_engine(rec_models, shared_data, labels, index, cfg, data_shape, primary)
+        return super()._get_engine(rec_models, shared_data, labels, index, cfg, data_shape, primary, **kw)
 
     def _stage_engine(self, scale):
         C, H, W = self.data_shape
@@ -75,7 +76,11 @@ class MultiScaleOptimizationAttacker(OptimizationBasedAttacker):
                 current = background
             else:
                 current = resize_bilinear(current, scale)
-            stage_best = super()._run_trial(self._stage_engine(scale), current, stats, trial, dryrun)
+            try:
+                stage_engine = self._stage_engine(scale)
+            except ValueError as err:    # e.g. a focus window larger than this stage's candidate
+                raise ValueError(f"stage {stage + 1}/{stages} (scale {scale}): {err}") from err
+            stage_best = super()._run_trial(stage_engine, current, stats, trial, dryrun)
             current = stage_best
             best = resize_bilinear(stage_best, H)                           # :66
             if dryrun:

@@ -51,6 +51,13 @@ class _EngineSum:
         return sum(eng.score(candidate, scoring) for eng in self.engines)
 
 
+def _refuse_view_stages_off_device(cfg, n_models):
+    """The host-driven loops (L-BFGS, several model queries) do not run the view pipeline; refuse shape-changing views there rather
+    than skip them."""
+    if str(cfg.optim.optimizer).lower() == "l-bfgs" or n_models > 1:
+        raise NotImplementedError("zoom / centerzoom / focus / antialias are not implemented for L-BFGS or multi-query attacks by the engine")
+
+
 class OptimizationBasedAttacker:
     """Implements the optimisation-based attacks of the reference on the engine."""
 
@@ -124,10 +131,12 @@ class OptimizationBasedAttacker:
             shared_data = host.normalize_gradients(shared_data)
         return rec_models, labels, stats, shared_data
 
-    def _get_engine(self, rec_models, shared_data, labels, index=0, cfg=None, data_shape=None, primary=True):
+    def _get_engine(self, rec_models, shared_data, labels, index=0, cfg=None, data_shape=None, primary=True, for_scoring=False):
         """Engine for model / payload ``index`` (``cfg`` overrides the attack config, used for the extra queries; ``data_shape``
         overrides the candidate's per-example shape and ``primary=False`` builds an additional engine next to the attacker's main
-        one -- both used by the multi-scale attacker's stages)."""
+        one -- both used by the multi-scale attacker's stages).  The program is compiled at the shape the model sees: the view's
+        (attacks/augment.py ``view_shape``).  ``for_scoring=True`` builds the scoring engine of a resizing view instead: compiled at
+        the candidate's shape, and without a Langevin noise seed (it never steps, so it draws nothing from the global RNG)."""
         if len(rec_models) != 1 and cfg is None:
             raise NotImplementedError("use _get_engines for several model queries")
         cfg = self.cfg if cfg is None else cfg
@@ -137,9 +146,18 @@ class OptimizationBasedAttacker:
         # FedAvg (objectives.py:48-72): the layer program is compiled for one local step's batch.  task_regularization and
         # deep_inversion act on the last local step; the features prior is refused by Engine.set_local_steps (see its docstring)
         shape = (n if local is None else int(local["data_per_step"]), *(self.data_shape if data_shape is None else data_shape))
-        seed = int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if cfg_get(self.cfg.optim, "langevin_noise", 0.0) else 0
+        if not for_scoring and local is None:
+            from . import augment
+
+            if augment.has_view_stages(cfg):
+                _refuse_view_stages_off_device(cfg, len(rec_models))
+            shape = augment.view_shape(cfg, shape)
+        seed = int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if cfg_get(self.cfg.optim, "langevin_noise", 0.0) and not for_scoring else 0
         if self._engine is not None and index == 0 and primary:
             self._engine.close()
+            for eng in getattr(self, "_score_engines", {}).values():
+                eng.close()
+            self._score_engines = {}
         # setup["backend"]: "tc" (TF32 tensor cores, default = torch's cuDNN-TF32 numerics) or "simt" (fp32, = allow_tf32 False)
         eng = Engine(model, shape, cfg, self.setup["device"], noise_seed=seed, backend=self.backend)
         eng.load_model()
@@ -193,6 +211,7 @@ class OptimizationBasedAttacker:
         clock["prologue"], t0 = time.perf_counter() - t0, time.perf_counter()
         multi = len(rec_models) > 1
         engine = _EngineSum(self._get_engines(rec_models, shared_data, labels)) if multi else self._get_engine(rec_models, shared_data, labels)
+        self._score_context = (rec_models, shared_data, labels)
         clock["engine"], t0 = time.perf_counter() - t0, time.perf_counter()
         num_trials = self.cfg.restarts.num_trials
         rank, world = bdist.rank_and_world()
@@ -231,8 +250,10 @@ class OptimizationBasedAttacker:
         if name == "l-bfgs" or isinstance(engine, _EngineSum):
             # host-driven loops, every closure evaluation on the engine(s): L-BFGS (common.py:18), and multi-query attacks,
             # whose candidate gradient is a sum over engines and cannot use one engine's fused on-device step
-            from . import lbfgs
+            from . import augment, lbfgs
 
+            if augment.has_view_stages(self.cfg):
+                _refuse_view_stages_off_device(self.cfg, 2)
             dm, ds = self.dm.to(candidate.device), self.ds.to(candidate.device)
             best, history = lbfgs.run_trial(engine, candidate, self.cfg, table, -dm / ds, (1 - dm) / ds, dryrun)
             stats[f"Trial_{trial}_Val"].extend(history)
@@ -278,19 +299,38 @@ class OptimizationBasedAttacker:
 
         key = (candidate.shape[0], candidate.shape[1])
         if key not in self._aug_plans:
-            self._aug_plans[key] = augment.build_plan(self.cfg, candidate.shape[0], candidate.shape[1], self.setup)
-        return self._aug_plans[key]
+            self._aug_plans[key] = augment.build_plan(self.cfg, candidate.shape[0], candidate.shape[1], self.setup, spatial=tuple(candidate.shape[2:]))
+        plan = self._aug_plans[key]
+        if plan is not None and plan.stages and plan.candidate_shape != tuple(candidate.shape):
+            plan = augment.with_spatial(plan, self.cfg, candidate.shape[2:])   # a multi-scale stage: same draws, its own geometry
+        return plan
 
     def _score_trial(self, engine, candidate):
         """optimization_based_attack.py:191-204."""
         scoring = self.cfg.restarts.scoring
         if scoring in ("euclidean", "cosine-similarity"):
-            return engine.score(candidate, scoring)
+            return self._scoring_engine(engine, candidate).score(candidate, scoring)
         if scoring in ("TV", "total-variation"):
             from ..engine import total_variation
 
             return total_variation(candidate.contiguous(), scale=1.0)[0]
         raise ValueError(f"Scoring mechanism {scoring} not implemented.")
+
+    def _scoring_engine(self, engine, candidate):
+        """The score is taken on the un-augmented candidate at its own shape (:191-204).  When a view resizes, the trial's engine
+        runs the model at the view's shape; the score then needs a program at the candidate's shape, built once per shape (a model
+        that cannot take it raises UnsupportedModelError, as the reference's forward pass would fail)."""
+        if isinstance(engine, _EngineSum):
+            return engine
+        t0 = engine.prog.tensors[0]
+        if (t0.N, t0.C, t0.H, t0.W) == tuple(candidate.shape):
+            return engine
+        shape = tuple(candidate.shape)
+        cache = self.__dict__.setdefault("_score_engines", {})
+        if shape not in cache:
+            rec_models, shared_data, labels = self._score_context
+            cache[shape] = self._get_engine(rec_models, shared_data, labels, data_shape=shape[1:], primary=False, for_scoring=True)
+        return cache[shape]
 
     def _select_optimal_reconstruction(self, candidate_solutions, scores, stats, shape):
         """optimization_based_attack.py:206-218 + the cross-rank MINLOC select (dist.py)."""

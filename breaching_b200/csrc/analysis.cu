@@ -3,6 +3,7 @@
 // PSNR = 10 log10(factor^2 / mse) per example follows on the host from those N numbers (analysis/metrics.py:108-130).
 #include "../../include/breaching_b200.h"
 #include "common.cuh"
+#include "augment.cuh"
 
 namespace bre {
 namespace {
@@ -83,8 +84,7 @@ extern "C" int bre_image_mse(const float* rec, const float* ref, int32_t N, int3
 }
 
 // ---- bilinear resize of NCHW batches (MultiScaleOptimizationAttacker, multiscale_optimization_attack.py:45-69) ---------------------
-// F.interpolate(mode="bilinear", align_corners=False): source coordinate = (dst + 0.5) * in/out - 0.5, clamped at 0; the two
-// neighbours per axis are i0 = floor, i1 = min(i0 + 1, in - 1) with weights (1 - l, l).
+// F.interpolate(mode="bilinear", align_corners=False): the index rule bilinear_src (augment.cuh), shared with the RESAMPLE stage.
 namespace bre {
 namespace {
 __global__ void __launch_bounds__(256) resize_bilinear_kernel(const float* __restrict__ src, float* __restrict__ dst, int planes, int Hi, int Wi,
@@ -95,12 +95,9 @@ __global__ void __launch_bounds__(256) resize_bilinear_kernel(const float* __res
     const long long t = i / Wo;
     const int y = (int)(t % Ho);
     const long long pl = t / Ho;
-    float fy = ((float)y + 0.5f) * sh - 0.5f, fx = ((float)x + 0.5f) * sw - 0.5f;
-    fy = fy < 0.f ? 0.f : fy;
-    fx = fx < 0.f ? 0.f : fx;
-    const int y0 = (int)fy, x0 = (int)fx;
-    const int y1 = y0 + (y0 < Hi - 1 ? 1 : 0), x1 = x0 + (x0 < Wi - 1 ? 1 : 0);
-    const float ly = fy - (float)y0, lx = fx - (float)x0;
+    int y0, y1, x0, x1; float ly, lx;
+    bilinear_src(y, sh, Hi, y0, y1, ly);
+    bilinear_src(x, sw, Wi, x0, x1, lx);
     const float* p = src + pl * Hi * Wi;
     const float top = (1.f - lx) * p[(long long)y0 * Wi + x0] + lx * p[(long long)y0 * Wi + x1];
     const float bot = (1.f - lx) * p[(long long)y1 * Wi + x0] + lx * p[(long long)y1 * Wi + x1];

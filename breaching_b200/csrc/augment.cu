@@ -8,6 +8,8 @@
 //                                             g(i, j) = (lin[j] + sx[n], lin[i] + sy[n]), lin = linspace(-1, 1, S), per-image random shifts
 //                                             of at most shift / (S - 1); padding "circular" maps g -> ((g + 1) mod 1) - 1 as the
 //                                             reference does (which samples the top-left quadrant twice per axis -- reproduced)
+// Shape-changing stages (each a stage of its own, see AugStage): RESAMPLE = a window resized bilinearly (Zoom :34-40, CenterZoom :43-55,
+// Focus :20-31), BLUR = binomial depthwise convolution (AntiAlias :198-226).  Their pull-backs are fixed-order gathers (no atomics).
 // Random draws come from Philox keyed by (seed, iteration, step), so the forward view and the transposed pull-back of one
 // iteration see the same draws without any host round trip; `bre_augment_*` take the draws explicitly (parity tests).
 #include <math.h>
@@ -34,27 +36,47 @@ __device__ __forceinline__ void philox4(uint64_t seed, uint32_t a, uint32_t b, u
 }
 __device__ __forceinline__ float u01(uint32_t v) { return ((float)(v >> 8) + 0.5f) * (1.0f / 16777216.0f); }
 
-// one thread block: the draws of this iteration -> AugDraws in global memory (read by the view / pull-back kernels)
-__global__ void aug_draw_kernel(AugPlan plan, const Scalars* sc, AugDraws* draws, int N) {
+// one thread block: the draws of this iteration, every stage -> draws[stage] in global memory (read by the view / pull-back kernels).
+// A PIXEL stage draws with its plan's seed (the first one with the pipeline's seed: a pipeline of one PIXEL stage draws exactly what a
+// single plan drew); a focus stage draws its window corner from Philox(seed, iteration, 0x10000 + stage).
+__global__ void aug_draw_kernel(AugPipeline pipe, const Scalars* sc, AugDraws* draws, int N) {
   pdl_prologue();
   const int it = sc != nullptr ? sc->it : 0;
-  for (int s = threadIdx.x; s < plan.n_steps; s += blockDim.x) {
-    uint32_t r[4];
-    philox4(plan.seed, (uint32_t)it, (uint32_t)s, 0u, r);
-    if (plan.kind[s] == AUG_SHIFT) {
-      const int lim = (int)plan.p0[s];
-      draws->o1[s] = lim > 0 ? (int)(r[0] % (uint32_t)(2 * lim)) - lim : 0;   // randint(-lim, lim)
-      draws->o2[s] = lim > 0 ? (int)(r[1] % (uint32_t)(2 * lim)) - lim : 0;
-    } else if (plan.kind[s] == AUG_FLIP) {
-      draws->o1[s] = u01(r[0]) < plan.p0[s] ? 1 : 0;
+  for (int k = 0; k < pipe.n_stages; ++k) {
+    const AugStage& st = pipe.st[k];
+    AugDraws* d = draws + k;
+    if (st.kind == AUG_STAGE_RESAMPLE && st.focus) {
+      if (threadIdx.x == 0) {      // Focus (:27-31): pert = (rand(2) * 2 - 1) * std; corner = (pert + in // 2 - size // 2).long().clamp
+        uint32_t r[4];
+        philox4(pipe.seed, (uint32_t)it, 0x10000u + (uint32_t)k, 0u, r);
+        const float py = (u01(r[0]) * 2.f - 1.f) * st.focus_std, px = (u01(r[1]) * 2.f - 1.f) * st.focus_std;
+        int y0 = (int)((py + (float)(st.Hi / 2)) - (float)(st.wh / 2)), x0 = (int)((px + (float)(st.Wi / 2)) - (float)(st.ww / 2));
+        y0 = y0 < 0 ? 0 : (y0 > st.Hi - st.wh ? st.Hi - st.wh : y0);
+        x0 = x0 < 0 ? 0 : (x0 > st.Wi - st.ww ? st.Wi - st.ww : x0);
+        d->o1[0] = y0; d->o2[0] = x0;
+      }
+      continue;
     }
-  }
-  // continuous shift: two uniforms per image
-  for (int n = threadIdx.x; n < N; n += blockDim.x) {
-    uint32_t r[4];
-    philox4(plan.seed, (uint32_t)it, 0xC0FFEEu, (uint32_t)n, r);
-    draws->sx[n] = u01(r[0]);
-    draws->sy[n] = u01(r[1]);
+    if (st.kind != AUG_STAGE_PIXEL) continue;
+    const AugPlan& plan = pipe.plan[k];
+    for (int s = threadIdx.x; s < plan.n_steps; s += blockDim.x) {
+      uint32_t r[4];
+      philox4(plan.seed, (uint32_t)it, (uint32_t)s, 0u, r);
+      if (plan.kind[s] == AUG_SHIFT) {
+        const int lim = (int)plan.p0[s];
+        d->o1[s] = lim > 0 ? (int)(r[0] % (uint32_t)(2 * lim)) - lim : 0;   // randint(-lim, lim)
+        d->o2[s] = lim > 0 ? (int)(r[1] % (uint32_t)(2 * lim)) - lim : 0;
+      } else if (plan.kind[s] == AUG_FLIP) {
+        d->o1[s] = u01(r[0]) < plan.p0[s] ? 1 : 0;
+      }
+    }
+    // continuous shift: two uniforms per image
+    for (int n = threadIdx.x; n < N; n += blockDim.x) {
+      uint32_t r[4];
+      philox4(plan.seed, (uint32_t)it, 0xC0FFEEu, (uint32_t)n, r);
+      d->sx[n] = u01(r[0]);
+      d->sy[n] = u01(r[1]);
+    }
   }
 }
 
@@ -178,6 +200,148 @@ __global__ void __launch_bounds__(256) aug_pull_cs_kernel(const float* __restric
   }
 }
 
+// RESAMPLE view: the window [y0, y0 + wh) x [x0, x0 + ww) of every plane, resized bilinearly to Ho x Wo (F.interpolate, bilinear,
+// align_corners = False; zoom: window = image, centerzoom / focus: a fixed / drawn corner; wh = Ho makes the copy exact)
+__device__ __forceinline__ void resample_corner(const AugStage& st, const AugDraws* d, int& y0, int& x0) {
+  y0 = st.y0; x0 = st.x0;
+  if (st.focus) { y0 = d->o1[0]; x0 = d->o2[0]; }
+}
+__global__ void __launch_bounds__(256) aug_resample_view_kernel(const float* __restrict__ x, float* __restrict__ out, int planes, AugStage st,
+                                                                const AugDraws* __restrict__ draws) {
+  pdl_prologue();
+  int y0, x0;
+  resample_corner(st, draws, y0, x0);
+  const float sh = (float)st.wh / (float)st.Ho, sw = (float)st.ww / (float)st.Wo;
+  const long long total = (long long)planes * st.Ho * st.Wo;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const int ox = (int)(e % st.Wo);
+    const long long t = e / st.Wo;
+    const int oy = (int)(t % st.Ho);
+    const long long pl = t / st.Ho;
+    int a0, a1, b0, b1; float ly, lx;
+    bilinear_src(oy, sh, st.wh, a0, a1, ly);
+    bilinear_src(ox, sw, st.ww, b0, b1, lx);
+    const float* p = x + pl * st.Hi * st.Wi + (long long)y0 * st.Wi + x0;
+    const float top = (1.f - lx) * p[(long long)a0 * st.Wi + b0] + lx * p[(long long)a0 * st.Wi + b1];
+    const float bot = (1.f - lx) * p[(long long)a1 * st.Wi + b0] + lx * p[(long long)a1 * st.Wi + b1];
+    out[e] = (1.f - ly) * top + ly * bot;
+  }
+}
+
+// weight of window index q in the bilinear stencil of output index o (both neighbours land on q at the clamped last index)
+__device__ __forceinline__ float bilinear_weight(int o, float scale, int in, int q) {
+  int i0, i1; float l;
+  bilinear_src(o, scale, in, i0, i1, l);
+  return (i0 == q ? 1.f - l : 0.f) + (i1 == q ? l : 0.f);
+}
+// the output indices whose stencil can touch window index q: source coordinates in [q - 1, q + 1), widened by two on each side
+// (the membership test is exact, the range only has to contain it)
+__device__ __forceinline__ void bilinear_range(int q, float scale, int out, int& lo, int& hi) {
+  lo = (int)floorf(((float)q - 0.5f) / scale - 0.5f) - 2;
+  hi = (int)ceilf(((float)q + 1.5f) / scale - 0.5f) + 2;
+  lo = lo < 0 ? 0 : lo;
+  hi = hi > out - 1 ? out - 1 : hi;
+}
+// RESAMPLE pull-back, separable in two fixed-order gathers (no atomics; each bilinear weight is evaluated once per gathered term):
+//   axis 0: tmp[pl, oy, qx] = sum_ox wx(ox -> qx) g[pl, oy, ox]                  (qx in the window, tmp is [planes, Ho, ww])
+//   axis 1: gx[pl, y, x]   = sum_oy wy(oy -> y - y0) tmp[pl, oy, x - x0]           (zero outside the window)
+__global__ void __launch_bounds__(256) aug_resample_pull_kernel(const float* __restrict__ g, float* __restrict__ out, int planes, AugStage st,
+                                                                const AugDraws* __restrict__ draws, int axis) {
+  pdl_prologue();
+  int y0, x0;
+  resample_corner(st, draws, y0, x0);
+  const float sh = (float)st.wh / (float)st.Ho, sw = (float)st.ww / (float)st.Wo;
+  const int rows = axis == 0 ? st.Ho : st.Hi, cols = axis == 0 ? st.ww : st.Wi;
+  const long long total = (long long)planes * rows * cols;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(e % cols);
+    const long long t = e / cols;
+    const int r = (int)(t % rows);
+    const long long pl = t / rows;
+    float acc = 0.f;
+    if (axis == 0) {
+      const float* row = g + (pl * st.Ho + r) * st.Wo;
+      int lo, hi;
+      bilinear_range(c, sw, st.Wo, lo, hi);
+      for (int ox = lo; ox <= hi; ++ox) {
+        const float w = bilinear_weight(ox, sw, st.ww, c);
+        if (w != 0.f) acc = fmaf(w, row[ox], acc);
+      }
+    } else {
+      const int qy = r - y0, qx = c - x0;
+      if (qy >= 0 && qy < st.wh && qx >= 0 && qx < st.ww) {
+        const float* col = g + pl * st.Ho * st.ww + qx;
+        int lo, hi;
+        bilinear_range(qy, sh, st.Ho, lo, hi);
+        for (int oy = lo; oy <= hi; ++oy) {
+          const float w = bilinear_weight(oy, sh, st.wh, qy);
+          if (w != 0.f) acc = fmaf(w, col[(long long)oy * st.ww], acc);
+        }
+      }
+    }
+    out[e] = acc;
+  }
+}
+
+// BLUR (AntiAlias :198-226): depthwise conv2d with the normalised outer product of the binomial row of `width`, zero padding
+// width // 2, `stride`.  The weights c[a] / 2^(width - 1) are dyadic: their products are the reference's filter exactly.
+__device__ __forceinline__ float binomial_weight(int width, int a) {
+  float c = 1.f;                                      // C(width - 1, a), exact in fp32 for width <= 7
+  for (int i = 0; i < a; ++i) c = c * (float)(width - 1 - i) / (float)(i + 1);
+  return ldexpf(c, -(width - 1));
+}
+__global__ void __launch_bounds__(256) aug_blur_view_kernel(const float* __restrict__ x, float* __restrict__ out, int planes, AugStage st) {
+  pdl_prologue();
+  const int pad = st.width / 2;
+  const long long total = (long long)planes * st.Ho * st.Wo;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const int ox = (int)(e % st.Wo);
+    const long long t = e / st.Wo;
+    const int oy = (int)(t % st.Ho);
+    const long long pl = t / st.Ho;
+    const float* p = x + pl * st.Hi * st.Wi;
+    float acc = 0.f;
+    for (int a = 0; a < st.width; ++a) {
+      const int y = oy * st.stride - pad + a;
+      if (y < 0 || y >= st.Hi) continue;
+      float row = 0.f;
+      for (int b = 0; b < st.width; ++b) {
+        const int xx = ox * st.stride - pad + b;
+        if (xx >= 0 && xx < st.Wi) row = fmaf(binomial_weight(st.width, b), p[(long long)y * st.Wi + xx], row);
+      }
+      acc = fmaf(binomial_weight(st.width, a), row, acc);
+    }
+    out[e] = acc;
+  }
+}
+// BLUR pull-back: input pixel (y, x) gathers the view gradients of the outputs (oy, ox) with oy * stride - pad + a = y, in order of a, b
+__global__ void __launch_bounds__(256) aug_blur_pull_kernel(const float* __restrict__ g, float* __restrict__ gx, int planes, AugStage st) {
+  pdl_prologue();
+  const int pad = st.width / 2;
+  const long long total = (long long)planes * st.Hi * st.Wi;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const int xq = (int)(e % st.Wi);
+    const long long t = e / st.Wi;
+    const int yq = (int)(t % st.Hi);
+    const long long pl = t / st.Hi;
+    const float* p = g + pl * st.Ho * st.Wo;
+    float acc = 0.f;
+    for (int a = 0; a < st.width; ++a) {
+      const int ny = yq + pad - a;
+      if (ny < 0 || ny % st.stride != 0 || ny / st.stride >= st.Ho) continue;
+      const int oy = ny / st.stride;
+      float row = 0.f;
+      for (int b = 0; b < st.width; ++b) {
+        const int nx = xq + pad - b;
+        if (nx < 0 || nx % st.stride != 0 || nx / st.stride >= st.Wo) continue;
+        row = fmaf(binomial_weight(st.width, b), p[(long long)oy * st.Wo + nx / st.stride], row);
+      }
+      acc = fmaf(binomial_weight(st.width, a), row, acc);
+    }
+    gx[e] = acc;
+  }
+}
+
 inline int grid_for(long long n) {
   long long b = (n + 255) / 256;
   const long long cap = (long long)kNumSMs * 16;
@@ -186,9 +350,9 @@ inline int grid_for(long long n) {
 
 }  // namespace
 
-int launch_aug_draw(const AugPlan& plan, const Scalars* sc, AugDraws* draws, int N, cudaStream_t s) {
+int launch_aug_draws(const AugPipeline& pipe, const Scalars* sc, AugDraws* draws, int N, cudaStream_t s) {
   if (N > AUG_MAX_BATCH) { set_error("augmentations: batch larger than AUG_MAX_BATCH"); return -4; }
-  BRE_KLAUNCH(aug_draw_kernel, 1, 64, 0, s, plan, sc, draws, N);
+  BRE_KLAUNCH(aug_draw_kernel, 1, 64, 0, s, pipe, sc, draws, N);
   BRE_CHECK_LAUNCH();
   return 0;
 }
@@ -206,6 +370,24 @@ int launch_aug_pull(float* g, float* tmp, float* gx, int N, int C, int H, int W,
     BRE_KLAUNCH(aug_pull_cs_kernel, grid, 256, 0, s, (const float*)tmp, g, N, C, H, W, plan, draws, 1);
   }
   BRE_KLAUNCH(aug_pull_perm_kernel, grid, 256, 0, s, src, gx, N, C, H, W, plan, draws);
+  BRE_CHECK_LAUNCH();
+  return 0;
+}
+
+int launch_aug_resample(const float* x, float* out, int N, const AugStage& st, const AugDraws* draws, bool transpose, float* tmp, cudaStream_t s) {
+  const int planes = N * st.C;
+  if (!transpose) BRE_KLAUNCH(aug_resample_view_kernel, grid_for((long long)planes * st.Ho * st.Wo), 256, 0, s, x, out, planes, st, draws);
+  else {
+    BRE_KLAUNCH(aug_resample_pull_kernel, grid_for((long long)planes * st.Ho * st.ww), 256, 0, s, x, (float*)tmp, planes, st, draws, 0);
+    BRE_KLAUNCH(aug_resample_pull_kernel, grid_for((long long)planes * st.Hi * st.Wi), 256, 0, s, (const float*)tmp, out, planes, st, draws, 1);
+  }
+  BRE_CHECK_LAUNCH();
+  return 0;
+}
+int launch_aug_blur(const float* x, float* out, int N, const AugStage& st, bool transpose, cudaStream_t s) {
+  const int planes = N * st.C;
+  if (!transpose) BRE_KLAUNCH(aug_blur_view_kernel, grid_for((long long)planes * st.Ho * st.Wo), 256, 0, s, x, out, planes, st);
+  else BRE_KLAUNCH(aug_blur_pull_kernel, grid_for((long long)planes * st.Hi * st.Wi), 256, 0, s, x, out, planes, st);
   BRE_CHECK_LAUNCH();
   return 0;
 }
@@ -246,5 +428,35 @@ extern "C" int bre_augment_view(const float* x, float* out, int32_t N, int32_t C
   }
   cudaStreamSynchronize(s);
   cudaFreeAsync(dev, s);
+  return rc;
+}
+
+extern "C" int bre_augment_resample(const float* x, float* out, int32_t N, int32_t C, int32_t Hi, int32_t Wi, int32_t y0, int32_t x0,
+                                    int32_t wh, int32_t ww, int32_t Ho, int32_t Wo, int32_t transpose, void* stream) {
+  if (!x || !out || N <= 0 || C <= 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || wh <= 0 || ww <= 0 || y0 < 0 || x0 < 0 || y0 + wh > Hi ||
+      x0 + ww > Wi) { set_error("bre_augment_resample: bad arguments (the window must lie inside the input)"); return BRE_ERR_INVALID; }
+  AugStage st;
+  memset(&st, 0, sizeof(st));
+  st.kind = AUG_STAGE_RESAMPLE; st.C = C; st.Hi = Hi; st.Wi = Wi; st.Ho = Ho; st.Wo = Wo; st.y0 = y0; st.x0 = x0; st.wh = wh; st.ww = ww;
+  cudaStream_t s = (cudaStream_t)stream;
+  float* tmp = nullptr;             // the pull-back's intermediate [N, C, Ho, ww]
+  if (transpose) BRE_CUDA_CHECK(cudaMallocAsync((void**)&tmp, (size_t)N * C * Ho * ww * sizeof(float), s));
+  const int rc = launch_aug_resample(x, out, N, st, nullptr, transpose != 0, tmp, s);
+  BRE_CUDA_CHECK(cudaStreamSynchronize(s));
+  if (tmp) cudaFreeAsync(tmp, s);
+  return rc;
+}
+
+extern "C" int bre_augment_blur(const float* x, float* out, int32_t N, int32_t C, int32_t Hi, int32_t Wi, int32_t width, int32_t stride,
+                                int32_t transpose, void* stream) {
+  if (!x || !out || N <= 0 || C <= 0 || Hi <= 0 || Wi <= 0 || width < 1 || width > 7 || stride < 1) {
+    set_error("bre_augment_blur: bad arguments (width 1..7, stride >= 1)"); return BRE_ERR_INVALID;
+  }
+  AugStage st;
+  memset(&st, 0, sizeof(st));
+  st.kind = AUG_STAGE_BLUR; st.C = C; st.Hi = Hi; st.Wi = Wi; st.width = width; st.stride = stride;
+  st.Ho = (Hi + 2 * (width / 2) - width) / stride + 1; st.Wo = (Wi + 2 * (width / 2) - width) / stride + 1;
+  const int rc = launch_aug_blur(x, out, N, st, transpose != 0, (cudaStream_t)stream);
+  BRE_CUDA_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
   return rc;
 }

@@ -223,23 +223,47 @@ struct bre_engine {
   }
   // candidate augmentations (augment.cu; optimization_based_attack.py:149-153): the model and the priors see view(x); the
   // gradient is pulled back through the transposed view (differentiable mode) or x itself is replaced by its view (the
-  // reference's non-differentiable mode, which assigns candidate.data)
+  // reference's non-differentiable mode, which assigns candidate.data).  The view is an ordered list of stages (AugStage); the
+  // last one writes x_aug, whose shape is program tensor 0's.  x and the rest of the candidate-side state keep the candidate's
+  // shape (xN, xC, xH, xW), which differs from tensor 0's when a stage resizes.
   bool aug_on = false, aug_diff = false;
-  AugPlan aug;
-  AugDraws* aug_draws = nullptr;
-  float *x_aug = nullptr, *gradx_aug = nullptr, *aug_tmp = nullptr, *cj_scale = nullptr, *cj_shift = nullptr;
+  AugPipeline aug_pipe;
+  AugDraws* aug_draws = nullptr;     // [AUG_MAX_STAGES]
+  float *x_aug = nullptr, *gradx_aug = nullptr, *aug_tmp = nullptr, *cj = nullptr;
+  float* aug_buf[2] = {nullptr, nullptr};   // stage-to-stage ping-pong (pipelines of several stages)
+  long long aug_cap = 0, aug_buf_cap = 0;   // capacity of x_aug / gradx_aug and of aug_tmp / aug_buf
   float* input_x() const { return aug_on && aug_diff ? x_aug : x; }          // what the first layer and the priors read
   float* input_grad() const { return aug_on && aug_diff ? gradx_aug : gradx; }
   void bind_input() { t[0].val = input_x(); t[0].td = input_grad(); }
+  bool view_resizes() const {   // candidate and program tensor 0 differ in shape
+    const bre_tensor_desc& v = td(0);
+    return ms_steps == 0 && (xN != v.N || xC != v.C || xH != v.H || xW != v.W);
+  }
   int augment_forward() {
-    BRE_LAUNCH(launch_aug_draw(aug, sc, aug_draws, xN, stream));
-    BRE_LAUNCH(launch_aug_view(x, x_aug, xN, xC, xH, xW, aug, aug_draws, stream));
+    BRE_LAUNCH(launch_aug_draws(aug_pipe, sc, aug_draws, xN, stream));
+    const float* src = x;
+    for (int k = 0; k < aug_pipe.n_stages; ++k) {
+      const AugStage& st = aug_pipe.st[k];
+      float* dst = k == aug_pipe.n_stages - 1 ? x_aug : aug_buf[k & 1];
+      if (st.kind == AUG_STAGE_PIXEL) BRE_LAUNCH(launch_aug_view(src, dst, xN, st.C, st.Hi, st.Wi, aug_pipe.plan[k], aug_draws + k, stream));
+      else if (st.kind == AUG_STAGE_RESAMPLE) BRE_LAUNCH(launch_aug_resample(src, dst, xN, st, aug_draws + k, false, nullptr, stream));
+      else BRE_LAUNCH(launch_aug_blur(src, dst, xN, st, false, stream));
+      src = dst;
+    }
     if (!aug_diff) BRE_CUDA_CHECK(cudaMemcpyAsync(x, x_aug, nx * sizeof(float), cudaMemcpyDeviceToDevice, stream));
     return 0;
   }
-  int augment_pull() {   // gradx <- view^T (gradx_aug + task_regularization * gradx_task)
-    if (task_grad_from_backward()) BRE_LAUNCH(launch_axpy(gradx_task, gradx_aug, cfg.task_regularization, nx, stream));
-    BRE_LAUNCH(launch_aug_pull(gradx_aug, aug_tmp, gradx, xN, xC, xH, xW, aug, aug_draws, stream));
+  int augment_pull() {   // gradx <- view^T (gradx_aug + task_regularization * gradx_task), stage by stage from the last
+    if (task_grad_from_backward()) BRE_LAUNCH(launch_axpy(gradx_task, gradx_aug, cfg.task_regularization, t[0].numel, stream));
+    float* src = gradx_aug;
+    for (int k = aug_pipe.n_stages - 1; k >= 0; --k) {
+      const AugStage& st = aug_pipe.st[k];
+      float* dst = k == 0 ? gradx : aug_buf[k & 1];
+      if (st.kind == AUG_STAGE_PIXEL) BRE_LAUNCH(launch_aug_pull(src, aug_tmp, dst, xN, st.C, st.Hi, st.Wi, aug_pipe.plan[k], aug_draws + k, stream));
+      else if (st.kind == AUG_STAGE_RESAMPLE) BRE_LAUNCH(launch_aug_resample(src, dst, xN, st, aug_draws + k, true, aug_tmp, stream));
+      else BRE_LAUNCH(launch_aug_blur(src, dst, xN, st, true, stream));
+      src = dst;
+    }
     return 0;
   }
   bool task_grad_folded() const { return aug_on && aug_diff; }   // the task-gradient term already sits inside gradx
@@ -948,26 +972,30 @@ struct bre_engine {
     return 0;
   }
 
-  int priors() {
+  int priors() {   // on what the model sees: the view in differentiable mode (its own shape), the candidate otherwise
+    const bool on_view = aug_on && aug_diff;
+    const bre_tensor_desc& vd = td(0);
+    const int pN = on_view ? vd.N : xN, pC = on_view ? vd.C : xC, pH = on_view ? vd.H : xH, pW = on_view ? vd.W : xW;
+    const long long pn = on_view ? t[0].numel : nx;
     const bool image_terms = cfg.tv_scale != 0.f || cfg.norm_scale != 0.f;
     if (!image_terms) {
       if (cfg.orthogonality != 0)
-        BRE_LAUNCH(launch_orthogonality(input_x(), input_grad(), xN, (long long)xC * xH * xW, true, sc, dpartials, dcounter, stream));
+        BRE_LAUNCH(launch_orthogonality(input_x(), input_grad(), pN, (long long)pC * pH * pW, true, sc, dpartials, dcounter, stream));
       return 0;
     }
-    if (xC != 3) {   // TV on non-RGB candidates is rejected at creation (the reference's grouped conv raises as well)
-      BRE_LAUNCH(launch_norm_prior(input_x(), input_grad(), nx, cfg.norm_scale, cfg.norm_p, 1, sc, dpartials, dcounter, stream));
+    if (pC != 3) {   // TV on non-RGB candidates is rejected at creation (the reference's grouped conv raises as well)
+      BRE_LAUNCH(launch_norm_prior(input_x(), input_grad(), pn, cfg.norm_scale, cfg.norm_p, 1, sc, dpartials, dcounter, stream));
       if (cfg.orthogonality != 0)
-        BRE_LAUNCH(launch_orthogonality(input_x(), input_grad(), xN, (long long)xC * xH * xW, false, sc, dpartials, dcounter, stream));
+        BRE_LAUNCH(launch_orthogonality(input_x(), input_grad(), pN, (long long)pC * pH * pW, false, sc, dpartials, dcounter, stream));
       return 0;
     }
     PriorArgs a;
-    a.x = input_x(); a.grad = input_grad(); a.N = xN; a.H = xH; a.W = xW; a.accumulate = 1;
+    a.x = input_x(); a.grad = input_grad(); a.N = pN; a.H = pH; a.W = pW; a.accumulate = 1;
     a.tv_scale = cfg.tv_scale; a.p = cfg.tv_inner_exp; a.q = cfg.tv_outer_exp; a.eps = cfg.tv_eps;
     a.double_opponents = cfg.tv_double_opponents; a.norm_scale = cfg.norm_scale; a.norm_p = cfg.norm_p;
     BRE_LAUNCH(launch_image_priors(a, sc, dpartials, dcounter, stream));
     if (cfg.orthogonality != 0)
-      BRE_LAUNCH(launch_orthogonality(input_x(), input_grad(), xN, (long long)xC * xH * xW, false, sc, dpartials, dcounter, stream));
+      BRE_LAUNCH(launch_orthogonality(input_x(), input_grad(), pN, (long long)pC * pH * pW, false, sc, dpartials, dcounter, stream));
     return 0;
   }
 
@@ -1628,6 +1656,11 @@ int bre_engine_score(bre_engine* e, const float* candidate, int32_t scoring, dou
   if (!e || !candidate || !out_score) return BRE_ERR_INVALID;
   if (scoring != BRE_OBJ_EUCLIDEAN && scoring != BRE_OBJ_COSINE) { set_error("scoring must be euclidean or cosine-similarity"); return BRE_ERR_UNSUPPORTED; }
   if (!e->model_loaded || !e->targets_loaded) { set_error("load model and targets first"); return BRE_ERR_STATE; }
+  if (e->view_resizes()) {   // the score is taken on the candidate itself (:191-204), which this program cannot take
+    set_error("bre_engine_score: the candidate's shape differs from the program's (a resizing augmentation is set); score it on an "
+              "engine compiled at the candidate's shape");
+    return BRE_ERR_UNSUPPORTED;
+  }
   BRE_CUDA_CHECK(cudaSetDevice(e->device));
   BRE_CUDA_CHECK(cudaMemcpyAsync(e->x, candidate, e->nx * sizeof(float), cudaMemcpyDefault, e->stream));
   if (e->ms_steps > 0) {
@@ -1677,6 +1710,7 @@ int bre_engine_forward(bre_engine* e, const float* data, float* logits_out) {
   if (!e || !data || !logits_out) { set_error("bre_engine_forward: bad arguments"); return BRE_ERR_INVALID; }
   if (!e->model_loaded) { set_error("load the model first"); return BRE_ERR_STATE; }
   if (e->ms_steps > 0) { set_error("bre_engine_forward: not available on a multi-step engine"); return BRE_ERR_UNSUPPORTED; }
+  if (e->view_resizes()) { set_error("bre_engine_forward: a resizing augmentation is set (the data would not have the program's shape)"); return BRE_ERR_UNSUPPORTED; }
   BRE_CUDA_CHECK(cudaSetDevice(e->device));
   BRE_CUDA_CHECK(cudaMemcpyAsync(e->x, data, e->nx * sizeof(float), cudaMemcpyDefault, e->stream));
   float* keep_q = e->soft_q;
@@ -1699,6 +1733,7 @@ int bre_engine_param_gradients(bre_engine* e, const float* data, const int64_t* 
   if (!e || !data || !labels || !grads_out) { set_error("bre_engine_param_gradients: bad arguments"); return BRE_ERR_INVALID; }
   if (!e->model_loaded) { set_error("load the model first"); return BRE_ERR_STATE; }
   if (e->ms_steps > 0 || e->seq_len > 0) { set_error("bre_engine_param_gradients: single-step vision programs only"); return BRE_ERR_UNSUPPORTED; }
+  if (e->view_resizes()) { set_error("bre_engine_param_gradients: a resizing augmentation is set (the data would not have the program's shape)"); return BRE_ERR_UNSUPPORTED; }
   if (n_labels != e->n_labels || n_params != (int)e->params.size()) { set_error("bre_engine_param_gradients: label / parameter count mismatch"); return BRE_ERR_INVALID; }
   BRE_CUDA_CHECK(cudaSetDevice(e->device));
   BRE_CUDA_CHECK(cudaMemcpyAsync(e->x, data, e->nx * sizeof(float), cudaMemcpyDefault, e->stream));
@@ -1738,49 +1773,153 @@ int bre_engine_bn_batch_stats(bre_engine* e, int32_t bn_index, float* mean_out, 
   return BRE_OK;
 }
 
-int bre_engine_set_augmentations(bre_engine* e, int32_t n_steps, const int32_t* kinds, const float* params, int32_t cs_enabled, float cs_shift,
-                                 int32_t cs_circular, const float* cj_scale, const float* cj_shift, int32_t differentiable, uint64_t seed) {
-  if (!e || n_steps < 0 || n_steps > AUG_MAX_STEPS || (n_steps > 0 && (!kinds || !params))) { set_error("bre_engine_set_augmentations: bad arguments"); return BRE_ERR_INVALID; }
+// (re)allocate the candidate-side state at the candidate's shape [N, C, H, W] (the precedent of bre_engine_set_local_steps): tensor 0
+// is the view, so x, gradx, m, v and best follow the candidate; gradx_task keeps tensor 0's shape (the task gradient at the view)
+static int set_candidate_shape(bre_engine* e, int N, int C, int H, int W) {
+  if (e->xN == N && e->xC == C && e->xH == H && e->xW == W) return 0;
+  e->xN = N; e->xC = C; e->xH = H; e->xW = W;
+  e->nx = (long long)N * C * H * W;
+  int rc = 0;
+  rc |= e->alloc(&e->x, e->nx); rc |= e->alloc(&e->gradx, e->nx);
+  rc |= e->alloc(&e->m, e->nx); rc |= e->alloc(&e->v, e->nx); rc |= e->alloc(&e->best, e->nx);
+  if (rc != 0) return BRE_ERR_CUDA;
+  e->trial_begun = false;
+  return 0;
+}
+
+// the ordered stage list -> e->aug_pipe; candidate shape [N, C, H, W]; n_stages = 0 switches augmentations off
+static int set_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage* stages, int32_t N, int32_t C, int32_t H, int32_t W,
+                      int32_t differentiable, uint64_t seed) {
+  if (n_stages < 0 || n_stages > AUG_MAX_STAGES || (n_stages > 0 && !stages)) { set_error("augmentations: at most 8 stages"); return BRE_ERR_INVALID; }
   if (e->ms_steps > 0) { set_error("augmentations are not supported together with local steps"); return BRE_ERR_UNSUPPORTED; }
-  if (e->xN > AUG_MAX_BATCH) { set_error("augmentations: batch too large"); return BRE_ERR_UNSUPPORTED; }
+  const bre_tensor_desc& v = e->td(0);
+  if (n_stages == 0) { N = v.N; C = v.C; H = v.H; W = v.W; }
+  if (N != v.N || C != v.C || H <= 0 || W <= 0) { set_error("augmentations: the candidate must have the program's batch and channels"); return BRE_ERR_INVALID; }
+  if (N > AUG_MAX_BATCH) { set_error("augmentations: batch too large"); return BRE_ERR_UNSUPPORTED; }
   BRE_CUDA_CHECK(cudaSetDevice(e->device));
-  e->graph_ready = false;
-  const bool any = n_steps > 0 || cs_enabled || cj_scale != nullptr;
-  memset(&e->aug, 0, sizeof(e->aug));
-  e->aug_on = any;
-  e->aug_diff = any && differentiable != 0;
-  if (any) {
-    for (int s = 0; s < n_steps; ++s) {
-      if (kinds[s] != AUG_SHIFT && kinds[s] != AUG_FLIP) { set_error("unknown augmentation step"); return BRE_ERR_INVALID; }
-      e->aug.kind[s] = kinds[s]; e->aug.p0[s] = params[s];
-    }
-    e->aug.n_steps = n_steps; e->aug.cs_enabled = cs_enabled; e->aug.cs_shift = cs_shift; e->aug.cs_circular = cs_circular; e->aug.seed = seed;
-    if (cs_enabled && e->xH != e->xW) { set_error("continuous_shift needs square images (the reference builds an S x S grid from shape[2])"); return BRE_ERR_UNSUPPORTED; }
-    if (!e->x_aug) {
-      BRE_TRY(e->alloc(&e->x_aug, e->nx)); BRE_TRY(e->alloc(&e->gradx_aug, e->nx)); BRE_TRY(e->alloc(&e->aug_tmp, e->nx));
-      BRE_TRY(e->alloc(&e->aug_draws, 1));
-      BRE_TRY(e->alloc(&e->cj_scale, (long long)e->xN * e->xC)); BRE_TRY(e->alloc(&e->cj_shift, (long long)e->xN * e->xC));
-    }
-    if (cj_scale != nullptr) {
-      if (!cj_shift) { set_error("colour scale and shift go together"); return BRE_ERR_INVALID; }
-      BRE_CUDA_CHECK(cudaMemcpyAsync(e->cj_scale, cj_scale, (size_t)e->xN * e->xC * sizeof(float), cudaMemcpyDefault, e->stream));
-      BRE_CUDA_CHECK(cudaMemcpyAsync(e->cj_shift, cj_shift, (size_t)e->xN * e->xC * sizeof(float), cudaMemcpyDefault, e->stream));
-      BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
-      e->aug.cj_scale = e->cj_scale; e->aug.cj_shift = e->cj_shift;
-    }
+  AugPipeline pipe;
+  memset(&pipe, 0, sizeof(pipe));
+  pipe.n_stages = n_stages;
+  pipe.seed = seed;
+  int h = H, w = W, pixel_runs = 0;
+  long long widest = (long long)N * C * H * W;
+  for (int k = 0; k < n_stages; ++k) {
+    const bre_aug_stage& in = stages[k];
+    AugStage& st = pipe.st[k];
+    st.kind = in.kind; st.C = C; st.Hi = h; st.Wi = w; st.Ho = h; st.Wo = w;
+    if (in.kind == BRE_AUG_PIXEL) {
+      AugPlan& plan = pipe.plan[k];
+      if (in.n_steps < 0 || in.n_steps > AUG_MAX_STEPS) { set_error("augmentations: at most four shift / flip steps per stage"); return BRE_ERR_INVALID; }
+      for (int s = 0; s < in.n_steps; ++s) {
+        if (in.kinds[s] != AUG_SHIFT && in.kinds[s] != AUG_FLIP) { set_error("unknown augmentation step"); return BRE_ERR_INVALID; }
+        plan.kind[s] = in.kinds[s]; plan.p0[s] = in.params[s];
+      }
+      plan.n_steps = in.n_steps; plan.cs_enabled = in.cs_enabled; plan.cs_shift = in.cs_shift; plan.cs_circular = in.cs_circular;
+      plan.seed = pixel_runs == 0 ? seed : seed ^ (0x9E3779B97F4A7C15ull * (unsigned long long)pixel_runs);   // the first run: the plain plan's keys
+      ++pixel_runs;
+      if (in.cs_enabled && h != w) { set_error("continuous_shift needs square images (the reference builds an S x S grid from shape[2])"); return BRE_ERR_UNSUPPORTED; }
+      if ((in.cj_scale != nullptr) != (in.cj_shift != nullptr)) { set_error("colour scale and shift go together"); return BRE_ERR_INVALID; }
+    } else if (in.kind == BRE_AUG_RESAMPLE) {
+      if (in.Ho <= 0 || in.Wo <= 0 || in.wh <= 0 || in.ww <= 0 || in.wh > h || in.ww > w || (!in.focus && (in.y0 < 0 || in.x0 < 0 || in.y0 + in.wh > h || in.x0 + in.ww > w))) {
+        set_error("augmentations: a resample window must lie inside its input"); return BRE_ERR_INVALID;
+      }
+      st.y0 = in.y0; st.x0 = in.x0; st.wh = in.wh; st.ww = in.ww; st.focus = in.focus; st.focus_std = in.focus_std; st.Ho = in.Ho; st.Wo = in.Wo;
+    } else if (in.kind == BRE_AUG_BLUR) {
+      if (in.width < 1 || in.width > 7 || in.stride < 1) { set_error("augmentations: antialias width must be 1..7 and stride >= 1"); return BRE_ERR_INVALID; }
+      st.width = in.width; st.stride = in.stride;
+      st.Ho = (h + 2 * (in.width / 2) - in.width) / in.stride + 1; st.Wo = (w + 2 * (in.width / 2) - in.width) / in.stride + 1;
+      if (st.Ho <= 0 || st.Wo <= 0) { set_error("augmentations: antialias output is empty"); return BRE_ERR_INVALID; }
+    } else { set_error("unknown augmentation stage"); return BRE_ERR_INVALID; }
+    h = st.Ho; w = st.Wo;
+    if ((long long)N * C * h * w > widest) widest = (long long)N * C * h * w;
+    if (st.kind == AUG_STAGE_RESAMPLE && (long long)N * C * st.Ho * st.ww > widest) widest = (long long)N * C * st.Ho * st.ww;   // pull-back intermediate
   }
+  if (n_stages > 0 && (h != v.H || w != v.W)) { set_error("augmentations: the last stage's output must have program tensor 0's shape"); return BRE_ERR_INVALID; }
+  if (n_stages > 0 && !differentiable && (H != v.H || W != v.W)) {
+    set_error("shape-changing augmentations need differentiable_augmentations: True (a non-differentiable view replaces the candidate by it)");
+    return BRE_ERR_UNSUPPORTED;
+  }
+  BRE_TRY(set_candidate_shape(e, N, C, H, W));
+  e->graph_ready = false;
+  e->aug_on = n_stages > 0;
+  e->aug_diff = e->aug_on && differentiable != 0;
+  if (e->aug_on) {
+    if (e->aug_cap < e->t[0].numel) {
+      BRE_TRY(e->alloc(&e->x_aug, e->t[0].numel)); BRE_TRY(e->alloc(&e->gradx_aug, e->t[0].numel));
+      e->aug_cap = e->t[0].numel;
+    }
+    if (e->aug_buf_cap < widest) {
+      BRE_TRY(e->alloc(&e->aug_tmp, widest)); BRE_TRY(e->alloc(&e->aug_buf[0], widest)); BRE_TRY(e->alloc(&e->aug_buf[1], widest));
+      e->aug_buf_cap = widest;
+    }
+    if (!e->aug_draws) {
+      BRE_TRY(e->alloc(&e->aug_draws, AUG_MAX_STAGES));
+      BRE_TRY(e->alloc(&e->cj, 2LL * AUG_MAX_STAGES * AUG_MAX_BATCH * C));
+    }
+    for (int k = 0; k < n_stages; ++k) {
+      if (stages[k].kind != BRE_AUG_PIXEL || stages[k].cj_scale == nullptr) continue;
+      float* sc_dev = e->cj + 2LL * k * AUG_MAX_BATCH * C;
+      float* sh_dev = sc_dev + (long long)AUG_MAX_BATCH * C;
+      BRE_CUDA_CHECK(cudaMemcpyAsync(sc_dev, stages[k].cj_scale, (size_t)N * C * sizeof(float), cudaMemcpyDefault, e->stream));
+      BRE_CUDA_CHECK(cudaMemcpyAsync(sh_dev, stages[k].cj_shift, (size_t)N * C * sizeof(float), cudaMemcpyDefault, e->stream));
+      pipe.plan[k].cj_scale = sc_dev; pipe.plan[k].cj_shift = sh_dev;
+    }
+    BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  }
+  e->aug_pipe = pipe;
   e->bind_input();
   return BRE_OK;
 }
 
+int bre_engine_set_augmentations(bre_engine* e, int32_t n_steps, const int32_t* kinds, const float* params, int32_t cs_enabled, float cs_shift,
+                                 int32_t cs_circular, const float* cj_scale, const float* cj_shift, int32_t differentiable, uint64_t seed) {
+  if (!e || n_steps < 0 || n_steps > AUG_MAX_STEPS || (n_steps > 0 && (!kinds || !params))) { set_error("bre_engine_set_augmentations: bad arguments"); return BRE_ERR_INVALID; }
+  if (e->ms_steps > 0) { set_error("augmentations are not supported together with local steps"); return BRE_ERR_UNSUPPORTED; }
+  const bool any = n_steps > 0 || cs_enabled || cj_scale != nullptr;
+  bre_aug_stage st;            // one PIXEL stage at the program's shape
+  memset(&st, 0, sizeof(st));
+  st.kind = BRE_AUG_PIXEL; st.n_steps = n_steps;
+  for (int s = 0; s < n_steps; ++s) { st.kinds[s] = kinds[s]; st.params[s] = params[s]; }
+  st.cs_enabled = cs_enabled; st.cs_shift = cs_shift; st.cs_circular = cs_circular;
+  st.cj_scale = cj_scale; st.cj_shift = cj_shift;
+  const bre_tensor_desc& v = e->td(0);
+  return set_stages(e, any ? 1 : 0, &st, v.N, v.C, v.H, v.W, differentiable, seed);
+}
+
+int bre_engine_set_augmentation_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage* stages, int32_t N, int32_t C, int32_t H, int32_t W,
+                                       int32_t differentiable, uint64_t seed) {
+  if (!e) { set_error("bre_engine_set_augmentation_stages: bad arguments"); return BRE_ERR_INVALID; }
+  if (!e->model_loaded) { set_error("load the model first"); return BRE_ERR_STATE; }
+  return set_stages(e, n_stages, stages, N, C, H, W, differentiable, seed);
+}
+
+static int read_draws(bre_engine* e, AugDraws* h) {
+  BRE_CUDA_CHECK(cudaSetDevice(e->device));
+  BRE_CUDA_CHECK(cudaMemcpyAsync(h, e->aug_draws, AUG_MAX_STAGES * sizeof(AugDraws), cudaMemcpyDeviceToHost, e->stream));
+  BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  return 0;
+}
+
 int bre_engine_last_augmentation(bre_engine* e, int32_t* o1, int32_t* o2, float* sx, float* sy) {
   if (!e || !e->aug_draws) { set_error("bre_engine_last_augmentation: no augmentations configured"); return BRE_ERR_STATE; }
-  BRE_CUDA_CHECK(cudaSetDevice(e->device));
-  AugDraws h;
-  BRE_CUDA_CHECK(cudaMemcpyAsync(&h, e->aug_draws, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
-  BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
-  for (int s = 0; s < AUG_MAX_STEPS; ++s) { if (o1) o1[s] = h.o1[s]; if (o2) o2[s] = h.o2[s]; }
-  for (int n = 0; n < e->xN && n < AUG_MAX_BATCH; ++n) { if (sx) sx[n] = h.sx[n]; if (sy) sy[n] = h.sy[n]; }
+  AugDraws h[AUG_MAX_STAGES];
+  BRE_TRY(read_draws(e, h));
+  int k = 0;                   // the first PIXEL stage (the only one of a plain plan)
+  while (k < e->aug_pipe.n_stages - 1 && e->aug_pipe.st[k].kind != AUG_STAGE_PIXEL) ++k;
+  for (int s = 0; s < AUG_MAX_STEPS; ++s) { if (o1) o1[s] = h[k].o1[s]; if (o2) o2[s] = h[k].o2[s]; }
+  for (int n = 0; n < e->xN && n < AUG_MAX_BATCH; ++n) { if (sx) sx[n] = h[k].sx[n]; if (sy) sy[n] = h[k].sy[n]; }
+  return BRE_OK;
+}
+
+int bre_engine_augmentation_draws(bre_engine* e, int32_t* n_stages, int32_t* o1, int32_t* o2, float* sx, float* sy) {
+  if (!e || !e->aug_draws) { set_error("bre_engine_augmentation_draws: no augmentations configured"); return BRE_ERR_STATE; }
+  AugDraws h[AUG_MAX_STAGES];
+  BRE_TRY(read_draws(e, h));
+  if (n_stages) *n_stages = e->aug_pipe.n_stages;
+  for (int k = 0; k < AUG_MAX_STAGES; ++k) {
+    for (int s = 0; s < AUG_MAX_STEPS; ++s) { if (o1) o1[k * AUG_MAX_STEPS + s] = h[k].o1[s]; if (o2) o2[k * AUG_MAX_STEPS + s] = h[k].o2[s]; }
+    for (int n = 0; n < AUG_MAX_BATCH; ++n) { if (sx) sx[k * AUG_MAX_BATCH + n] = h[k].sx[n]; if (sy) sy[k * AUG_MAX_BATCH + n] = h[k].sy[n]; }
+  }
   return BRE_OK;
 }
 

@@ -34,6 +34,14 @@ class OpDesc(ctypes.Structure):
                                   ("bn_train", ctypes.c_int32)]
 
 
+class AugStage(ctypes.Structure):   # bre_aug_stage
+    _fields_ = [("kind", ctypes.c_int32), ("n_steps", ctypes.c_int32), ("kinds", ctypes.c_int32 * 4), ("params", ctypes.c_float * 4),
+                ("cs_enabled", ctypes.c_int32), ("cs_circular", ctypes.c_int32), ("cs_shift", ctypes.c_float),
+                ("cj_scale", ctypes.c_void_p), ("cj_shift", ctypes.c_void_p)] + \
+               [(n, ctypes.c_int32) for n in ("y0", "x0", "wh", "ww", "Ho", "Wo", "focus")] + \
+               [("focus_std", ctypes.c_float), ("width", ctypes.c_int32), ("stride", ctypes.c_int32)]
+
+
 class AttackCfg(ctypes.Structure):
     _fields_ = [
         ("objective", ctypes.c_int32),
@@ -85,6 +93,7 @@ EXPORTS = [
     "bre_engine_param_gradients", "bre_engine_bn_batch_stats", "bre_engine_forward", "bre_image_mse",
     "bre_engine_begin_joint_trial", "bre_engine_get_joint_labels", "bre_resize_bilinear",
     "bre_engine_set_augmentations", "bre_engine_last_augmentation", "bre_augment_view",
+    "bre_engine_set_augmentation_stages", "bre_engine_augmentation_draws", "bre_augment_resample", "bre_augment_blur",
 ]
 
 
@@ -144,6 +153,10 @@ def load_library(path=None):
     lib.bre_engine_set_augmentations.argtypes = [vp, i32, P(i32), P(f32), i32, f32, i32, vp, vp, i32, ctypes.c_uint64]
     lib.bre_engine_last_augmentation.argtypes = [vp, P(i32), P(i32), P(f32), P(f32)]
     lib.bre_augment_view.argtypes = [vp, vp, i32, i32, i32, i32, i32, P(i32), P(i32), P(i32), f32, i32, P(f32), P(f32), vp, vp, i32, vp, vp]
+    lib.bre_engine_set_augmentation_stages.argtypes = [vp, i32, P(AugStage), i32, i32, i32, i32, i32, ctypes.c_uint64]
+    lib.bre_engine_augmentation_draws.argtypes = [vp, P(i32), P(i32), P(i32), P(f32), P(f32)]
+    lib.bre_augment_resample.argtypes = [vp, vp] + [i32] * 11 + [vp]
+    lib.bre_augment_blur.argtypes = [vp, vp] + [i32] * 7 + [vp]
     lib.bre_resize_bilinear.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, vp]
     lib.bre_image_mse.argtypes = [vp, vp, i32, i32, i32, vp, vp, i32, P(ctypes.c_double), vp]
     for name in EXPORTS:
@@ -389,9 +402,14 @@ class Engine:
         return out
 
     def set_augmentations(self, plan):
-        """``plan`` (attacks/augment.py ``AugmentationPlan``) or ``None`` to switch augmentations off."""
+        """``plan`` (attacks/augment.py ``AugmentationPlan``) or ``None`` to switch augmentations off.  A plan with ``stages`` (it
+        contains a resample or blur stage) runs the model on the view's shape, which must be this engine's program shape; the
+        candidate then has the plan's candidate shape and ``input_shape`` / ``numel`` follow it."""
+        if plan is not None and plan.stages:
+            return self._set_augmentation_stages(plan)
         if plan is None:
             _check(self.lib, self.lib.bre_engine_set_augmentations(self.h, 0, None, None, 0, 0.0, 0, None, None, 0, 0), "bre_engine_set_augmentations")
+            self._candidate_shape(None)
             return
         n = len(plan.steps)
         kinds = (ctypes.c_int32 * max(n, 1))(*[k for k, _ in plan.steps])
@@ -404,6 +422,47 @@ class Engine:
                                                                float(plan.continuous_shift or 0.0), int(plan.circular), _ptr(scale), _ptr(shift),
                                                                int(plan.differentiable), int(plan.seed) & 0xFFFFFFFFFFFFFFFF),
                "bre_engine_set_augmentations")
+        self._candidate_shape(None)
+
+    def _candidate_shape(self, shape):
+        """Candidate shape of a stage plan (``None``: back to the shape the engine was built for)."""
+        if shape is None:
+            shape, self._built_shape = getattr(self, "_built_shape", None) or self.input_shape, None
+        elif getattr(self, "_built_shape", None) is None:
+            self._built_shape = self.input_shape
+        self.input_shape = tuple(int(s) for s in shape)
+        self.numel = 1
+        for s_ in self.input_shape:
+            self.numel *= s_
+
+    def _set_augmentation_stages(self, plan):
+        from .attacks import augment as A
+
+        arr = (AugStage * len(plan.stages))()
+        keep = []
+        for st, cs in zip(plan.stages, arr):
+            cs.Ho, cs.Wo = st.out_hw
+            if st.kind == A.PIXEL:
+                cs.kind, cs.n_steps = 0, len(st.steps)
+                for i, (k, p) in enumerate(st.steps):
+                    cs.kinds[i], cs.params[i] = int(k), float(p)
+                cs.cs_enabled, cs.cs_shift, cs.cs_circular = int(st.continuous_shift is not None), float(st.continuous_shift or 0.0), int(st.circular)
+                if st.colour_scale is not None:
+                    sc, sh = _f32c(st.colour_scale, self.device), _f32c(st.colour_shift, self.device)
+                    keep += [sc, sh]
+                    cs.cj_scale, cs.cj_shift = sc.data_ptr(), sh.data_ptr()
+            elif st.kind == A.RESAMPLE:
+                cs.kind = 1
+                (cs.y0, cs.x0), (cs.wh, cs.ww) = st.corner, st.window
+                cs.focus, cs.focus_std = int(st.focus_std is not None), float(st.focus_std or 0.0)
+            else:
+                cs.kind, cs.width, cs.stride = 2, int(st.width), int(st.stride)
+        torch.cuda.synchronize(self.device)
+        self._aug_keep = tuple(keep)
+        N, Cc, H, W = plan.candidate_shape
+        _check(self.lib, self.lib.bre_engine_set_augmentation_stages(self.h, len(plan.stages), arr, N, Cc, H, W, int(plan.differentiable),
+                                                                     int(plan.seed) & 0xFFFFFFFFFFFFFFFF), "bre_engine_set_augmentation_stages")
+        self._candidate_shape(plan.candidate_shape)
 
     def last_augmentation(self):
         o1, o2 = (ctypes.c_int32 * 4)(), (ctypes.c_int32 * 4)()
@@ -411,6 +470,17 @@ class Engine:
         _check(self.lib, self.lib.bre_engine_last_augmentation(self.h, o1, o2, sx, sy), "bre_engine_last_augmentation")
         n = self.input_shape[0]
         return list(o1), list(o2), list(sx)[:n], list(sy)[:n]
+
+    def augmentation_draws(self):
+        """Every stage's draws of the last evaluation: list of dicts (o1, o2: 4 offsets; sx, sy: per image; a focus stage's window
+        corner is (o1[0], o2[0]) = (row, column))."""
+        n_st = ctypes.c_int32()
+        o1, o2 = (ctypes.c_int32 * 32)(), (ctypes.c_int32 * 32)()
+        sx, sy = (ctypes.c_float * 512)(), (ctypes.c_float * 512)()
+        _check(self.lib, self.lib.bre_engine_augmentation_draws(self.h, ctypes.byref(n_st), o1, o2, sx, sy), "bre_engine_augmentation_draws")
+        n = self.input_shape[0]
+        return [dict(o1=list(o1[4 * k:4 * k + 4]), o2=list(o2[4 * k:4 * k + 4]), sx=list(sx[64 * k:64 * k + n]), sy=list(sy[64 * k:64 * k + n]))
+                for k in range(n_st.value)]
 
     def run(self, n_iters):
         _check(self.lib, self.lib.bre_engine_run(self.h, int(n_iters)), "bre_engine_run")
@@ -615,6 +685,38 @@ def augment_view(x, steps=(), offsets=(), continuous_shift=None, circular=True, 
         rc = lib.bre_augment_view(_ptr(x), _ptr(out), N, C, H, W, n, kinds, o1, o2, float(continuous_shift or 0.0), int(circular), sx, sy, _ptr(cs),
                                   _ptr(csh), int(transpose), _ptr(scratch), ctypes.c_void_p(stream))
     _check(lib, rc, "bre_augment_view")
+    return out
+
+
+def augment_resample(x, corner, window, out_hw, transpose=False, in_hw=None):
+    """Stand-alone RESAMPLE stage: the window ``corner`` = (y0, x0), ``window`` = (wh, ww) of x [N, C, H, W] resized bilinearly to
+    ``out_hw``.  ``transpose``: x is the gradient at the view [N, C, Ho, Wo], pulled back to [N, C, *in_hw]."""
+    lib = load_library()
+    x = _f32c(x)
+    N, C = x.shape[:2]
+    Hi, Wi = (x.shape[2], x.shape[3]) if not transpose else in_hw
+    out = torch.empty((N, C, *(in_hw if transpose else out_hw)), dtype=torch.float32, device=x.device)
+    stream = torch.cuda.current_stream(x.device).cuda_stream
+    with torch.cuda.device(x.device):
+        rc = lib.bre_augment_resample(_ptr(x), _ptr(out), N, C, Hi, Wi, int(corner[0]), int(corner[1]), int(window[0]), int(window[1]),
+                                      int(out_hw[0]), int(out_hw[1]), int(bool(transpose)), ctypes.c_void_p(stream))
+    _check(lib, rc, "bre_augment_resample")
+    return out
+
+
+def augment_blur(x, width, stride=1, transpose=False, in_hw=None):
+    """Stand-alone BLUR stage (antialias); ``transpose``: x is the gradient at the view, pulled back to [N, C, *in_hw]."""
+    lib = load_library()
+    x = _f32c(x)
+    N, C = x.shape[:2]
+    Hi, Wi = (x.shape[2], x.shape[3]) if not transpose else in_hw
+    pad = width // 2
+    Ho, Wo = (Hi + 2 * pad - width) // stride + 1, (Wi + 2 * pad - width) // stride + 1
+    out = torch.empty((N, C, *((Hi, Wi) if transpose else (Ho, Wo))), dtype=torch.float32, device=x.device)
+    stream = torch.cuda.current_stream(x.device).cuda_stream
+    with torch.cuda.device(x.device):
+        rc = lib.bre_augment_blur(_ptr(x), _ptr(out), N, C, Hi, Wi, int(width), int(stride), int(bool(transpose)), ctypes.c_void_p(stream))
+    _check(lib, rc, "bre_augment_blur")
     return out
 
 

@@ -235,6 +235,41 @@ int bre_augment_view(const float* x, float* out, int32_t N, int32_t C, int32_t H
                      const int32_t* o1, const int32_t* o2, float cs_shift, int32_t cs_circular, const float* sx, const float* sy,
                      const float* cj_scale, const float* cj_shift, int32_t transpose, float* scratch, void* stream);
 
+/* The view as an ordered list of up to 8 stages, each with its own input and output shape (augment.cu):
+ *   BRE_AUG_PIXEL     a run of the shape-keeping kinds with the parameters of bre_engine_set_augmentations (n_steps, kinds,
+ *                     params, cs_*, cj_scale / cj_shift [N * C], device or host, NULL = no colour);
+ *   BRE_AUG_RESAMPLE  the window [y0, y0 + wh) x [x0, x0 + ww) resized bilinearly to Ho x Wo (F.interpolate, bilinear,
+ *                     align_corners = False): zoom (window = input), centerzoom (fixed corner), focus (focus != 0: the corner is drawn
+ *                     every evaluation as clamp(trunc(pert + in // 2 - size // 2), 0, in - size), pert uniform in [-focus_std, focus_std));
+ *   BRE_AUG_BLUR      antialias: depthwise binomial filter of `width` (1..7), zero padding width // 2, `stride`.
+ * The candidate is [N, C, H, W]; the last stage's output must be program tensor 0 (the model runs on the view).  The candidate-side
+ * state (x, optimiser moments, best, box, candidate gradient) takes the candidate's shape.  A stage list that changes the shape needs
+ * differentiable != 0.  n_stages = 0 switches augmentations off and restores the program's shape. */
+enum { BRE_AUG_PIXEL = 0, BRE_AUG_RESAMPLE = 1, BRE_AUG_BLUR = 2 };
+typedef struct bre_aug_stage {
+  int32_t kind;
+  int32_t n_steps, kinds[4];
+  float params[4];
+  int32_t cs_enabled, cs_circular;
+  float cs_shift;
+  const float* cj_scale;
+  const float* cj_shift;
+  int32_t y0, x0, wh, ww, Ho, Wo, focus;
+  float focus_std;
+  int32_t width, stride;
+} bre_aug_stage;
+int bre_engine_set_augmentation_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage* stages, int32_t N, int32_t C, int32_t H,
+                                       int32_t W, int32_t differentiable, uint64_t seed);
+/* All draws of the last evaluation, per stage k (8 x 4 offsets, 8 x 64 uniforms): PIXEL stages as bre_engine_last_augmentation,
+ * focus stages their window corner (o1[4 k], o2[4 k]) = (row, column). */
+int bre_engine_augmentation_draws(bre_engine* e, int32_t* n_stages, int32_t* o1, int32_t* o2, float* sx, float* sy);
+/* Stand-alone RESAMPLE / BLUR stage with an explicit window: transpose = 0 maps x [N, C, Hi, Wi] to the view, transpose = 1 pulls
+ * x = the gradient at the view back to out [N, C, Hi, Wi] (fixed-order gathers, bitwise reproducible). */
+int bre_augment_resample(const float* x, float* out, int32_t N, int32_t C, int32_t Hi, int32_t Wi, int32_t y0, int32_t x0, int32_t wh,
+                         int32_t ww, int32_t Ho, int32_t Wo, int32_t transpose, void* stream);
+int bre_augment_blur(const float* x, float* out, int32_t N, int32_t C, int32_t Hi, int32_t Wi, int32_t width, int32_t stride,
+                     int32_t transpose, void* stream);
+
 /* ---- the steps either side of the hot path (SURVEY.md section 8 f-2, f-3) ----------------------------------------- */
 /* User-side update production (cases/users.py:148-169 `_compute_batch_gradient`): one forward + backward of the loaded model
  * on `data` (candidate layout, device or host) with index `labels` -> gradient of the mean task loss w.r.t. every parameter,
