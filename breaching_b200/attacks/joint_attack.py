@@ -258,7 +258,7 @@ class OptimizationJointAttacker(OptimizationBasedAttacker):
         if candidate_labels.dim() == 3:      # token models: the engine works on rows = batch * seq_len
             x = x.reshape(-1, x.shape[-1], 1, 1)
         clock, t0 = self.last_timing, time.perf_counter()
-        engine.begin_joint_trial(x, candidate_labels.detach().contiguous(), table)
+        engine.begin_joint_trial(x, candidate_labels.detach().contiguous(), table, trial=trial)
         clock["trial_begin"] = clock.get("trial_begin", 0.0) + time.perf_counter() - t0
         t0 = time.perf_counter()
         T = int(self.cfg.optim.max_iterations)

@@ -263,7 +263,7 @@ class OptimizationBasedAttacker:
             if plan is not None or getattr(engine, "_aug_active", False):   # (re-setting invalidates the captured graph: only when needed)
                 engine.set_augmentations(plan)
                 engine._aug_active = plan is not None
-        engine.begin_trial(candidate, table)
+        engine.begin_trial(candidate, table, trial=trial)   # the global index: ranks sharing one noise seed still draw different fields
         callback = int(cfg_get(opt, "callback", 0) or 0)
         chunk = callback if callback > 0 else T
         total = 1 if dryrun else T

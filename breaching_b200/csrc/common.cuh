@@ -139,7 +139,7 @@ struct Scalars {
   int it;                // iterations executed (0-based index of the *next* step)
   int recorded;          // len(stats["Trial_k_Val"])
   int stopped;           // non-finite objective seen (:131-133)
-  int improved;          // scratch: this iteration improved fmin
+  int trial;             // global index of the running trial: every restart draws its own Langevin noise field
 };
 
 }  // namespace bre

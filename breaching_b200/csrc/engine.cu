@@ -306,6 +306,7 @@ struct bre_engine {
   bool graph_ready = false;
   int launch_count = 0, launches_per_iter = 0;
   bool model_loaded = false, targets_loaded = false, trial_begun = false;
+  int trial_index = 0;   // global index of the trials begun from now on (bre_engine_set_trial_index)
 
   template <typename T>
   int alloc(T** ptr, long long n) {
@@ -1495,9 +1496,16 @@ static int reset_trial_state(bre_engine* e) {
   Scalars h;
   memset(&h, 0, sizeof(h));
   h.fmin = std::numeric_limits<double>::infinity();
+  h.trial = e->trial_index;
   BRE_CUDA_CHECK(cudaMemcpyAsync(e->sc, &h, sizeof(h), cudaMemcpyHostToDevice, e->stream));
   BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));  // `h` is a stack object
   return 0;
+}
+
+int bre_engine_set_trial_index(bre_engine* e, int32_t trial) {
+  if (!e || trial < 0) { set_error("bre_engine_set_trial_index: bad arguments"); return BRE_ERR_INVALID; }
+  e->trial_index = trial;   // read by the next begin_trial into the device scalar block: no kernel argument changes, the graph stays valid
+  return BRE_OK;
 }
 
 int bre_engine_begin_trial(bre_engine* e, const float* candidate, const float* lr_table, int32_t n_lr) {
@@ -1985,6 +1993,20 @@ int bre_engine_debug_tensor(bre_engine* e, int32_t which, int32_t tensor, float*
   return BRE_OK;
 }
 
+int bre_engine_debug_step_state(bre_engine* e, int32_t which, float* out_host) {
+  if (!e || !out_host || which < 0 || which > 6) { set_error("bre_engine_debug_step_state: bad arguments"); return BRE_ERR_INVALID; }
+  if (!e->trial_begun) { set_error("bre_engine_begin_trial must be called first"); return BRE_ERR_STATE; }
+  const StepArgs a = e->step_args();
+  const float* bufs[7] = {a.grad, a.grad_task, a.m, a.v, e->label_grad, e->ell_m, e->ell_v};
+  const float* src = bufs[which];
+  if (which >= 4 && !e->joint) src = nullptr;
+  if (!src) { set_error(which == 1 ? "the step reads no separate task gradient (none needed, or folded into the candidate gradient)" : "no joint trial"); return BRE_ERR_STATE; }
+  BRE_CUDA_CHECK(cudaSetDevice(e->device));
+  BRE_CUDA_CHECK(cudaMemcpyAsync(out_host, src, (which >= 4 ? e->n_ell : a.n) * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+  BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  return BRE_OK;
+}
+
 int bre_engine_debug_op(bre_engine* e, int32_t op, int32_t* flags) {
   if (!e || !flags || op < 0 || op >= (int)e->ops.size()) return BRE_ERR_INVALID;
   e->op_flags.resize(e->ops.size(), 0);
@@ -2046,6 +2068,47 @@ int bre_match_reduce(const float* G, const float* g, const float* chunk_weights,
   BRE_CUDA_CHECK(cudaMemcpyAsync(&h, sc, sizeof(h), cudaMemcpyDeviceToHost, s));
   BRE_CUDA_CHECK(cudaStreamSynchronize(s));
   sums5_host[0] = h.dot; sums5_host[1] = h.nG; sums5_host[2] = h.ng; sums5_host[3] = h.sq; sums5_host[4] = h.l1w;
+  return BRE_OK;
+}
+
+int bre_optimizer_step(float* x, float* m, float* v, float* best, const float* grad, const float* grad_task, const float* lr_table,
+                       int32_t n_lr, const float* lo, const float* hi, int64_t n, int32_t C, int32_t HW, const bre_attack_cfg* cfg,
+                       float* history, int32_t max_hist, bre_step_scalars* io, void* stream) {
+  if (!x || !m || !v || !best || !grad || !lr_table || !cfg || !history || !io || n <= 0 || n_lr <= 0 || C <= 0 || HW <= 0 || max_hist < 0 ||
+      (cfg->boxed && (!lo || !hi)) || n % ((int64_t)C * HW) != 0) {
+    set_error("bre_optimizer_step: bad arguments");
+    return BRE_ERR_INVALID;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  Scalars h;
+  memset(&h, 0, sizeof(h));
+  h.match = io->match; h.task_loss = io->task_loss; h.tv = io->tv; h.norm = io->norm; h.di = io->di; h.feat = io->feat;
+  h.fmin = io->fmin; h.it = io->it; h.recorded = io->recorded; h.stopped = io->stopped; h.trial = io->trial;
+  Scalars* sc = nullptr; double* partials = nullptr; int* counter = nullptr;
+  int rc = dev_alloc(&sc, 1);
+  if (rc == 0) rc = dev_alloc(&partials, kStepMaxBlocks);
+  if (rc == 0) rc = dev_alloc(&counter, 1);
+  if (rc == 0 && cudaMemcpyAsync(sc, &h, sizeof(h), cudaMemcpyHostToDevice, s) != cudaSuccess) rc = BRE_ERR_CUDA;
+  StepArgs a;
+  a.x = x; a.m = m; a.v = v; a.best = best; a.grad = grad; a.grad_task = grad_task; a.lr_table = lr_table; a.n_lr = n_lr;
+  a.lo = lo; a.hi = hi; a.n = n; a.C = C; a.HW = HW; a.cfg = *cfg;
+  // the tail of bre_engine::iteration(), through the same launchers
+  if (rc == 0 && cfg->grad_clip >= 0.f) rc = launch_grad_norm(a, sc, partials, counter, s);
+  if (rc == 0) rc = launch_pixel_step(a, sc, s);
+  if (rc == 0) rc = launch_commit(sc, history, max_hist, cfg->objective_excludes_task ? 0.f : cfg->task_regularization, s);
+  if (rc == 0 && cudaMemcpyAsync(&h, sc, sizeof(h), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = BRE_ERR_CUDA;
+  if (cudaStreamSynchronize(s) != cudaSuccess && rc == 0) rc = BRE_ERR_CUDA;
+  cudaFree(sc); cudaFree(partials); cudaFree(counter);
+  if (rc == BRE_ERR_CUDA) set_error(std::string("bre_optimizer_step: ") + cudaGetErrorString(cudaGetLastError()));
+  if (rc != 0) return rc;
+  io->fmin = h.fmin; io->it = h.it; io->recorded = h.recorded; io->stopped = h.stopped;
+  io->grad_norm_sq = h.grad_norm_sq; io->last_objective = h.last_objective;
+  return BRE_OK;
+}
+
+int bre_langevin_noise(uint64_t seed, uint32_t trial, uint32_t it, uint64_t first, int64_t n, float* out, void* stream) {
+  if (!out || n <= 0) { set_error("bre_langevin_noise: bad arguments"); return BRE_ERR_INVALID; }
+  BRE_TRY(launch_langevin_noise(seed, trial, it, first, n, out, (cudaStream_t)stream));
   return BRE_OK;
 }
 

@@ -355,7 +355,9 @@ __global__ void __launch_bounds__(256) norm_prior_kernel(const float* __restrict
 }
 
 // --------------------------------------------------------------------------------------------------
-// Philox4x32-10 (counter-based RNG for the Langevin noise; same draw in grad-norm and step kernels)
+// Philox4x32-10, the counter-based generator of the Langevin noise.  Key = the 64-bit seed; counter words = (element index low,
+// element index high, iteration, trial index): the grad-norm and the step kernel recompute the same draw for an element, and
+// every (trial, iteration, element) has its own.
 // --------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
   const uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
@@ -363,8 +365,9 @@ __device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint
   const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
   c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
 }
-__device__ __forceinline__ float gaussian_noise(uint64_t seed, uint32_t it, uint64_t idx) {
-  uint32_t c[4] = {(uint32_t)idx, (uint32_t)(idx >> 32), it, 0x9E3779B9u};
+// N(0,1) by Box-Muller from the first two output words: uniforms on the open 24-bit grid ((w >> 8) + 0.5) / 2^24
+__device__ __forceinline__ float gaussian_noise(uint64_t seed, uint32_t trial, uint32_t it, uint64_t idx) {
+  uint32_t c[4] = {(uint32_t)idx, (uint32_t)(idx >> 32), it, trial};
   uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
 #pragma unroll
   for (int r = 0; r < 10; ++r) { philox_round(c, k0, k1); k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
@@ -376,8 +379,17 @@ __device__ __forceinline__ float gaussian_noise(uint64_t seed, uint32_t it, uint
 __device__ __forceinline__ float raw_gradient(const StepArgs& a, const Scalars* sc, long long i, float lr) {
   float gr = a.grad[i];
   if (a.grad_task != nullptr && a.cfg.task_regularization != 0.f) gr = fmaf(a.cfg.task_regularization, a.grad_task[i], gr);
-  if (a.cfg.langevin_noise > 0.f) gr = fmaf(a.cfg.langevin_noise * lr, gaussian_noise(a.cfg.noise_seed, (uint32_t)sc->it, (uint64_t)i), gr);
+  if (a.cfg.langevin_noise > 0.f)
+    gr = fmaf(a.cfg.langevin_noise * lr, gaussian_noise(a.cfg.noise_seed, (uint32_t)sc->trial, (uint32_t)sc->it, (uint64_t)i), gr);
   return gr;
+}
+
+// the bare N(0,1) draws of elements [first, first + n) (parity tests of the generator)
+__global__ void __launch_bounds__(256) langevin_noise_kernel(uint64_t seed, uint32_t trial, uint32_t it, uint64_t first, long long n,
+                                                             float* __restrict__ out) {
+  pdl_prologue();
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    out[i] = gaussian_noise(seed, trial, it, first + (uint64_t)i);
 }
 
 __global__ void __launch_bounds__(256) grad_norm_kernel(StepArgs a, Scalars* sc, double* partials, int* counter) {
@@ -711,7 +723,7 @@ int launch_norm_prior(const float* x, float* grad, long long n, float scale, flo
 
 static inline int step_grid(long long n) {
   long long b = (n + 255) / 256;
-  const long long cap = (long long)kNumSMs * 8;
+  const long long cap = kStepMaxBlocks;
   return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 
@@ -722,6 +734,11 @@ int launch_grad_norm(const StepArgs& a, Scalars* sc, double* partials, int* coun
 }
 int launch_pixel_step(const StepArgs& a, Scalars* sc, cudaStream_t s) {
   BRE_KLAUNCH(pixel_step_kernel, step_grid(a.n), 256, 0, s, a, sc);
+  BRE_CHECK_LAUNCH();
+  return 0;
+}
+int launch_langevin_noise(uint64_t seed, uint32_t trial, uint32_t it, uint64_t first, long long n, float* out, cudaStream_t s) {
+  BRE_KLAUNCH(langevin_noise_kernel, step_grid(n), 256, 0, s, seed, trial, it, first, n, out);
   BRE_CHECK_LAUNCH();
   return 0;
 }

@@ -46,6 +46,10 @@ struct StepArgs {   // closure tail + optimiser + projection + best-so-far (opti
 };
 int launch_grad_norm(const StepArgs& a, Scalars* sc, double* partials, int* counter, cudaStream_t s);
 int launch_pixel_step(const StepArgs& a, Scalars* sc, cudaStream_t s);
+constexpr int kStepMaxBlocks = kNumSMs * 8;    // grid cap of the two kernels above = capacity launch_grad_norm needs in `partials`
+// out[i] = the N(0,1) draw that the two kernels above scale by langevin_noise * lr and add to the gradient of element first + i
+// in iteration `it` of trial `trial` (the same device function, not a restatement)
+int launch_langevin_noise(uint64_t seed, uint32_t trial, uint32_t it, uint64_t first, long long n, float* out, cudaStream_t s);
 // label leaf of the joint attacks: q = softmax(label logits) per row; g <- q * (g - <q, g>) (chain through that softmax)
 int launch_row_softmax(const float* ell, float* q, int rows, int C, cudaStream_t s);
 int launch_softmax_chain(const float* q, float* g, int rows, int C, cudaStream_t s);

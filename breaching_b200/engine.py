@@ -42,6 +42,12 @@ class AugStage(ctypes.Structure):   # bre_aug_stage
                [("focus_std", ctypes.c_float), ("width", ctypes.c_int32), ("stride", ctypes.c_int32)]
 
 
+class StepScalars(ctypes.Structure):   # bre_step_scalars
+    _fields_ = [(n, ctypes.c_double) for n in ("match", "task_loss", "tv", "norm", "di", "feat", "fmin")] + \
+               [(n, ctypes.c_int32) for n in ("it", "recorded", "stopped", "trial")] + \
+               [("grad_norm_sq", ctypes.c_double), ("last_objective", ctypes.c_double)]
+
+
 class AttackCfg(ctypes.Structure):
     _fields_ = [
         ("objective", ctypes.c_int32),
@@ -94,6 +100,7 @@ EXPORTS = [
     "bre_engine_begin_joint_trial", "bre_engine_get_joint_labels", "bre_resize_bilinear",
     "bre_engine_set_augmentations", "bre_engine_last_augmentation", "bre_augment_view",
     "bre_engine_set_augmentation_stages", "bre_engine_augmentation_draws", "bre_augment_resample", "bre_augment_blur",
+    "bre_engine_set_trial_index", "bre_engine_debug_step_state", "bre_optimizer_step", "bre_langevin_noise",
 ]
 
 
@@ -159,6 +166,10 @@ def load_library(path=None):
     lib.bre_augment_blur.argtypes = [vp, vp] + [i32] * 7 + [vp]
     lib.bre_resize_bilinear.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, vp]
     lib.bre_image_mse.argtypes = [vp, vp, i32, i32, i32, vp, vp, i32, P(ctypes.c_double), vp]
+    lib.bre_engine_set_trial_index.argtypes = [vp, i32]
+    lib.bre_engine_debug_step_state.argtypes = [vp, i32, vp]
+    lib.bre_optimizer_step.argtypes = [vp] * 7 + [i32, vp, vp, i64, i32, i32, P(AttackCfg), vp, i32, P(StepScalars), vp]
+    lib.bre_langevin_noise.argtypes = [ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64, i64, vp, vp]
     for name in EXPORTS:
         if name not in ("bre_last_error", "bre_version", "bre_engine_destroy"):
             getattr(lib, name).restype = ctypes.c_int
@@ -376,7 +387,12 @@ class Engine:
         for s_ in self.input_shape:
             self.numel *= s_
 
-    def begin_trial(self, candidate, lr_table):
+    def set_trial_index(self, trial):
+        """Global index of the trials begun from now on: each index draws its own Langevin noise field from the engine's seed."""
+        _check(self.lib, self.lib.bre_engine_set_trial_index(self.h, int(trial)), "bre_engine_set_trial_index")
+
+    def begin_trial(self, candidate, lr_table, trial=0):
+        self.set_trial_index(trial)
         cand = _f32c(candidate)
         if cand.numel() != self.numel:
             raise EngineError(f"candidate has {cand.numel()} elements, engine expects {self.numel}")
@@ -385,8 +401,9 @@ class Engine:
             torch.cuda.synchronize(self.device)
         _check(self.lib, self.lib.bre_engine_begin_trial(self.h, _ptr(cand), _ptr(lr), lr.numel()), "bre_engine_begin_trial")
 
-    def begin_joint_trial(self, candidate, label_logits, lr_table):
+    def begin_joint_trial(self, candidate, label_logits, lr_table, trial=0):
         """Joint data + label optimisation on the device: ``label_logits`` [N, classes] (token models: [batch, seq, vocab])."""
+        self.set_trial_index(trial)
         cand, ell = _f32c(candidate, self.device), _f32c(label_logits, self.device)
         if cand.numel() != self.numel:
             raise EngineError(f"candidate has {cand.numel()} elements, engine expects {self.numel}")
@@ -619,6 +636,15 @@ class Engine:
         _check(self.lib, self.lib.bre_engine_debug_tensor(self.h, code, tid, _ptr(out)), "bre_engine_debug_tensor")
         return out
 
+    def debug_step_state(self, which):
+        """What the optimiser step of the last iteration read and left: "grad" (candidate gradient before noise / clip / sign),
+        "grad_task" (raises when the step reads no separate task gradient), "m", "v"; "label_grad" / "label_m" / "label_v" for the
+        label-logit leaf of a joint trial."""
+        code = {"grad": 0, "grad_task": 1, "m": 2, "v": 3, "label_grad": 4, "label_m": 5, "label_v": 6}[which]
+        out = torch.empty(self._label_shape if code >= 4 else self.input_shape, dtype=torch.float32)
+        _check(self.lib, self.lib.bre_engine_debug_step_state(self.h, code, _ptr(out)), "bre_engine_debug_step_state")
+        return out
+
     def debug_op(self, index):
         """What the engine did with op ``index`` in the last sweeps: dict(fused, tangent_in_unwritten, stem_columns)."""
         out = ctypes.c_int32()
@@ -646,6 +672,38 @@ def match_reduce(G, g, chunk_weights=None, mask_value=-1.0, readback=True):
                                   out if readback else None, ctypes.c_void_p(stream))
     _check(lib, rc, "bre_match_reduce")
     return list(out) if readback else None
+
+
+def optimizer_step(x, m, v, best, grad, ccfg, lr_table, history, scalars, grad_task=None, lo=None, hi=None, C=1, HW=1):
+    """One optimiser step + bookkeeping of the engine's iteration on caller-owned CUDA tensors (updated in place): the kernels
+    ``Engine.run`` launches after the sweeps.  ``ccfg``: ``AttackCfg``; ``lr_table`` / ``history`` / ``lo`` / ``hi``: CUDA fp32;
+    ``scalars``: dict(it, fmin, match, task_loss, tv, norm, di, feat, recorded, stopped, trial), missing entries 0 (fmin: +inf).
+    Returns the dict after the step, with ``grad_norm_sq`` and ``last_objective``."""
+    lib = load_library()
+    for t in (x, m, v, best, grad, lr_table, history, grad_task, lo, hi):
+        assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous())
+    io = StepScalars()
+    io.fmin = float("inf")
+    for key, val in scalars.items():
+        setattr(io, key, val)
+    stream = torch.cuda.current_stream(x.device).cuda_stream
+    with torch.cuda.device(x.device):
+        rc = lib.bre_optimizer_step(_ptr(x), _ptr(m), _ptr(v), _ptr(best), _ptr(grad), _ptr(grad_task), _ptr(lr_table), lr_table.numel(),
+                                    _ptr(lo), _ptr(hi), x.numel(), int(C), int(HW), ctypes.byref(ccfg), _ptr(history), history.numel(),
+                                    ctypes.byref(io), ctypes.c_void_p(stream))
+    _check(lib, rc, "bre_optimizer_step")
+    return {name: getattr(io, name) for name, _ in StepScalars._fields_}
+
+
+def langevin_noise(seed, trial, it, n, first=0, device="cuda"):
+    """The N(0,1) draws the step kernels use for elements ``first .. first + n`` in iteration ``it`` of trial ``trial``."""
+    lib = load_library()
+    out = torch.empty(int(n), dtype=torch.float32, device=device)
+    stream = torch.cuda.current_stream(out.device).cuda_stream
+    with torch.cuda.device(out.device):
+        rc = lib.bre_langevin_noise(int(seed) & 0xFFFFFFFFFFFFFFFF, int(trial), int(it), int(first), out.numel(), _ptr(out), ctypes.c_void_p(stream))
+    _check(lib, rc, "bre_langevin_noise")
+    return out
 
 
 def total_variation(x, scale=0.1, inner_exp=1.0, outer_exp=1.0, eps=1e-8, double_opponents=False, grad=None):

@@ -85,7 +85,7 @@ typedef struct bre_attack_cfg {
   int32_t max_iterations;         /* cfg.optim.max_iterations (soft-sign schedule + LR table length) */
   float langevin_noise;           /* :167-170 */
   float grad_clip;                /* :171-174 ; < 0 = disabled */
-  uint64_t noise_seed;            /* Philox seed for the Langevin noise */
+  uint64_t noise_seed;            /* Philox key of the Langevin noise; the counter is (element, iteration, trial index) */
   /* regularizers.py -- a scale of 0 disables the term */
   float tv_scale, tv_inner_exp, tv_outer_exp, tv_eps; int32_t tv_double_opponents;
   float norm_scale, norm_p;
@@ -145,6 +145,11 @@ int bre_engine_load_feature_targets(bre_engine* e, const float* measured, int64_
 /* Start a trial: candidate [N,C,H,W] fp32 (device or host), LR table of length n_lr (host; entry `it` is
  * the step size used by optimiser step `it`, common.py:19-38).  Resets Adam state, best-so-far, history. */
 int bre_engine_begin_trial(bre_engine* e, const float* candidate, const float* lr_table, int32_t n_lr);
+/* Global index (>= 0, default 0) of the trials begun after this call.  The Langevin noise of element i in iteration `it` is drawn
+ * from Philox(noise_seed; i, it, trial index), so restarts on one engine -- and the trials that the ranks of a multi-GPU run take
+ * from one shared list -- get independent noise fields, as the reference's per-step randn_like gives them, when each is begun under
+ * its own index; the same (seed, index) replays the same field. */
+int bre_engine_set_trial_index(bre_engine* e, int32_t trial);
 
 /* Enqueue `n_iters` iterations of optimization_based_attack.py:110-138 (closure + step + projection +
  * best-so-far + history) on the engine's stream; returns without waiting. */
@@ -199,6 +204,11 @@ int bre_engine_debug_step_param(bre_engine* e, int32_t which, int32_t step, int3
  * tangent of a conv output whose only consumer is the BN op fused into the conv's epilogue is not written in single-step
  * evaluations (it holds whatever an earlier evaluation left). */
 int bre_engine_debug_tensor(bre_engine* e, int32_t which, int32_t tensor, float* out_host);
+/* Candidate-side buffers of the optimiser step as the last iteration left them (tests), to host: which 0 = the candidate gradient
+ * the step read (before noise / clip / sign), 1 = the separate task-loss gradient (BRE_ERR_STATE when the step reads none: no
+ * task_regularization, or already folded into 0), 2 / 3 = the optimiser moments m / v (SGD: m = momentum buffer); candidate-shaped.
+ * 4 / 5 / 6 = gradient, m, v of the label-logit leaf of a joint trial ([N, classes]). */
+int bre_engine_debug_step_state(bre_engine* e, int32_t which, float* out_host);
 /* What the engine did with op `op` (tests): bit 0 = it ran in the epilogue of the preceding tensor-core GEMM in the last forward
  * sweep (fuse_bnact), bit 1 = its input tangent was not stored in the last tangent-forward sweep (that fused case), bit 2 = the
  * op runs on the column path of the candidate-fed convolution, which rounds the candidate, weight and direction to TF32 itself. */
@@ -302,6 +312,26 @@ int bre_match_reduce(const float* G, const float* g, const float* chunk_weights,
 int bre_total_variation(const float* x, float* grad, int32_t N, int32_t H, int32_t W, float scale, float inner_exp,
                         float outer_exp, float eps, int32_t double_opponents, int32_t accumulate,
                         double* value_host, void* stream);
+/* The tail of one iteration, alone: gradient post-processing (task term, Langevin noise, clip by the global norm, sign),
+ * Adam / AdamW / SGD update, box projection, best-so-far and the trial bookkeeping (optimization_based_attack.py:112-135,166-184)
+ * -- the grad-norm (when cfg->grad_clip >= 0), step and commit launches that bre_engine_run enqueues after the four sweeps -- on
+ * caller-owned device buffers.  x, m, v, best, grad: [n] fp32, n = images * C * HW; grad_task: [n] or NULL (added times
+ * cfg->task_regularization); lr_table [n_lr]: iterations >= n_lr step with 0; lo / hi [C]: box of channel (i / HW) % C, read only
+ * when cfg->boxed; history [max_hist]: entry `recorded` is written while recorded < max_hist.  `io` (host) carries the scalar
+ * state in and out; the call waits for the stream. */
+typedef struct bre_step_scalars {
+  double match, task_loss, tv, norm, di, feat; /* in: objective pieces; phi = their sum with task_loss times task_regularization
+                                                  (times 0 when cfg->objective_excludes_task) */
+  double fmin;                                 /* in / out: minimal objective so far (+inf at the start of a trial) */
+  int32_t it, recorded, stopped, trial;        /* in / out (trial: in): 0-based index of this step, history length, stop flag */
+  double grad_norm_sq, last_objective;         /* out: squared norm of the noised gradient (clip only), float(phi) */
+} bre_step_scalars;
+int bre_optimizer_step(float* x, float* m, float* v, float* best, const float* grad, const float* grad_task, const float* lr_table,
+                       int32_t n_lr, const float* lo, const float* hi, int64_t n, int32_t C, int32_t HW, const bre_attack_cfg* cfg,
+                       float* history, int32_t max_hist, bre_step_scalars* io, void* stream);
+/* out[i] (device, i < n) = the standard normal draw of element first + i in iteration `it` of trial `trial` under `seed`: what the
+ * step adds to that element's gradient, divided by langevin_noise * lr.  Same device function as the step kernels. */
+int bre_langevin_noise(uint64_t seed, uint32_t trial, uint32_t it, uint64_t first, int64_t n, float* out, void* stream);
 /* Token-sequence ops of the transformer / TAG path (language_models.py:150-205 as attacked in embedding space; SURVEY
  * section 8 rows a15 / a16), stand-alone, one call per sweep (0 forward, 1 backward, 2 tangent-forward, 3 tangent-backward;
  * rules in oracle/transformer_interp.py).  fp32 device pointers, [rows, C] row-major, rows = batch * seq_len.
