@@ -7,7 +7,8 @@
 //     reads tf32 operands K-major only.  Rather than materialise transposed copies, the consumer warps load mma.sync
 //     m16n8k8 .tf32 fragments from the swizzled stages with ld.shared (any layout is addressable that way).
 // Both consumers leave the accumulator in the same register layout (warp w: rows 16w + [0, 16) and 64 + 16w + [0, 16)),
-// so the epilogue is shared.  Operand staging, two producers:
+// so the epilogue is shared.  Launches whose m-tile holds <= 64 GEMM rows run 64-row tiles (rows 0-63 only, BM = 64).
+// Operand staging, two producers:
 //   * TMA (default wherever the geometry allows): one thread issues cp.async.bulk.tensor loads -- im2col-mode tensor
 //     maps for the gathered activation operand (the hardware walks 128 output pixels x 32 channels of one filter tap,
 //     zero-filling the padding halo), tiled maps for the weight operand -- which land directly in the 128-byte-swizzled
@@ -251,11 +252,15 @@ __device__ long long g_tc_trace[16];
 #define TC_MARK(i, cond) do { } while (0)
 #endif
 
-template <int MODE, int BN, bool TMA, bool CLS = false>
+// BM = 64 (launches whose m-tile holds <= 64 GEMM rows): the im2col box, the MMAs and the epilogue cover rows 0-63 only, and the
+// stage is half as large (see launch_igemm_tc).
+template <int MODE, int BN, bool TMA, bool CLS = false, int BM = TC_BM>
 __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d, int proxy_fence,
                                                             const __grid_constant__ std::conditional_t<CLS, TcMapsCls, TcMaps> maps, ClsPlan plan) {
   static_assert(!CLS || (MODE == GEMM_DGRAD && TMA), "per-class gathers: strided dgrad with the TMA producer only");
-  constexpr uint32_t A_BYTES = TC_BM * TC_BK * 4, B_BYTES = BN * TC_BK * 4;
+  static_assert(BM == TC_BM || (BM == 64 && TMA && !CLS && MODE != GEMM_WGRAD), "64-row tiles: fprop / stride-1 dgrad on the TMA producer");
+  constexpr int MH = BM / 64;   // wgmma M = 64 row halves
+  constexpr uint32_t A_BYTES = BM * TC_BK * 4, B_BYTES = BN * TC_BK * 4;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;                                  // [STAGES][A_BYTES]
   const int nst = 1 << d.stage_shift, stage_mask = nst - 1;
@@ -270,7 +275,7 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
   const int ptid = tid & (TC_THREADS - 1);   // index inside the producer warpgroup (warps 4-7)
   const bool consumer = warp < TC_THREADS / 32;
   const int n0 = blockIdx.y * BN, z = blockIdx.z;
-  int m0 = blockIdx.x * TC_BM;
+  int m0 = blockIdx.x * BM;
   int kb_begin = z * d.kblocks_per_split;
   int kb_end = min(d.total_kblocks, kb_begin + d.kblocks_per_split);
   const int HoWo = g.Ho * g.Wo, HW = g.H * g.W;
@@ -605,9 +610,9 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
   //      has been read.  No CTA-wide barrier inside the loop.
   // acc[h][4 j + q] = tile element (64 h + 16 w + g + 8 (q >> 1), 8 j + 2 t + (q & 1)), w = warp, g = lane / 4, t = lane % 4
   // (the wgmma m64nN accumulator fragment of half h, and the union of the mma.sync m16n8 fragments of the same elements)
-  float acc[2][BN / 2];
+  float acc[MH][BN / 2];
 #pragma unroll
-  for (int h = 0; h < 2; ++h)
+  for (int h = 0; h < MH; ++h)
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
   const int gq = lane >> 2, tq = lane & 3;
@@ -624,14 +629,14 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
 #pragma unroll
         for (int j = 0; j < TC_BK / 8; ++j) {
           const uint64_t db = wgmma_desc_k128(sb + 32 * j);
-          wgmma_tf32<BN>(acc[0], wgmma_desc_k128(sa + 32 * j), db);
-          wgmma_tf32<BN>(acc[1], wgmma_desc_k128(sa + 64 * 128 + 32 * j), db);
+#pragma unroll
+          for (int h = 0; h < MH; ++h) wgmma_tf32<BN>(acc[h], wgmma_desc_k128(sa + h * 64 * 128 + 32 * j), db);
         }
         wgmma_commit();
         // this k-block's MMAs stay in flight while the next stage is waited for; the previous stage is free once its group is
         wgmma_wait<1>();
-        fence_regs(acc[0]);
-        fence_regs(acc[1]);
+#pragma unroll
+        for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
         __syncwarp();
         if (i > 0 && lane == 0) mbar_arrive(&bar_empty[(i - 1) & stage_mask]);
       } else {
@@ -640,9 +645,9 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
 #pragma unroll
         for (int j = 0; j < TC_BK / 8; ++j) {
           const int k0 = 8 * j + tq;
-          uint32_t af[2][4];
+          uint32_t af[MH][4];
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
+          for (int h = 0; h < MH; ++h) {
             const int r = 64 * h + 16 * warp + gq;
             af[h][0] = ld_op<a_mn>(pa, r, k0);
             af[h][1] = ld_op<a_mn>(pa, r + 8, k0);
@@ -652,8 +657,8 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
 #pragma unroll
           for (int jn = 0; jn < BN / 8; ++jn) {
             const uint32_t b0 = ld_op<b_mn>(pb, 8 * jn + gq, k0), b1 = ld_op<b_mn>(pb, 8 * jn + gq, k0 + 4);
-            mma_tf32(&acc[0][4 * jn], af[0], b0, b1);
-            mma_tf32(&acc[1][4 * jn], af[1], b0, b1);
+#pragma unroll
+            for (int h = 0; h < MH; ++h) mma_tf32(&acc[h][4 * jn], af[h], b0, b1);
           }
         }
         __syncwarp();
@@ -662,8 +667,8 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
     }
     if constexpr (MODE == GEMM_FPROP) {
       wgmma_wait<0>();
-      fence_regs(acc[0]);
-      fence_regs(acc[1]);
+#pragma unroll
+      for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
     }
     TC_MARK(5, tid == 0);
   } else {
@@ -715,7 +720,7 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
   if (consumer && splits == 1) {
     // (a class no filter tap reaches has nkb = 0 and writes the zero accumulator)
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
+    for (int h = 0; h < MH; ++h) {
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int mm = m0 + 64 * h + 16 * warp + gq + 8 * hr;
@@ -760,9 +765,9 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
     // the peers' shared memory (DSMEM, ld.shared::cluster) in fixed rank order -- deterministic, no global workspace, no
     // atomics, no "last CTA" tail.
     consumer_sync();
-    float* part = reinterpret_cast<float*>(sA);  // [128 rows][BN] fp32, 16-byte chunks XOR-swizzled by (row & 15)
+    float* part = reinterpret_cast<float*>(sA);  // [BM rows][BN] fp32, 16-byte chunks XOR-swizzled by (row & 15)
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
+    for (int h = 0; h < MH; ++h) {
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int r = 64 * h + 16 * warp + gq + 8 * hr;
@@ -783,17 +788,19 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
       // Every thread owns BN/(4 S) float4 slots of this CTA's row slice and needs the S peers' copies of each: BN/4 = 16
       // remote 16-byte loads per thread whatever S is.  All of them are issued before the first is consumed (a DSMEM round
       // trip is ~0.5 us; one slot at a time made this phase 2.2 us), then summed in fixed rank order.
+      // A slice with fewer slots than threads (BM = 64, S = 8, BN = 32: 64 slots) leaves the surplus threads idle.
       auto reduce_rows = [&](auto s_tag) {
         constexpr int S = decltype(s_tag)::value;
-        constexpr int C4 = BN / 4, SLOTS = (TC_BM / S) * C4 / TC_THREADS > 0 ? (TC_BM / S) * C4 / TC_THREADS : 1;
+        constexpr int C4 = BN / 4, NSLOT = (BM / S) * C4, SLOTS = NSLOT / TC_THREADS > 0 ? NSLOT / TC_THREADS : 1;
         const uint32_t part_s = smem_u32(sA);
         float4 t[SLOTS][S];
         int rr[SLOTS], cc[SLOTS];
 #pragma unroll
         for (int sl = 0; sl < SLOTS; ++sl) {
           const int slot = tid + sl * TC_THREADS;
-          rr[sl] = z * (TC_BM / S) + slot / C4;
+          rr[sl] = z * (BM / S) + slot / C4;
           cc[sl] = slot % C4;
+          if (NSLOT < TC_THREADS && slot >= NSLOT) continue;
           const uint32_t local = part_s + (uint32_t)(rr[sl] * BN + ((cc[sl] ^ (rr[sl] & (BN / 4 - 1) & 15)) << 2)) * 4u;
 #pragma unroll
           for (int q = 0; q < S; ++q) t[sl][q] = ld_dsmem4(local, (uint32_t)q);
@@ -801,7 +808,7 @@ __global__ void __launch_bounds__(TC_BLOCK) igemm_tc_kernel(GemmArgs a, TcDims d
 #pragma unroll
         for (int sl = 0; sl < SLOTS; ++sl) {
           const int r = rr[sl], c4 = cc[sl];
-          if (m0 + r >= Mrows) continue;
+          if ((NSLOT < TC_THREADS && tid + sl * TC_THREADS >= NSLOT) || m0 + r >= Mrows) continue;
           float4 acc4 = t[sl][0];
 #pragma unroll
           for (int q = 1; q < S; ++q) { acc4.x += t[sl][q].x; acc4.y += t[sl][q].y; acc4.z += t[sl][q].z; acc4.w += t[sl][q].w; }
@@ -945,13 +952,14 @@ bool tma_eligible(const GemmArgs& a) {
   return true;
 }
 
-bool build_maps(const GemmArgs& a, int BN, TcMaps* maps) {
+// BM: pixels per im2col box (the tile's rows; part of the map's cache key)
+bool build_maps(const GemmArgs& a, int BN, TcMaps* maps, int BM = TC_BM) {
   const ConvGeom& g = a.g;
   const CUtensorMapSwizzle K128 = CU_TENSOR_MAP_SWIZZLE_128B;
   for (int s = 0; s < a.nsrc; ++s) {
     if (a.mode == GEMM_FPROP) {
       if (!im2col_map(&maps->act[s], a.act[s], g.N, g.H, g.W, g.Ci, a.x_sN, a.x_sP, -g.pad, -g.pad, g.pad - (g.S - 1), g.pad - (g.R - 1),
-                      g.stride, TC_BK, TC_BM, K128))
+                      g.stride, TC_BK, BM, K128))
         return false;
       const long long K = (long long)g.R * g.S * g.Ci;
       const long long dims[2] = {K, g.Co}, strides[1] = {K};
@@ -961,7 +969,7 @@ bool build_maps(const GemmArgs& a, int BN, TcMaps* maps) {
       // rows = pixels of the input gradient; the gathered tensor is dout [N][Ho][Wo][Co]; tap (r, s) reads (y + pad - r, x + pad - s)
       const int lw = g.pad - (g.S - 1), lh = g.pad - (g.R - 1);
       if (!im2col_map(&maps->act[s], a.act[s], g.N, g.Ho, g.Wo, g.Co, (long long)g.Ho * g.Wo * g.Co, g.Co, lw, lh, lw + g.W - g.Wo,
-                      lh + g.H - g.Ho, 1, TC_BK, TC_BM, K128))
+                      lh + g.H - g.Ho, 1, TC_BK, BM, K128))
         return false;
       const long long dims[3] = {g.Ci, (long long)g.R * g.S, g.Co}, strides[2] = {g.Ci, (long long)g.R * g.S * g.Ci};
       const int box[3] = {32, 1, TC_BK};
@@ -1047,7 +1055,7 @@ bool build_cls(const GemmArgs& a, ClsPlan* plan, TcMapsCls* maps) {
   return n > 0;
 }
 
-template <int MODE, int BN, bool TMA, bool CLS = false>
+template <int MODE, int BN, bool TMA, bool CLS = false, int BM = TC_BM>
 int launch_tc(const GemmArgs& a, const TcDims& d0, const std::conditional_t<CLS, TcMapsCls, TcMaps>& maps, cudaStream_t stream,
               const ClsPlan* plan_in = nullptr) {
   TcDims d = d0;
@@ -1055,7 +1063,7 @@ int launch_tc(const GemmArgs& a, const TcDims& d0, const std::conditional_t<CLS,
   memset(&plan, 0, sizeof(plan));
   if (CLS) plan = *plan_in;
   // CLS: the m-tiles of all classes side by side; the k extent that sizes the split is the largest class's
-  const int tm = CLS ? plan.tile0[plan.ncls] : ceil_div(d.M, TC_BM), tn = d.Nc / BN;
+  const int tm = CLS ? plan.tile0[plan.ncls] : ceil_div(d.M, BM), tn = d.Nc / BN;
   if (CLS) {
     int kmax = 0;
     for (int c = 0; c < plan.ncls; ++c) kmax = kmax > plan.Ty[c] * plan.Tx[c] ? kmax : plan.Ty[c] * plan.Tx[c];
@@ -1088,13 +1096,17 @@ int launch_tc(const GemmArgs& a, const TcDims& d0, const std::conditional_t<CLS,
   // memory so more CTAs share an SM and the per-CTA prologue / epilogue overlap (BRE_TC_SHORTK_STAGES=4 turns it off)
   static const int shortk_env = [] { const char* e = getenv("BRE_TC_SHORTK_STAGES"); return e ? atoi(e) : 2; }();
   const bool shortk = shortk_env == 2 && d.kblocks_per_split <= 6 && tm == 1 && tiles * splits > 2LL * kNumSMs;
-  const int stages = (stages_env == 8 || stages_env == 2) ? stages_env : (shortk ? 2 : TC_STAGES);
+  // 64-row tiles stage half the bytes per k-block, so an 8-deep ring (fprop 128 KB, 128 x 32 dgrad 96 KB) still leaves room for one
+  // 96 KB CTA of the successor.  It pays on launches that are one wave or less and whose CTAs walk long k-ranges: there the k-loop
+  // is the latency of the ring round trip divided by the k-blocks in flight.
+  const bool deep = BM == 64 && tiles * splits <= kNumSMs && d.kblocks_per_split >= 16;
+  const int stages = (stages_env == 8 || stages_env == 2 || stages_env == 4) ? stages_env : (shortk ? 2 : (deep ? 8 : TC_STAGES));
   d.stage_shift = stages == 8 ? 3 : (stages == 2 ? 1 : 2);
-  const size_t smem = (size_t)stages * (TC_BM + BN) * TC_BK * 4;
-  const size_t smem_max = (size_t)TC_MAX_STAGES * (TC_BM + BN) * TC_BK * 4;
+  const size_t smem = (size_t)stages * (BM + BN) * TC_BK * 4;
+  const size_t smem_max = (size_t)TC_MAX_STAGES * (BM + BN) * TC_BK * 4;
   static bool attr_done = false;
   if (!attr_done) {
-    BRE_CUDA_CHECK(cudaFuncSetAttribute(igemm_tc_kernel<MODE, BN, TMA, CLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+    BRE_CUDA_CHECK(cudaFuncSetAttribute(igemm_tc_kernel<MODE, BN, TMA, CLS, BM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
     attr_done = true;
   }
   static const int proxy_fence_env = [] {
@@ -1105,9 +1117,13 @@ int launch_tc(const GemmArgs& a, const TcDims& d0, const std::conditional_t<CLS,
     if (nprod < 1 || nprod > 4) nprod = 2;
     return (e && atoi(e) ? 1 : 0) | ((pf ? atoi(pf) : 1) ? 2 : 0) | (nprod << 2);
   }();
+  // At most one producer lane per ring stage: a lane that shares a stage with another one could wait on the "empty" parity of a
+  // phase two rounds old, which reads as complete, and overwrite a stage still in use (BRE_TC_PRODUCERS=4 with a 2-deep ring).
+  int proxy_fence = proxy_fence_env;
+  if (((proxy_fence >> 2) & 7) > stages) proxy_fence = (proxy_fence & 3) | (stages << 2);
   {
-    cudaError_t lerr = launch_kernel(igemm_tc_kernel<MODE, BN, TMA, CLS>, dim3(tm, tn, splits), dim3(TC_BLOCK), smem, stream, splits, a, d,
-                                     proxy_fence_env, maps, plan);
+    cudaError_t lerr = launch_kernel(igemm_tc_kernel<MODE, BN, TMA, CLS, BM>, dim3(tm, tn, splits), dim3(TC_BLOCK), smem, stream, splits, a, d,
+                                     proxy_fence, maps, plan);
     if (lerr != cudaSuccess) { set_error(std::string("igemm_tc launch failed: ") + cudaGetErrorString(lerr)); return -2; }
   }
   BRE_CHECK_LAUNCH();
@@ -1172,11 +1188,24 @@ int launch_igemm_tc(const GemmArgs& a, cudaStream_t stream) {
   const long long wide_tiles = (long long)ceil_div(d.M, TC_BM) * (d.Nc / 64);
   const bool underfilled = a.mode != GEMM_FPROP && d.Nc % 64 == 0 && wide_tiles * 16 <= kNumSMs && d.total_kblocks >= 64 &&
                            narrow_tiles_ok(a);
-  if (d.Nc % 64 != 0 || (underfilled && build_maps(a, 32, &maps))) {
-    if (d.Nc % 64 != 0 && !build_maps(a, 32, &maps)) { set_error("igemm_tc: tensor-map encoding failed for a narrow-tile shape"); return -4; }
-    if (a.mode == GEMM_FPROP) return launch_tc<GEMM_FPROP, 32, true>(a, d, maps, stream);
-    if (a.mode == GEMM_DGRAD) return launch_tc<GEMM_DGRAD, 32, true>(a, d, maps, stream);
+  // 64-row tiles for an m-tile of <= 64 GEMM rows (batch 1: every 7 x 7 layer-4 launch, M = 49): a 128-row im2col box would stage
+  // 64+ rows past the end of the tensor every k-block.  Rows 0-63 see the same wgmma / mma.sync instructions on the same operands,
+  // the tile count, split and k-ranges do not change (ceil(M / 64) = ceil(M / 128) = 1), so the result is bitwise that of
+  // 128-row tiles.  BRE_TC_STREAM=0 keeps 128-row tiles.
+  static const int stream_env = [] { const char* e = getenv("BRE_TC_STREAM"); return e ? atoi(e) : 1; }();
+  const bool rows64 = stream_env && d.M <= 64 && (a.mode == GEMM_FPROP || a.mode == GEMM_DGRAD) && tma_eligible(a);
+  if (d.Nc % 64 != 0 || (underfilled && build_maps(a, 32, &maps, rows64 ? 64 : TC_BM))) {
+    if (d.Nc % 64 != 0 && !build_maps(a, 32, &maps, rows64 ? 64 : TC_BM)) {
+      set_error("igemm_tc: tensor-map encoding failed for a narrow-tile shape");
+      return -4;
+    }
+    if (a.mode == GEMM_FPROP) return rows64 ? launch_tc<GEMM_FPROP, 32, true, false, 64>(a, d, maps, stream) : launch_tc<GEMM_FPROP, 32, true>(a, d, maps, stream);
+    if (a.mode == GEMM_DGRAD) return rows64 ? launch_tc<GEMM_DGRAD, 32, true, false, 64>(a, d, maps, stream) : launch_tc<GEMM_DGRAD, 32, true>(a, d, maps, stream);
     return launch_tc<GEMM_WGRAD, 32, true>(a, d, maps, stream);
+  }
+  if (rows64 && build_maps(a, 64, &maps, 64)) {
+    if (a.mode == GEMM_FPROP) return launch_tc<GEMM_FPROP, 64, true, false, 64>(a, d, maps, stream);
+    return launch_tc<GEMM_DGRAD, 64, true, false, 64>(a, d, maps, stream);
   }
   const bool tma = tma_eligible(a) && build_maps(a, 64, &maps);
   if (a.mode == GEMM_FPROP) return tma ? launch_tc<GEMM_FPROP, 64, true>(a, d, maps, stream) : launch_tc<GEMM_FPROP, 64, false>(a, d, maps, stream);

@@ -75,6 +75,19 @@ def split_plan(mode, g, nsrc):
     return tiles, bn, splits, -(-kb // splits)
 
 
+def ring_plan(mode, g, nsrc):
+    """(tile rows, ring depth) as launch_igemm_tc / launch_tc choose them (honouring BRE_TC_STREAM and BRE_TC_STAGES)."""
+    N, H, W, Ci, Co, R, st, pd = g
+    M, Nc, K = gemm_shape(mode, g)
+    tiles, bn, splits, kbc = split_plan(mode, g, nsrc)
+    stream = int(os.environ.get("BRE_TC_STREAM", "1")) != 0
+    bm = 64 if stream and M <= 64 and (mode == 0 or (mode == 1 and st == 1)) else BM
+    shortk = kbc <= 6 and tiles == Nc // bn and tiles * splits > 2 * NUM_SMS
+    deep = bm == 64 and tiles * splits <= NUM_SMS and kbc >= 16
+    forced = int(os.environ.get("BRE_TC_STAGES", "0"))
+    return bm, forced if forced in (2, 4, 8) else (2 if shortk else 8 if deep else 4)
+
+
 def launches_of(prog, dev):
     """(label, mode, geometry, nsrc, thunk, keep-alive tensors) for every GEMM launch of one iteration, in bench.py's order."""
     import bench
@@ -183,23 +196,26 @@ def main():
     bbuild.build()
     torch.manual_seed(0)
     os.makedirs(args.out, exist_ok=True)
-    gpu = dict(name=torch.cuda.get_device_name(dev), BRE_TC_MAX_SPLITS=os.environ.get("BRE_TC_MAX_SPLITS"))
+    gpu = dict(name=torch.cuda.get_device_name(dev), BRE_TC_MAX_SPLITS=os.environ.get("BRE_TC_MAX_SPLITS"),
+               BRE_TC_STREAM=os.environ.get("BRE_TC_STREAM"))
 
     import bench
 
     prog = bench.EngineRunner(2, bench.build_case(2), dev, "tc", 0).prog
     rows = []
-    print(f"{'launch':38s} {'M x N x K':>20s} {'tiles':>7s} {'splits':>6s} {'kb/CTA':>6s} {'us':>8s}")
+    print(f"{'launch':38s} {'M x N x K':>20s} {'tiles':>10s} {'stages':>6s} {'splits':>6s} {'kb/CTA':>6s} {'us':>8s}")
     for label, mode, g, nsrc, fn, _keep in launches_of(prog, dev):
         M, Nc, K = gemm_shape(mode, g)
         us = time_launch(fn, dev, args.repeats)
         if g[1] == 1 and g[2] == 1:   # the classification head: linear_small kernels, not the tensor-core GEMM
-            tiles = bn = splits = kbc = 0
+            tiles = bm = bn = stages = splits = kbc = 0
         else:
             tiles, bn, splits, kbc = split_plan(mode, g, nsrc)
-        rows.append(dict(launch=label, mode=mode, geom=list(g), nsrc=nsrc, M=M, N=Nc, K=K * nsrc, tiles=tiles, tile_n=bn, splits=splits,
-                         kblocks_per_cta=kbc, us=us))
-        print(f"{label:38s} {f'{M} x {Nc} x {K * nsrc}':>20s} {f'{tiles}x{bn}':>7s} {splits:6d} {kbc:6d} {us:8.2f}", flush=True)
+            bm, stages = ring_plan(mode, g, nsrc)
+        rows.append(dict(launch=label, mode=mode, geom=list(g), nsrc=nsrc, M=M, N=Nc, K=K * nsrc, tiles=tiles, tile_m=bm, tile_n=bn,
+                         stages=stages, splits=splits, kblocks_per_cta=kbc, us=us))
+        print(f"{label:38s} {f'{M} x {Nc} x {K * nsrc}':>20s} {f'{tiles}x{bm}x{bn}':>10s} {stages:6d} {splits:6d} {kbc:6d} {us:8.2f}",
+              flush=True)
     total = sum(r["us"] for r in rows)
     print(f"sum over {len(rows)} launches: {total:.1f} us")
     with open(os.path.join(args.out, "gemm_launches.json"), "w") as f:
