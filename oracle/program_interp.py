@@ -25,9 +25,10 @@ from breaching_b200 import compiler as C
 from oracle import transformer_interp as TI
 
 
-def objective_direction(kind, G, g, scale=1.0, tag_scale=0.1, scale_scheme="linear", fudge=1e-7, mask_value=1e-6):
+def objective_direction(kind, G, g, scale=1.0, tag_scale=0.1, scale_scheme="linear", fudge=1e-7, mask_value=1e-6, weights=None):
     """Return ``(value, v)`` with ``v_l = d value / d G_l`` for the matching objectives of
-    ``attacks/auxiliaries/objectives.py`` (closed forms; SURVEY.md section 7.3)."""
+    ``attacks/auxiliaries/objectives.py`` (closed forms; SURVEY.md section 7.3).  ``weights``: explicit per-tensor weights of
+    tag-euclidean instead of those of ``scale_scheme``."""
     dot = sum((a * b).sum() for a, b in zip(G, g))
     if kind == "euclidean":
         val = 0.5 * sum((a - b).pow(2).sum() for a, b in zip(G, g)) * scale
@@ -37,7 +38,9 @@ def objective_direction(kind, G, g, scale=1.0, tag_scale=0.1, scale_scheme="line
         return val, [0.5 * scale * torch.sign(a - b) for a, b in zip(G, g)]
     if kind == "tag-euclidean":
         L = len(G)
-        if scale_scheme == "linear":
+        if weights is not None:
+            w = torch.as_tensor(weights, dtype=G[0].dtype)
+        elif scale_scheme == "linear":
             w = torch.arange(L, 0, -1, dtype=G[0].dtype) / L
         elif scale_scheme == "exp":
             w = torch.arange(L, 0, -1, dtype=G[0].dtype).softmax(dim=0)

@@ -68,6 +68,39 @@ the lowest op index), where the buffer becomes final.
 
 The vision cross-entropy seed takes soft targets (a float ``labels`` tensor [N, classes]) as well as class indices.
 
+Objective terms (``check_terms``; the six scalars of ``Engine.last_terms()`` and the returned objective).  Every term is
+recomputed in float64 from the engine's own inputs to it (the stored G, the stored logits, the stored candidate / view, the
+stored BN and feature inputs), with the configuration scalars at the fp32 values the kernels read; the bounds are first order:
+
+  * ``match``: ``match_reduce_kernel`` forms the five sums dot = sum G g, nG = sum G^2, ng = sum g^2, sq = sum (G - g)^2 and
+    l1w = sum w |G - g| (w: the tensor's tag-euclidean weight, 1 otherwise; masked-cosine drops every element with
+    ``|g| <= float32(1e-6)`` from all five) over groups of 4 elements in fp32 before a double reduction, and rounds G - g once:
+    each sum S_k is off by at most ``e_k = (4 2^-23 + n 2^-53) A_k`` (A_k = the sum of its |terms|; n terms in the double
+    reduction), sq and l1w by ``2u A`` / ``u A`` more for the rounded difference.  ``finalize_objective`` in double: euclidean
+    ``s sq / 2`` (bound ``|s| e_sq / 2``), l1 ``s l1w / 2``, tag-euclidean ``s (sq + t l1w) / 2``, the cosine kinds
+    ``s (1 - c)`` with ``c = dot / sqrt(nG ng)``, ``|dc| <= e_dot / sqrt(nG ng) + |c| (e_nG / nG + e_ng / ng) / 2``, angular
+    ``s acos(c) / pi`` with the chain factor ``1 / (pi sqrt(1 - c^2))`` (c clamped to the fudge interval; zero outside it);
+  * ``task_loss``: the mean over rows of ``-sum_c q_c (z_c - lse)`` (q one-hot for class indices): per row the fp32 max,
+    ``expf`` of the shifted logits summed in double, ``logf`` and a few roundings cost
+    ``sum_c |q_c| ((16 + 2 rng) u + 4 u (|z_c - max| + |max| + |log sum|)) + 2 u |l_n|`` (rng = the row's logit range, as for
+    the seeds), and the mean is rounded to fp32 (``u |L|``);
+  * ``total_variation`` / ``norm``: per point the fp32 differences (exact for plain channels by Sterbenz up to one rounding;
+    the double-opponent planes carry the rounding of their own difference), ``|d| + eps``, the powers and the sum
+    ``(A^p + B^p)^q``; every power other than an exponent of 1 costs ``POW_C u`` relative (``POW_C = 8``: CUDA's ``powf`` is
+    within 4 ulp; squares and square roots are within it), every add / subtract one ``u``; propagated to first order
+    through p and q and summed with the double reduction's ``n 2^-53``; the norm ``s / p mean(x^p)`` costs ``POW_C u |x|^p``
+    per element;
+  * ``deep_inversion``: per BN layer ``mult (||rv - var|| + ||rm - mean||)`` from the batch mean and biased variance of the
+    stored BN input (``mult = float32(scale x first_bn_multiplier)`` at the first BN layer), with the bound of the fp32
+    statistics used for the DeepInversion adjoint: ``|mult| TRAIN_C (M + 8) u (nm kap_m + nv kap_v)``;
+  * ``features``: ``s mean((f - m)^2)`` from the stored input of the last linear layer, the difference rounded to fp32 and
+    squared and summed in double: ``|s| (2u + n 2^-53) mean((f - m)^2)``;
+  * the returned objective: exactly ``match + tv + norm + di + features (+ float32(tau) task_loss)``, summed in that order in
+    double (``bre_engine_objective_and_gradient``).
+
+``check_score(score, kind)``: ``Engine.score`` returns the fp32 rounding of the match term with scale 1 of the G it left
+(``D`` for a multi-step engine), within the match bound plus ``u |match|``.
+
 A buffer source provides ``tensor(which, tid)`` (``which`` in val / delta / tangent / tangent_delta, NCHW, ``None`` where a
 tensor has no such buffer), ``param(which, index)`` (G / v_operand / W_operand, torch layout; multi-step steps also v and TG), ``unwritten`` (tensor ids whose
 tangent is not stored because the BN op reading it ran in the producing GEMM's epilogue; that pair is then checked as one)
@@ -85,6 +118,71 @@ U2 = 2.0 ** -23         # 2u per accumulation step
 TF32_HALF = 2.0 ** -11  # half a TF32 ulp, relative
 TINY = 1e-30
 TRAIN_C = 8.0           # stated constant of the composite train-mode BN / DeepInversion bounds
+POW_C = 8.0             # stated constant of one fp32 power (powf: 4 ulp), in units of u
+D53 = 2.0 ** -53        # one double rounding
+MASK_VALUE = float(torch.tensor(1e-6, dtype=torch.float32))   # masked-cosine threshold as the kernels compare it
+TERMS = ("match", "task_loss", "total_variation", "norm", "deep_inversion", "features")
+
+
+def f32(v):
+    """The fp32 value of a configuration scalar, as the kernels read it."""
+    return float(torch.tensor(float(v), dtype=torch.float32))
+
+
+def tag_weights(L, scheme):
+    """Per-tensor weights of tag-euclidean as the attack hands them to the engine (fp32; objectives.py:115-124)."""
+    if scheme == "linear":
+        return torch.arange(L, 0, -1, dtype=torch.float32) / L
+    if scheme == "exp":
+        w = torch.arange(L, 0, -1, dtype=torch.float32).softmax(dim=0)
+        return w / w[0]
+    return torch.ones(L)
+
+
+def match_sums(G, g, kind, weights=None):
+    """The five sums of ``match_reduce_kernel`` in float64 and their error bounds: ({dot, nG, ng, sq, l1w}, {same: bound})."""
+    masked = kind == "masked-cosine-similarity"
+    S = dict(dot=0.0, nG=0.0, ng=0.0, sq=0.0, l1w=0.0)
+    A = dict(S)
+    n = 0
+    for j, (a, b) in enumerate(zip(G, g)):
+        a, b = a.double().flatten(), b.double().flatten()
+        if masked:
+            keep = (b.to(torch.float32).abs() > MASK_VALUE).double()
+            a, b = a * keep, b * keep
+        w = 1.0 if weights is None else float(weights[j])
+        d = a - b
+        terms = dict(dot=a * b, nG=a * a, ng=b * b, sq=d * d, l1w=w * d.abs())
+        for k, t in terms.items():
+            S[k] += float(t.sum())
+            A[k] += float(t.abs().sum())
+        n += a.numel()
+    rel = 4 * U2 + n * D53
+    E = {k: rel * A[k] for k in S}
+    E["sq"] += 2 * U * A["sq"]
+    E["l1w"] += U * A["l1w"]
+    return S, E
+
+
+def match_value(kind, S, E, scale, tag_scale=0.1, fudge=1e-7):
+    """``finalize_objective`` in float64 on the sums ``S`` and its first-order bound from the sum errors ``E``."""
+    s = abs(scale)
+    if kind == "euclidean":
+        return 0.5 * scale * S["sq"], 0.5 * s * E["sq"]
+    if kind == "l1":
+        return 0.5 * scale * S["l1w"], 0.5 * s * E["l1w"]
+    if kind == "tag-euclidean":
+        return 0.5 * scale * (S["sq"] + tag_scale * S["l1w"]), 0.5 * s * (E["sq"] + abs(tag_scale) * E["l1w"])
+    den = (S["nG"] * S["ng"]) ** 0.5
+    c = S["dot"] / den
+    dc = E["dot"] / den + abs(c) * 0.5 * (E["nG"] / S["nG"] + E["ng"] / S["ng"])
+    if kind == "angular":
+        lo, hi = -1.0 + fudge, 1.0 - fudge
+        cc = min(max(c, lo), hi)
+        inside = lo < c < hi
+        return torch.acos(torch.tensor(cc, dtype=torch.float64)).item() / torch.pi * scale, \
+            (s * dc / (torch.pi * (1.0 - cc * cc) ** 0.5) if inside else 0.0)
+    return (1.0 - c) * scale, s * dc
 
 
 def rna(t):
@@ -666,23 +764,31 @@ class SweepChecker:
         self._cmp(i, "B", f"G[{op.beta}] (BN beta gradient)", self.Pm("G", op.beta), du.sum(dim=(0, 2, 3)),
                   (Pch + 4) * U2 * du.abs().sum(dim=(0, 2, 3)))
 
-    def _di_adjoint(self, i, op, z):
-        """DeepInversion adjoint at the input of BN op i (program_interp.deep_inversion, engine statistics of ``z``)."""
-        di = self.obj["di"]
-        first = min(j for j, o in enumerate(self.prog.ops) if o.kind == C.OP_BNACT and o.has_bn)
-        mult = di["scale"] * (di.get("first_bn_multiplier", 10.0) if i == first else 1.0)
+    def _first_bn(self):
+        return min(j for j, o in enumerate(self.prog.ops) if o.kind == C.OP_BNACT and o.has_bn)
+
+    def _di_layer(self, i, z):
+        """Batch statistics of the BN input ``z`` of op i against the running statistics: (M, mean, var, nm, nv, kap_m, kap_v),
+        kap_m / kap_v the conditioning of the fp32 statistics (P = M terms) and of the norms of their differences."""
         rm, rv = self.bn[i]
         M = z.shape[0] * z.shape[2] * z.shape[3]
         mean = z.mean(dim=(0, 2, 3))
         var = z.var(dim=(0, 2, 3), unbiased=False)
         nv, nm = torch.norm(rv - var, 2), torch.norm(rm - mean, 2)
+        kap_m = 1.0 + (mean.abs().norm() + rm.norm()) / nm
+        kap_v = 1.0 + ((z * z).mean(dim=(0, 2, 3)).norm() + rv.norm()) / nv
+        return M, mean, var, nm, nv, kap_m, kap_v
+
+    def _di_adjoint(self, i, op, z):
+        """DeepInversion adjoint at the input of BN op i (program_interp.deep_inversion, engine statistics of ``z``)."""
+        di = self.obj["di"]
+        mult = di["scale"] * (di.get("first_bn_multiplier", 10.0) if i == self._first_bn() else 1.0)
+        rm, rv = self.bn[i]
+        M, mean, var, nm, nv, kap_m, kap_v = self._di_layer(i, z)
         cm = (mean - rm) / nm / M
         cv = (var - rv) / nv * 2.0 / M
         v = lambda t: t.view(1, -1, 1, 1)  # noqa: E731
         adj = mult * (v(cm) + v(cv) * (z - v(mean)))
-        # fp32 batch statistics (P = M terms) and the norms of their differences to the running statistics
-        kap_m = 1.0 + (mean.abs().norm() + rm.norm()) / nm
-        kap_v = 1.0 + ((z * z).mean(dim=(0, 2, 3)).norm() + rv.norm()) / nv
         mag = abs(mult) * (v(cm.abs()) * kap_m + v(cv.abs()) * kap_v * ((z - v(mean)).abs() + v(mean.abs()) + z.abs()))
         return adj, TRAIN_C * (M + 8) * U * mag
 
@@ -718,9 +824,13 @@ class SweepChecker:
         _, v = objective_direction(o["kind"], G, self.g, scale=o["scale"], **kw)
         s = abs(o["scale"])
         if o["kind"] in ("cosine-similarity", "angular", "fast-cosine-similarity", "masked-cosine-similarity"):
-            nG = sum(a.pow(2).sum() for a in G).sqrt()
-            ng = sum(b.pow(2).sum() for b in self.g).sqrt()
-            al, be = 1.0 / (nG * ng), abs(sum((a * b).sum() for a, b in zip(G, self.g))) / (nG.pow(3) * ng)
+            Gs, gs = G, self.g
+            if o["kind"] == "masked-cosine-similarity":   # the kernels' coefficients come from the masked sums
+                keep = [(b.to(torch.float32).abs() > MASK_VALUE).double() for b in self.g]
+                Gs, gs = [a * k for a, k in zip(G, keep)], [b * k for b, k in zip(self.g, keep)]
+            nG = sum(a.pow(2).sum() for a in Gs).sqrt()
+            ng = sum(b.pow(2).sum() for b in gs).sqrt()
+            al, be = 1.0 / (nG * ng), abs(sum((a * b).sum() for a, b in zip(Gs, gs))) / (nG.pow(3) * ng)
             if o["kind"] == "angular":   # chain factor d acos(c) / dc
                 c = float(sum((a * b).sum() for a, b in zip(G, self.g)) / (nG * ng))
                 al, be = al / (torch.pi * max(1.0 - c * c, 1e-14) ** 0.5), be / (torch.pi * max(1.0 - c * c, 1e-14) ** 0.5)
@@ -728,8 +838,9 @@ class SweepChecker:
         elif o["kind"] == "l1":    # 0.5 s sign(G - g): exact in fp32
             mags = [0.5 * s * torch.ones_like(a) for a in G]
         else:
-            # euclidean s (G - g) and tag-euclidean s ((G - g) + tag_scale / 2 w_l sign(G - g)): one rounded difference, one product
-            # (and one fma), each relative to the magnitudes of its terms
+            # euclidean s (G - g) and tag-euclidean s ((G - g) + tag_scale / 2 w_l sign(G - g)): make_v_kernel evaluates
+            # fma(-s, g, fma(s, G, c3 w sign(G - g))) -- the difference G - g is never rounded on its own, so each of the two
+            # roundings is relative to s (|G| + |g|) + c3 w, not to s |G - g| (which vanishes where G and g agree)
             L = len(G)
             w = [0.0] * L
             if o["kind"] == "tag-euclidean":
@@ -742,7 +853,7 @@ class SweepChecker:
                 else:
                     w = [1.0] * L
                 w = [0.5 * o.get("tag_scale", 0.1) * wl for wl in w]
-            mags = [s * ((a - b).abs() + wl) for a, b, wl in zip(G, self.g, w)]
+            mags = [s * (a.abs() + b.abs() + wl) for a, b, wl in zip(G, self.g, w)]
         for j in range(n):
             y = self.Pm("v_operand", j)
             bound = 16 * U * mags[j] + (TF32_HALF * v[j].abs() if on_grid(y) else 0.0)
@@ -904,6 +1015,127 @@ class SweepChecker:
             raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
         return self.findings
 
+    # ------------------------------------------------------------------ objective terms
+    def _match_term(self, G, kind, scale):
+        o = self.obj
+        w = tag_weights(len(G), o.get("scale_scheme", "linear")) if kind == "tag-euclidean" else None
+        S, E = match_sums(G, self.g, kind, w)
+        val, bound = match_value(kind, S, E, f32(scale), f32(o.get("tag_scale", 0.1)), f32(1e-7))
+        return val, bound + 16 * D53 * (abs(val) + abs(scale))
+
+    def _task_loss_term(self):
+        z = self.T("val", self.prog.logits).flatten(1)
+        q = self._targets(z.shape[0])
+        mx = z.max(dim=1, keepdim=True).values
+        lse = torch.logsumexp(z, dim=1, keepdim=True)
+        rng = (z - mx).abs().amax(dim=1, keepdim=True)
+        ln = -(q * (z - lse)).sum(dim=1)
+        en = (q.abs() * ((16 + 2 * rng) * U + 4 * U * ((z - mx).abs() + mx.abs() + (lse - mx).abs()))).sum(dim=1) + 2 * U * ln.abs()
+        L = float(ln.mean())
+        return L, float(en.mean()) + U * abs(L)
+
+    def _tv_term(self, x):
+        t = self.obj["tv"]
+        p, q, eps, s = (f32(t.get(k, d)) for k, d in (("inner_exp", 1), ("outer_exp", 1), ("eps", 1e-8), ("scale", 0.0)))
+        X, Xe = x, torch.zeros_like(x)
+        if t.get("double_opponents", False):   # planes x_a - x_b, each carrying the rounding of its own difference
+            d = torch.cat([x[:, 0:1] - x[:, 1:2], x[:, 0:1] - x[:, 2:3], x[:, 1:2] - x[:, 2:3]], dim=1)
+            X, Xe = torch.cat([x, d], dim=1), torch.cat([Xe, U * d.abs()], dim=1)
+        nb_h = lambda t_: F.pad(t_, (0, 0, 0, 1))[:, :, 1:, :]  # noqa: E731  (neighbour below / right, 0 past the edge)
+        nb_w = lambda t_: F.pad(t_, (0, 1, 0, 0))[:, :, :, 1:]  # noqa: E731
+        cp, cq = (0.0 if e == 1.0 else POW_C for e in (p, q))
+        parts = []
+        for nb in (nb_h, nb_w):
+            dd = nb(X) - X
+            A = dd.abs() + eps
+            eA = U * dd.abs() + Xe + nb(Xe) + U * A
+            Ap = A.pow(p)
+            parts.append((A, eA, Ap))
+        (A, eA, Ap), (B, eB, Bp) = parts
+        ssum = Ap + Bp
+        es = abs(p) * (A.pow(p - 1) * eA + B.pow(p - 1) * eB) + cp * U * ssum + U * ssum
+        f = ssum.pow(q)
+        ef = abs(q) * ssum.pow(q - 1) * es + cq * U * f
+        n = f.numel()
+        val = s * float(f.sum()) / n
+        return val, abs(s) * float(ef.sum() + n * D53 * f.abs().sum()) / n + 4 * D53 * abs(val)
+
+    def _norm_term(self, x):
+        nr = self.obj["norm"]
+        s, p = f32(nr["scale"]), f32(nr.get("p", 2.0))
+        xp = x.pow(p)
+        val = s / p * float(xp.mean())
+        return val, abs(s / p) * ((0.0 if p == 1.0 else POW_C * U) + xp.numel() * D53) * float(xp.abs().mean()) + 4 * D53 * abs(val)
+
+    def _di_term(self):
+        di = self.obj["di"]
+        first = self._first_bn()
+        val, bound = 0.0, 0.0
+        for i, op in enumerate(self.prog.ops):
+            if op.kind != C.OP_BNACT or not op.has_bn:
+                continue
+            mult = f32(f32(di["scale"]) * (f32(di.get("first_bn_multiplier", 10.0)) if i == first else 1.0))
+            M, _, _, nm, nv, kap_m, kap_v = self._di_layer(i, self.T("val", op.tin))
+            val += mult * float(nv + nm)
+            bound += abs(mult) * TRAIN_C * (M + 8) * U * float(nm * kap_m + nv * kap_v)
+        return val, bound + 4 * D53 * abs(val)
+
+    def _features_term(self):
+        fs = self.obj["features"]
+        lin = max(j for j, o in enumerate(self.prog.ops) if o.kind == C.OP_LINEAR)
+        x = self.T("val", self.prog.ops[lin].tin)
+        diff = x.reshape(x.shape[0], -1) - fs["measured"].double().reshape(x.shape[0], -1)
+        n, s = diff.numel(), f32(fs["scale"])
+        sq = float(diff.pow(2).sum())
+        return s * sq / n, abs(s) * (2 * U + n * D53) * sq / n + 4 * D53 * abs(s * sq / n)
+
+    def check_terms(self, terms, value=None, G=None, x=None, raise_on_failure=True):
+        """The objective terms ``terms`` (``Engine.last_terms()``) and the returned objective ``value`` of the last evaluation (see
+        the module docstring).  ``G``: the matched gradient (default: the stored G); ``x``: what the image priors act on (default:
+        the stored candidate / view, tensor 0).  Findings are reported with kind "terms" and the term's name as the sweep."""
+        if self.seq:
+            raise NotImplementedError("objective terms of token programs")
+        o = self.obj
+        G = G if G is not None else [self.Pm("G", j) for j in range(len(self.P))]
+        x = x.double() if x is not None else self.T("val", 0)
+        ref = {k: (0.0, 0.0) for k in TERMS}
+        ref["match"] = self._match_term(G, o["kind"], o["scale"])
+        ref["task_loss"] = self._task_loss_term()
+        if o["tv"] is not None:
+            ref["total_variation"] = self._tv_term(x)
+        if o["norm"] is not None:
+            ref["norm"] = self._norm_term(x)
+        if o["di"] is not None:
+            ref["deep_inversion"] = self._di_term()
+        if o["features"] is not None:
+            ref["features"] = self._features_term()
+        for k in TERMS:
+            r, b = ref[k]
+            self._cmp(-1, k, k, torch.tensor(float(terms[k]), dtype=torch.float64), torch.tensor(r, dtype=torch.float64), b, kind="terms")
+        if value is not None:   # assembled in double in this order: no rounding of its own to allow for
+            phi = terms["match"] + terms["total_variation"] + terms["norm"] + terms["deep_inversion"] + terms["features"]
+            tau = f32(o["task_regularization"])
+            if tau != 0.0:
+                phi += tau * terms["task_loss"]
+            self._cmp(-1, "value", "objective = sum of the terms", torch.tensor(float(value), dtype=torch.float64),
+                      torch.tensor(phi, dtype=torch.float64), 0.0, kind="terms")
+        if raise_on_failure and self.findings:
+            raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
+        return self.findings
+
+    def check_score(self, score, kind, G=None, raise_on_failure=True):
+        """``Engine.score(x, kind)`` (euclidean or cosine-similarity): the fp32 rounding of the match term with scale 1 of the
+        G the scoring pass left (read afresh from the source; ``G``: the matched gradient of a multi-step engine, D)."""
+        G = G if G is not None else [self.src.param("G", j).double() for j in range(len(self.P))]
+        S, E = match_sums(G, self.g, kind)
+        ref, bound = match_value(kind, S, E, 1.0)
+        bound = bound + U * abs(ref) + 16 * D53 * (abs(ref) + 1.0)
+        self._cmp(-1, kind, f"score ({kind})", torch.tensor(float(score), dtype=torch.float64), torch.tensor(ref, dtype=torch.float64),
+                  bound, kind="score")
+        if raise_on_failure and self.findings:
+            raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
+        return self.findings
+
 
 class InterpreterSource:
     """Buffers of a float64 ``ProgramInterpreter.matching_gradient`` run; ``grad_x``: the full candidate gradient (priors and
@@ -1012,6 +1244,30 @@ class MultiStepChecker:
             self._absorb(chk, k)
             self.steps.append(chk)
         self.glue_relations(n)
+        if raise_on_failure and self.findings:
+            raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
+        return self.findings
+
+    def _last_step_checker(self):
+        last = self.K - 1
+        return SweepChecker(self.prog, [w.double() for w in self.glue.W[last]], self.bn, self.g, self.labels[last], self.obj,
+                            self.src[last])
+
+    def check_terms(self, terms, value=None, raise_on_failure=True):
+        """The objective terms of a full multi-step evaluation: match from D_K, task loss and DeepInversion from the last local
+        step's buffers, TV / norm on the whole candidate (see ``SweepChecker.check_terms``)."""
+        chk = self._last_step_checker()
+        chk.check_terms(terms, value, G=[d.double() for d in self.glue.D[self.K]], x=self.glue.x, raise_on_failure=False)
+        self._absorb(chk, None)
+        if raise_on_failure and self.findings:
+            raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
+        return self.findings
+
+    def check_score(self, score, kind, D, raise_on_failure=True):
+        """``Engine.score`` of a multi-step engine: the match of ``D`` (``debug_step_param("D", ...)`` after the scoring pass)."""
+        chk = self._last_step_checker()
+        chk.check_score(score, kind, G=[d.double() for d in D], raise_on_failure=False)
+        self._absorb(chk, None)
         if raise_on_failure and self.findings:
             raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
         return self.findings

@@ -193,6 +193,31 @@ def sweep_objective(cfg, features=None):
     return obj
 
 
+def tensor_weights(cfg, L):
+    """Per-tensor weights the attack hands to ``Engine.load_targets`` for tag-euclidean (optimization_attack.py), else None."""
+    from oracle.sweep_check import tag_weights
+
+    if cfg.objective.type != "tag-euclidean":
+        return None
+    return tag_weights(L, cfg.objective.get("scale_scheme", "linear"))
+
+
+def masked_targets(grads):
+    """Target gradients that reach both sides of masked-cosine's strict ``|g| > float32(1e-6)``: in the largest tensor exact zeros,
+    +-float32(1e-6) and its two fp32 neighbours; one other tensor of at least 1024 elements zeroed whole (fully masked chunks)."""
+    g = [t.detach().clone().float() for t in grads]
+    big = max(range(len(g)), key=lambda j: g[j].numel())
+    m = torch.tensor(1e-6, dtype=torch.float32)
+    edge = torch.stack([m, torch.nextafter(m, torch.tensor(0.0)), torch.nextafter(m, torch.tensor(1.0))])
+    edge = torch.cat([edge, -edge, torch.zeros(3)])
+    flat = g[big].view(-1)
+    n = (flat.numel() // (2 * edge.numel())) * edge.numel()
+    flat[:n] = edge.repeat(n // edge.numel())
+    whole = next(j for j in range(len(g)) if j != big and g[j].numel() >= 1024)
+    g[whole].zero_()
+    return g
+
+
 def unwritten_tangents(eng):
     """Tensors whose tangent the last evaluation did not store (fuse_bnact: a conv output whose only consumer is the BN op that ran
     in the conv's epilogue), as the engine reports them."""

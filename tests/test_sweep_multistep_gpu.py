@@ -16,7 +16,7 @@ from breaching_b200 import get_attack_config, synthetic  # noqa: E402
 from breaching_b200.engine import Engine, EngineError  # noqa: E402
 from breaching_b200.schedule import lr_table  # noqa: E402
 from helpers import case_from_fixture, cfg_from_fixture, load_golden, sweep_objective  # noqa: E402
-from oracle.sweep_check import MultiStepChecker  # noqa: E402
+from oracle.sweep_check import MultiStepChecker, SweepCheckError  # noqa: E402
 
 DEV = torch.device("cuda:0")
 WHICH = ("val", "delta", "tangent", "tangent_delta")
@@ -125,11 +125,16 @@ def check_engine(name, backend, options=(), env=None, monkeypatch=None):
             if key[0] in ("val", "delta"):
                 assert torch.equal(t, r[key]), (k, key)
     eng.set_option("debug_multistep_stop", 0)
-    _, grad = eng.objective_and_gradient(xd)
+    value, grad = eng.objective_and_gradient(xd)
+    terms = eng.last_terms()
     W = [[eng.debug_step_param("W", k, j) for j in range(n)] for k in range(K + 1)]
     Wo = [[eng.debug_step_param("W_operand", k, j) for j in range(n)] for k in range(K + 1)]
     stem = {i for i in range(len(eng.prog.ops)) if eng.debug_op(i)["stem_columns"]}
     prog = eng.prog
+    scores = []   # (kind, score, the D its pass accumulated)
+    for kind in ("euclidean", "cosine-similarity"):
+        sc = eng.score(xd, kind)
+        scores.append((kind, sc, [eng.debug_step_param("D", 0, j) for j in range(n)]))
     offsets = [(k * dps) % x.shape[0] for k in range(K)]
     eng.close()
     glue = EngineGlue(W, Wo, D, x, grad.cpu(), offsets, float(torch.tensor(local["lr"], dtype=torch.float32)))
@@ -139,7 +144,12 @@ def check_engine(name, backend, options=(), env=None, monkeypatch=None):
     chk = MultiStepChecker(prog, bn, shared[0]["gradients"], local["labels"], sweep_objective(cfg), srcs, glue)
     chk.stem, chk.unwritten = sorted(stem), unwritten
     try:
-        chk.check()
+        chk.check(raise_on_failure=False)
+        chk.check_terms(terms, value, raise_on_failure=False)
+        for kind, sc, Ds in scores:
+            chk.check_score(sc, kind, Ds, raise_on_failure=False)
+        if chk.findings:
+            raise SweepCheckError("\n".join(repr(f) for f in chk.findings[:20]))
     finally:
         print(f"\n[{name} / {backend} {dict(options)} {env or ''}] " +
               ", ".join(f"{k}/{s}: {r:.3g}" for (k, s), r in sorted(chk.ratios.items())) +
