@@ -2159,4 +2159,13 @@ int bre_conv_gemm(int32_t mode, int32_t backend, const float* a, const float* w,
   return launch_igemm_simt(g, s);
 }
 
+int bre_debug_last_gemm_plan(int32_t* out) {
+  if (!out) { set_error("bre_debug_last_gemm_plan: null output"); return BRE_ERR_INVALID; }
+  const GemmPlan& p = last_gemm_plan();
+  const int32_t v[GEMM_PLAN_FIELDS] = {p.family, p.mode, p.nsrc, p.tile_rows, p.tile_width, p.splits, p.stages, p.producer,
+                                       p.total_kblocks, p.kblocks_per_split, p.vec};
+  memcpy(out, v, sizeof(v));
+  return BRE_OK;
+}
+
 }  // extern "C"

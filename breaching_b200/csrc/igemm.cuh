@@ -61,6 +61,23 @@ struct GemmArgs {
 
 constexpr int IG_BM = 64, IG_BN = 64, IG_BK = 16, IG_THREADS = 256;
 
+// What the launchers chose for the last GEMM issued by the calling host thread (bre_debug_last_gemm_plan): the kernel family,
+// tiles, split, ring depth and operand producer.  Host side only: written just before the launch, never passed to a kernel.
+enum GemmFamily { GEMM_FAM_SIMT = 0, GEMM_FAM_DGRAD_SMALL_CI = 1, GEMM_FAM_LINEAR_SMALL = 2, GEMM_FAM_LINEAR_TALL = 3, GEMM_FAM_TC = 4 };
+enum GemmProducer { GEMM_PROD_NONE = 0, GEMM_PROD_TMA = 1, GEMM_PROD_CP_ASYNC = 2, GEMM_PROD_CLASSES = 3 };
+struct GemmPlan {
+  int family = -1, mode = -1, nsrc = 0;
+  int tile_rows = 0, tile_width = 0;   // output tile (SIMT / tensor core); linear_small: rows of the kernel instance
+  int splits = 1, stages = 0;          // split-K factor (grid z; linear_tall: reduction chunks), ring depth
+  int producer = GEMM_PROD_NONE;
+  int total_kblocks = 0, kblocks_per_split = 0;   // k-blocks of TC_BK = 32 (tensor core) / IG_BK = 16 (SIMT) over all sources
+  int vec = 0;                         // SIMT: bit 0 vector A loads, bit 1 vector B loads, bit 2 vector stores; dgrad_small_ci /
+                                       // linear_small fprop: vector loads
+};
+constexpr int GEMM_PLAN_FIELDS = 11;
+void record_gemm_plan(const GemmPlan& p);
+const GemmPlan& last_gemm_plan();
+
 int launch_igemm_simt(const GemmArgs& a, cudaStream_t stream);
 // linear layers on <= 16 rows (the classification head at small batch): dedicated fp32 kernels (linear_small.cu)
 bool linear_small_supported(const GemmArgs& a);

@@ -502,6 +502,10 @@ int launch_dgrad_small_ci(const GemmArgs& a, cudaStream_t stream) {
   if (smem > 200 * 1024) { set_error("dgrad_small_ci: filter too large for shared memory"); return -4; }
   const int Wcp = ((Wc + SC_PX - 1) / SC_PX) * SC_PX;
   dim3 grid(ceil_div((long long)Wcp * g.stride, 32 * SC_PX), g.H, g.N), block(128);
+  GemmPlan plan;
+  plan.family = GEMM_FAM_DGRAD_SMALL_CI; plan.mode = a.mode; plan.nsrc = a.nsrc;
+  plan.tile_rows = 32 * SC_PX; plan.tile_width = g.Ci; plan.vec = vec;
+  record_gemm_plan(plan);
 #define BRE_LAUNCH_SC(CI_)                                                                                              \
   do {                                                                                                                  \
     static size_t cap = 0;                                                                                              \
@@ -522,7 +526,12 @@ int launch_dgrad_small_ci(const GemmArgs& a, cudaStream_t stream) {
   return 0;
 }
 
+thread_local GemmPlan g_last_plan;
+
 }  // namespace
+
+void record_gemm_plan(const GemmPlan& p) { g_last_plan = p; }
+const GemmPlan& last_gemm_plan() { return g_last_plan; }
 
 int launch_igemm_simt(const GemmArgs& a, cudaStream_t stream) {
   Dims d;
@@ -574,6 +583,12 @@ int launch_igemm_simt(const GemmArgs& a, cudaStream_t stream) {
   if (tn > 65535 || splits > 65535) { set_error("igemm: grid too large"); return -1; }
 
   dim3 grid(tm, tn, splits), block(IG_THREADS);
+  GemmPlan plan;
+  plan.family = GEMM_FAM_SIMT; plan.mode = a.mode; plan.nsrc = a.nsrc;
+  plan.tile_rows = IG_BM; plan.tile_width = IG_BN; plan.splits = splits; plan.stages = 2;
+  plan.total_kblocks = d.total_steps; plan.kblocks_per_split = d.steps_per_split;
+  plan.vec = (d.vecA ? 1 : 0) | (d.vecB ? 2 : 0) | (d.vecOut ? 4 : 0);
+  record_gemm_plan(plan);
   if (a.mode == GEMM_FPROP) BRE_KLAUNCH((igemm_simt_kernel<GEMM_FPROP>), grid, block, 0, stream, a, d);
   else if (a.mode == GEMM_DGRAD) BRE_KLAUNCH((igemm_simt_kernel<GEMM_DGRAD>), grid, block, 0, stream, a, d);
   else BRE_KLAUNCH((igemm_simt_kernel<GEMM_WGRAD>), grid, block, 0, stream, a, d);

@@ -1121,6 +1121,11 @@ int launch_tc(const GemmArgs& a, const TcDims& d0, const std::conditional_t<CLS,
   // phase two rounds old, which reads as complete, and overwrite a stage still in use (BRE_TC_PRODUCERS=4 with a 2-deep ring).
   int proxy_fence = proxy_fence_env;
   if (((proxy_fence >> 2) & 7) > stages) proxy_fence = (proxy_fence & 3) | (stages << 2);
+  GemmPlan rec;
+  rec.family = GEMM_FAM_TC; rec.mode = MODE; rec.nsrc = a.nsrc; rec.tile_rows = BM; rec.tile_width = BN; rec.splits = splits;
+  rec.stages = stages; rec.producer = CLS ? GEMM_PROD_CLASSES : (TMA ? GEMM_PROD_TMA : GEMM_PROD_CP_ASYNC);
+  rec.total_kblocks = d.total_kblocks; rec.kblocks_per_split = d.kblocks_per_split;
+  record_gemm_plan(rec);
   {
     cudaError_t lerr = launch_kernel(igemm_tc_kernel<MODE, BN, TMA, CLS, BM>, dim3(tm, tn, splits), dim3(TC_BLOCK), smem, stream, splits, a, d,
                                      proxy_fence, maps, plan);

@@ -127,16 +127,22 @@ __global__ void __launch_bounds__(256) linear_small_wgrad_kernel(GemmArgs a) {
 template <int NB>
 int launch_nb(const GemmArgs& a, cudaStream_t stream) {
   const int Co = a.g.Co, Ci = a.g.Ci;
+  GemmPlan plan;
+  plan.family = GEMM_FAM_LINEAR_SMALL; plan.mode = a.mode; plan.nsrc = a.nsrc; plan.tile_rows = NB;
   if (a.mode == GEMM_FPROP) {
     auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
     int vec = (Ci % 4 == 0) && (a.x_sN % 4 == 0);
     for (int s = 0; s < a.nsrc; ++s) vec = vec && al16(a.act[s]) && al16(a.wgt[s]);
+    plan.vec = vec;
+    record_gemm_plan(plan);
     BRE_KLAUNCH((linear_small_fprop_kernel<NB>), ceil_div((long long)Co * 32, 256), 256, 0, stream, a, vec);
   } else if (a.mode == GEMM_DGRAD) {
+    record_gemm_plan(plan);
     BRE_KLAUNCH((linear_small_dgrad_kernel<NB>), ceil_div(Ci, 32), 32 * (NB >= 16 ? 8 : (NB >= 8 ? 16 : 32)), 0, stream, a);
   } else {
     long long blocks = ((long long)Co * Ci + 255) / 256;
     if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
+    record_gemm_plan(plan);
     BRE_KLAUNCH((linear_small_wgrad_kernel<NB>), (int)blocks, 256, 0, stream, a);
   }
   BRE_CHECK_LAUNCH();
@@ -274,6 +280,10 @@ bool linear_tall_supported(const GemmArgs& a) {
 int launch_linear_tall(const GemmArgs& a, cudaStream_t stream) {
   const int Co = a.g.Co, Ci = a.g.Ci;
   const int chunk = tall_chunk(Co), chunks = ceil_div(Co, chunk);
+  GemmPlan plan;
+  plan.family = GEMM_FAM_LINEAR_TALL; plan.mode = a.mode; plan.nsrc = a.nsrc; plan.tile_rows = LT_ROWS; plan.tile_width = Ci;
+  plan.splits = chunks; plan.total_kblocks = Co; plan.kblocks_per_split = chunk;
+  record_gemm_plan(plan);
   auto go = [&](auto cj_tag) -> int {
     constexpr int CJ = decltype(cj_tag)::value;
     const size_t smem = (size_t)(LT_MAXC * CJ * 32 + LT_MAXC * LT_PITCH) * sizeof(float);

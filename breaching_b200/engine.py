@@ -101,6 +101,7 @@ EXPORTS = [
     "bre_engine_set_augmentations", "bre_engine_last_augmentation", "bre_augment_view",
     "bre_engine_set_augmentation_stages", "bre_engine_augmentation_draws", "bre_augment_resample", "bre_augment_blur",
     "bre_engine_set_trial_index", "bre_engine_debug_step_state", "bre_optimizer_step", "bre_langevin_noise",
+    "bre_debug_last_gemm_plan",
 ]
 
 
@@ -170,6 +171,7 @@ def load_library(path=None):
     lib.bre_engine_debug_step_state.argtypes = [vp, i32, vp]
     lib.bre_optimizer_step.argtypes = [vp] * 7 + [i32, vp, vp, i64, i32, i32, P(AttackCfg), vp, i32, P(StepScalars), vp]
     lib.bre_langevin_noise.argtypes = [ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64, i64, vp, vp]
+    lib.bre_debug_last_gemm_plan.argtypes = [P(i32)]
     for name in EXPORTS:
         if name not in ("bre_last_error", "bre_version", "bre_engine_destroy"):
             getattr(lib, name).restype = ctypes.c_int
@@ -819,6 +821,21 @@ def conv_gemm(mode, a, w, out, N, H, W, Ci, Co, R, S, stride, pad, a2=None, w2=N
                                pad, ctypes.c_void_p(stream))
     _check(lib, rc, "bre_conv_gemm")
     return out
+
+
+GEMM_FAMILIES = {-1: None, 0: "igemm_simt", 1: "dgrad_small_ci", 2: "linear_small", 3: "linear_tall", 4: "tc"}
+GEMM_PRODUCERS = {0: None, 1: "tma", 2: "cp.async", 3: "classes"}
+
+
+def last_gemm_plan():
+    """The launch plan of the last GEMM issued by this host thread (bre_debug_last_gemm_plan): kernel family, mode, nsrc, tile rows /
+    width, split-K factor, ring depth, operand producer, k-blocks in all and per split, and the SIMT vector-loader flags."""
+    lib = load_library()
+    buf = (ctypes.c_int32 * 11)()
+    _check(lib, lib.bre_debug_last_gemm_plan(buf), "bre_debug_last_gemm_plan")
+    v = list(buf)
+    return dict(family=GEMM_FAMILIES[v[0]], mode=v[1], nsrc=v[2], tile_rows=v[3], tile_width=v[4], splits=v[5], stages=v[6],
+                producer=GEMM_PRODUCERS[v[7]], total_kblocks=v[8], kblocks_per_split=v[9], vec=v[10])
 
 
 def token_layernorm(sweep, x, gamma, beta, stats, in1=None, in2=None, in3=None, v_gamma=None, v_beta=None, eps=1e-5, want_param_grad=False,

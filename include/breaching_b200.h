@@ -362,6 +362,12 @@ int bre_token_match(const float* rec, const float* emb, const int64_t* subset, i
 int bre_conv_gemm(int32_t mode, int32_t backend, const float* a, const float* w, const float* a2, const float* w2,
                   float* out, int32_t N, int32_t H, int32_t W, int32_t Ci, int32_t Co, int32_t R, int32_t S,
                   int32_t stride, int32_t pad, void* stream);
+/* The launch plan of the last GEMM issued by the calling host thread (any entry point: bre_conv_gemm or the engine), host-side
+ * bookkeeping only.  out[11] = family (-1 none yet, 0 SIMT implicit GEMM, 1 dgrad_small_ci, 2 linear_small, 3 linear_tall, 4 tensor
+ * core), mode, nsrc, tile rows, tile width, splits (grid z; linear_tall: reduction chunks), ring depth, producer (0 none, 1 TMA,
+ * 2 cp.async, 3 TMA per parity class), total k-blocks, k-blocks per split (32-wide on the tensor cores, 16-wide on SIMT), vector
+ * flags (SIMT: bit 0 A loads, bit 1 B loads, bit 2 stores; dgrad_small_ci / linear_small fprop: vector loads). */
+int bre_debug_last_gemm_plan(int32_t* out);
 
 const char* bre_last_error(void);
 const char* bre_version(void);

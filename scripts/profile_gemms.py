@@ -36,13 +36,50 @@ def gemm_shape(mode, g):
     return Co, R * R * Ci, N * Ho * Wo
 
 
-def split_plan(mode, g, nsrc):
-    """(tiles, tile width, split-K factor, k-blocks per CTA) as launch_igemm_tc / launch_tc choose them."""
+def _env(name, default):
+    return int(os.environ.get(name, str(default)))
+
+
+def tma_ok(mode, g):
+    """tma_eligible in igemm_tc.cu: the TMA producer covers this contraction (BRE_TC_TMA=0 turns it off everywhere)."""
+    N, H, W, Ci, Co, R, st, pd = g
+    if not _env("BRE_TC_TMA", 1) or st > 8 or pd > 127 or R - 1 - pd > 127 or R > 128:
+        return False
+    if mode == 1:
+        return st == 1
+    if mode == 2:
+        return Ci % 32 == 0
+    return True
+
+
+def narrow_ok(mode, g):
+    """narrow_tiles_ok in igemm_tc.cu: 128 x 32 / 64 x 32 tiles exist for the TMA producer of fprop, stride-1 dgrad and wgrad."""
+    return bool(_env("BRE_TC_NARROW", 1)) and tma_ok(mode, g)
+
+
+def classes_ok(mode, g):
+    """cls_eligible in igemm_tc.cu (stride-2 dgrad as per-parity-class TMA gathers; the tap-corner range check never binds here)."""
+    N, H, W, Ci, Co, R, st, pd = g
+    return mode == 1 and st == 2 and bool(_env("BRE_TC_STRIDED_TMA", 1)) and bool(_env("BRE_TC_TMA", 1)) and R <= 16
+
+
+def tc_supported(mode, g):
+    """igemm_tc_supported in igemm_tc.cu for NHWC / OHWI operands on 16-byte aligned buffers."""
+    N, H, W, Ci, Co, R, st, pd = g
+    M, Nc, K = gemm_shape(mode, g)
+    if Nc % 64 != 0 and not (Nc % 32 == 0 and narrow_ok(mode, g)):
+        return False
+    if R * R > 64:
+        return False
+    return {0: Ci % BK == 0, 1: Co % BK == 0, 2: Co % 4 == 0 and Ci % 4 == 0}[mode]
+
+
+def _tc_split(mode, g, nsrc):
     N, H, W, Ci, Co, R, st, pd = g
     M, Nc, K = gemm_shape(mode, g)
     kb = -(-K // BK) * nsrc
     tm = -(-M // BM)
-    cls = mode == 1 and st == 2
+    cls = classes_ok(mode, g)
     if cls:   # strided dgrad: one m-tile range per parity class, k extent of the largest class
         tm, kmax = 0, 0
         for ey in range(2):
@@ -56,14 +93,13 @@ def split_plan(mode, g, nsrc):
                 tx = -(-(R - ex) // 2) if ex < R else 0
                 kmax = max(kmax, ty * tx)
         kb = max(kmax * (Co // BK) * nsrc, 1)
-    narrow_ok = mode != 0 and not cls and (mode != 2 or Ci % 32 == 0)
-    underfilled = Nc % 64 == 0 and tm * (Nc // 64) * 16 <= NUM_SMS and kb >= 64 and narrow_ok
+    underfilled = mode != 0 and not cls and Nc % 64 == 0 and tm * (Nc // 64) * 16 <= NUM_SMS and kb >= 64 and narrow_ok(mode, g)
     bn = 32 if Nc % 64 != 0 or underfilled else 64
     tiles = tm * (Nc // bn)
     splits = 1
     while splits < MAX_CLUSTER and tiles * splits < NUM_SMS and kb // (splits * 2) >= 2:
         splits *= 2
-    cap = int(os.environ.get("BRE_TC_MAX_SPLITS", "0"))
+    cap = _env("BRE_TC_MAX_SPLITS", 0)
     if cap > 0:
         splits = min(splits, cap)
     p = 1
@@ -72,7 +108,12 @@ def split_plan(mode, g, nsrc):
     splits = p
     while splits > 1 and splits > kb:
         splits //= 2
-    return tiles, bn, splits, -(-kb // splits)
+    return tiles, bn, splits, -(-kb // splits), kb, cls
+
+
+def split_plan(mode, g, nsrc):
+    """(tiles, tile width, split-K factor, k-blocks per CTA) as launch_igemm_tc / launch_tc choose them."""
+    return _tc_split(mode, g, nsrc)[:4]
 
 
 def ring_plan(mode, g, nsrc):
@@ -80,12 +121,94 @@ def ring_plan(mode, g, nsrc):
     N, H, W, Ci, Co, R, st, pd = g
     M, Nc, K = gemm_shape(mode, g)
     tiles, bn, splits, kbc = split_plan(mode, g, nsrc)
-    stream = int(os.environ.get("BRE_TC_STREAM", "1")) != 0
-    bm = 64 if stream and M <= 64 and (mode == 0 or (mode == 1 and st == 1)) else BM
-    shortk = kbc <= 6 and tiles == Nc // bn and tiles * splits > 2 * NUM_SMS
+    # 64-row tiles are im2col boxes of the TMA producer: a fprop the producer does not cover (stride > 8) keeps 128-row cp.async tiles
+    bm = 64 if _env("BRE_TC_STREAM", 1) and M <= 64 and mode in (0, 1) and tma_ok(mode, g) else BM
+    shortk = _env("BRE_TC_SHORTK_STAGES", 2) == 2 and kbc <= 6 and tiles == Nc // bn and tiles * splits > 2 * NUM_SMS
     deep = bm == 64 and tiles * splits <= NUM_SMS and kbc >= 16
-    forced = int(os.environ.get("BRE_TC_STAGES", "0"))
+    forced = _env("BRE_TC_STAGES", 0)
     return bm, forced if forced in (2, 4, 8) else (2 if shortk else 8 if deep else 4)
+
+
+def tc_plan(mode, g, nsrc):
+    """The whole tensor-core launch plan, in the form engine.last_gemm_plan() reports it."""
+    tiles, bn, splits, kbc, kb, cls = _tc_split(mode, g, nsrc)
+    bm, stages = ring_plan(mode, g, nsrc)
+    producer = "classes" if cls else "tma" if bm == 64 or bn == 32 or tma_ok(mode, g) else "cp.async"
+    return dict(family="tc", mode=mode, nsrc=nsrc, tile_rows=bm, tile_width=bn, splits=splits, stages=stages, producer=producer,
+                total_kblocks=kb, kblocks_per_split=kbc, vec=0)
+
+
+SIMT_BM, SIMT_BN, SIMT_BK, SIMT_WS_TILES, SC_PX, SC_KCH = 64, 64, 16, 1024, 4, 4
+
+
+def _linear(g):
+    N, H, W, Ci, Co, R, st, pd = g
+    return R == 1 and H == 1 and W == 1 and st == 1 and pd == 0
+
+
+def linear_tall_ok(mode, g, nsrc):
+    """linear_tall_supported in linear_small.cu (with bre_conv_gemm's 1024-tile workspace)."""
+    N, H, W, Ci, Co, R, st, pd = g
+    if not _env("BRE_LINEAR_TALL", 1) or mode != 1 or not _linear(g) or not 1 <= N <= 32 or Ci % 32 or Ci > 128 or Co < 8192:
+        return False
+    return -(-Co // _tall_chunk(Co)) * 32 * Ci <= SIMT_WS_TILES * SIMT_BM * SIMT_BN
+
+
+def _tall_chunk(Co):
+    c = -(-Co // (4 * NUM_SMS))
+    c += c & 1
+    return min(max(c, 32), 96)
+
+
+def linear_small_preferred(mode, g, nsrc):
+    N, H, W, Ci, Co, R, st, pd = g
+    if not _env("BRE_LINEAR_SMALL_ROWS", 0) or mode == 2 or not (_linear(g) and 1 <= N <= 32):
+        return False
+    return (Ci if mode == 0 else Co) * nsrc <= 512
+
+
+def simt_plan(mode, g, nsrc):
+    """launch_igemm_simt in igemm_simt.cu (linear_small / dgrad_small_ci / the SIMT implicit GEMM) for NHWC / OHWI operands on 16-byte
+    aligned buffers, in the form engine.last_gemm_plan() reports it."""
+    N, H, W, Ci, Co, R, st, pd = g
+    M, Nc, K = gemm_shape(mode, g)
+    base = dict(mode=mode, nsrc=nsrc, tile_rows=0, tile_width=0, splits=1, stages=0, producer=None, total_kblocks=0, kblocks_per_split=0,
+                vec=0)
+    if _env("BRE_LINEAR_SMALL", 1) and _linear(g) and 1 <= N <= 32 and (N <= 16 or linear_small_preferred(mode, g, nsrc)):
+        nb = next(b for b in (1, 2, 4, 8, 16, 32) if N <= b)
+        return dict(base, family="linear_small", tile_rows=nb, vec=int(mode == 0 and Ci % 4 == 0))
+    if mode == 1 and Ci <= 4 and Co <= 16 * SC_KCH and nsrc * -(-R // st) * R * Co * Ci * 4 <= 200 * 1024:
+        return dict(base, family="dgrad_small_ci", tile_rows=32 * SC_PX, tile_width=Ci, vec=int(Co % 4 == 0))
+    total = -(-K // SIMT_BK) * nsrc
+    x_vec = Ci % 4 == 0
+    vec_a, vec_b, vec_out = {0: (x_vec, K % 4 == 0, Nc % 4 == 0), 1: (Co % 4 == 0, Ci % 4 == 0, x_vec),
+                             2: (Co % 4 == 0, x_vec, Nc % 4 == 0)}[mode]
+    tiles = -(-M // SIMT_BM) * -(-Nc // SIMT_BN)
+    splits = 1
+    if tiles < 2 * NUM_SMS:
+        splits = min(-(-2 * NUM_SMS // tiles), max(total // 4, 1))
+    splits = min(splits, total)
+    if splits > 1 and tiles * splits > SIMT_WS_TILES:
+        splits = max(SIMT_WS_TILES // tiles, 1)
+    per = -(-total // splits)
+    return dict(base, family="igemm_simt", tile_rows=SIMT_BM, tile_width=SIMT_BN, splits=-(-total // per), stages=2, total_kblocks=total,
+                kblocks_per_split=per, vec=int(vec_a) | 2 * int(vec_b) | 4 * int(vec_out))
+
+
+def gemm_plan(mode, g, nsrc, backend):
+    """The plan bre_conv_gemm launches for `backend` (0 SIMT, 1 tensor cores, 2 the engine's dispatch), None if it refuses the shape."""
+    if linear_tall_ok(mode, g, nsrc):
+        N, H, W, Ci, Co, R, st, pd = g
+        chunk = _tall_chunk(Co)
+        return dict(family="linear_tall", mode=mode, nsrc=nsrc, tile_rows=32, tile_width=Ci, splits=-(-Co // chunk), stages=0, producer=None,
+                    total_kblocks=Co, kblocks_per_split=chunk, vec=0)
+    if backend == 1:
+        return tc_plan(mode, g, nsrc) if tc_supported(mode, g) else None
+    if backend == 2 and linear_small_preferred(mode, g, nsrc):
+        return simt_plan(mode, g, nsrc)
+    if backend == 2 and tc_supported(mode, g):
+        return tc_plan(mode, g, nsrc)
+    return simt_plan(mode, g, nsrc)
 
 
 def launches_of(prog, dev):
