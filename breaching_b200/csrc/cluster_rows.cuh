@@ -28,10 +28,17 @@ __device__ __forceinline__ double ld_cluster_f64(const double* local, unsigned r
   return v;
 }
 
-// Segment [c0, c1) of a row of C elements served by this CTA (4-element aligned starts so that float4 access stays possible).
+// The row plan, one rule for the kernels and the host: a row of C elements on a cluster of cs CTAs is cut into segments of
+// row_segment_len(C, cs) elements (4-element aligned starts so that float4 access stays possible); a segment of at most
+// kSegCache elements per thread is cached in registers (row_seg_fits), a longer one is streamed from memory.
+constexpr int kSegCache = 26;
+__host__ __device__ __forceinline__ int row_segment_len(int C, int cs) { return (((C + cs - 1) / cs) + 3) & ~3; }
+__host__ __device__ __forceinline__ bool row_seg_fits(int C, int cs) { return row_segment_len(C, cs) <= kSegCache * kRowThreads; }
+
+// Segment [c0, c1) of a row of C elements served by this CTA.
 __device__ __forceinline__ void row_segment(int C, int& c0, int& c1) {
-  const int n = (int)cluster_size(), r = (int)cluster_rank();
-  const int per = (((C + n - 1) / n) + 3) & ~3;
+  const int r = (int)cluster_rank();
+  const int per = row_segment_len(C, (int)cluster_size());
   c0 = r * per < C ? r * per : C;
   c1 = c0 + per < C ? c0 + per : C;
 }
@@ -85,13 +92,8 @@ __device__ __forceinline__ void cluster_exit() { cluster_barrier(); }
 // plain loops every pass is a chain of dependent L2 round trips.  When the segment fits, each thread loads its elements once, all loads in flight together, and the passes run out of
 // registers.  `seg_fits` depends only on the row width and the cluster size, so it is uniform over the cluster (the barriers inside the
 // reductions need every CTA on the same path).
-constexpr int kSegCache = 26;
 struct SegCache { float v[kSegCache]; };
-__device__ __forceinline__ bool seg_fits(int C) {
-  const int n = (int)cluster_size();
-  const int per = (((C + n - 1) / n) + 3) & ~3;
-  return per <= kSegCache * kRowThreads;
-}
+__device__ __forceinline__ bool seg_fits(int C) { return row_seg_fits(C, (int)cluster_size()); }
 __device__ __forceinline__ void seg_load(SegCache& s, const float* __restrict__ row, int c0, int c1, float fill) {
 #pragma unroll
   for (int k = 0; k < kSegCache; ++k) {

@@ -17,6 +17,7 @@
 #include "tokens.cuh"
 #include "objective.cuh"
 #include "augment.cuh"
+#include "cluster_rows.cuh"
 
 namespace bre {
 void set_pdl(bool on);
@@ -1994,10 +1995,10 @@ int bre_engine_debug_tensor(bre_engine* e, int32_t which, int32_t tensor, float*
 }
 
 int bre_engine_debug_step_state(bre_engine* e, int32_t which, float* out_host) {
-  if (!e || !out_host || which < 0 || which > 6) { set_error("bre_engine_debug_step_state: bad arguments"); return BRE_ERR_INVALID; }
+  if (!e || !out_host || which < 0 || which > 7) { set_error("bre_engine_debug_step_state: bad arguments"); return BRE_ERR_INVALID; }
   if (!e->trial_begun) { set_error("bre_engine_begin_trial must be called first"); return BRE_ERR_STATE; }
   const StepArgs a = e->step_args();
-  const float* bufs[7] = {a.grad, a.grad_task, a.m, a.v, e->label_grad, e->ell_m, e->ell_v};
+  const float* bufs[8] = {a.grad, a.grad_task, a.m, a.v, e->label_grad, e->ell_m, e->ell_v, e->soft_q_buf};
   const float* src = bufs[which];
   if (which >= 4 && !e->joint) src = nullptr;
   if (!src) { set_error(which == 1 ? "the step reads no separate task gradient (none needed, or folded into the candidate gradient)" : "no joint trial"); return BRE_ERR_STATE; }
@@ -2166,6 +2167,40 @@ int bre_debug_last_gemm_plan(int32_t* out) {
                                        p.total_kblocks, p.kblocks_per_split, p.vec};
   memcpy(out, v, sizeof(v));
   return BRE_OK;
+}
+
+int bre_debug_row_plan(int32_t C, int32_t* cs, int32_t* fits) {
+  if (C < 1 || !cs || !fits) { set_error("bre_debug_row_plan: bad arguments"); return BRE_ERR_INVALID; }
+  *cs = row_cluster_size(C);
+  *fits = row_seg_fits(C, *cs) ? 1 : 0;
+  return BRE_OK;
+}
+
+int bre_row_op(int32_t op, const float* in0, const float* in1, const float* in2, const int64_t* labels, int32_t rows, int32_t C, int32_t Vs,
+               int32_t T, float coef, int32_t round_out, float* out0, float* out1, float* out2, void* stream) {
+  const bool token = op == BRE_ROW_TOKEN_CE_FWD || op == BRE_ROW_TOKEN_CE_TAN_BWD || op == BRE_ROW_TOKEN_LABEL_GRAD;
+  const bool fwd = op == BRE_ROW_TOKEN_CE_FWD || op == BRE_ROW_CE_FWD;
+  const bool three_in = op == BRE_ROW_TOKEN_LABEL_GRAD || op == BRE_ROW_CE_LABEL_GRAD;
+  bool ok = op >= BRE_ROW_SOFTMAX && op <= BRE_ROW_CE_TAN_BWD && rows >= 1 && C >= 1 && Vs >= C && in0 && out0;
+  ok = ok && (token ? T >= 1 && rows % T == 0 : Vs == C);
+  ok = ok && (op == BRE_ROW_SOFTMAX || op == BRE_ROW_SOFTMAX_CHAIN || op == BRE_ROW_CE_FWD || in1) && (!three_in || in2);
+  ok = ok && (!fwd || (out1 && out2)) && (op != BRE_ROW_CE_FWD || (labels != nullptr) != (in1 != nullptr));
+  ok = ok && (!round_out || token || (op == BRE_ROW_CE_TAN_BWD && labels));
+  if (!ok) { set_error("bre_row_op: bad arguments"); return BRE_ERR_INVALID; }
+  cudaStream_t s = (cudaStream_t)stream;
+  const long long* lab = (const long long*)labels;
+  switch (op) {
+    case BRE_ROW_SOFTMAX: return launch_row_softmax(in0, out0, rows, C, s);
+    case BRE_ROW_SOFTMAX_CHAIN: return launch_softmax_chain(in0, out0, rows, C, s);
+    case BRE_ROW_TOKEN_CE_FWD: return launch_token_ce_fwd(in0, in1, rows, C, Vs, T, out0, out1, out2, round_out != 0, s);
+    case BRE_ROW_TOKEN_CE_TAN_BWD: return launch_token_ce_tan_bwd(in0, in1, rows, C, Vs, T, out0, round_out != 0, s);
+    case BRE_ROW_TOKEN_LABEL_GRAD: return launch_token_label_grad(in0, in1, in2, rows, C, Vs, T, coef, out0, s);
+    case BRE_ROW_CE_FWD: return launch_ce_fwd(in0, lab, in1, rows, C, out0, out1, out2, s);
+    case BRE_ROW_CE_LABEL_GRAD: return launch_ce_label_grad(in0, in1, in2, rows, C, coef, out0, s);
+    default:
+      if (lab) return launch_ce_tan_bwd_seeded(in0, in1, lab, rows, C, coef, out0, round_out != 0, s);
+      return launch_ce_tan_bwd(in0, in1, rows, C, out0, s);
+  }
 }
 
 }  // extern "C"

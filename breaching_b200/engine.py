@@ -101,7 +101,7 @@ EXPORTS = [
     "bre_engine_set_augmentations", "bre_engine_last_augmentation", "bre_augment_view",
     "bre_engine_set_augmentation_stages", "bre_engine_augmentation_draws", "bre_augment_resample", "bre_augment_blur",
     "bre_engine_set_trial_index", "bre_engine_debug_step_state", "bre_optimizer_step", "bre_langevin_noise",
-    "bre_debug_last_gemm_plan",
+    "bre_debug_last_gemm_plan", "bre_debug_row_plan", "bre_row_op",
 ]
 
 
@@ -172,6 +172,8 @@ def load_library(path=None):
     lib.bre_optimizer_step.argtypes = [vp] * 7 + [i32, vp, vp, i64, i32, i32, P(AttackCfg), vp, i32, P(StepScalars), vp]
     lib.bre_langevin_noise.argtypes = [ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64, i64, vp, vp]
     lib.bre_debug_last_gemm_plan.argtypes = [P(i32)]
+    lib.bre_debug_row_plan.argtypes = [i32, P(i32), P(i32)]
+    lib.bre_row_op.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, vp, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("bre_last_error", "bre_version", "bre_engine_destroy"):
             getattr(lib, name).restype = ctypes.c_int
@@ -641,8 +643,8 @@ class Engine:
     def debug_step_state(self, which):
         """What the optimiser step of the last iteration read and left: "grad" (candidate gradient before noise / clip / sign),
         "grad_task" (raises when the step reads no separate task gradient), "m", "v"; "label_grad" / "label_m" / "label_v" for the
-        label-logit leaf of a joint trial."""
-        code = {"grad": 0, "grad_task": 1, "m": 2, "v": 3, "label_grad": 4, "label_m": 5, "label_v": 6}[which]
+        label-logit leaf of a joint trial, and "soft_q": the soft targets softmax(label logits) the last joint iteration evaluated."""
+        code = {"grad": 0, "grad_task": 1, "m": 2, "v": 3, "label_grad": 4, "label_m": 5, "label_v": 6, "soft_q": 7}[which]
         out = torch.empty(self._label_shape if code >= 4 else self.input_shape, dtype=torch.float32)
         _check(self.lib, self.lib.bre_engine_debug_step_state(self.h, code, _ptr(out)), "bre_engine_debug_step_state")
         return out
@@ -836,6 +838,42 @@ def last_gemm_plan():
     v = list(buf)
     return dict(family=GEMM_FAMILIES[v[0]], mode=v[1], nsrc=v[2], tile_rows=v[3], tile_width=v[4], splits=v[5], stages=v[6],
                 producer=GEMM_PRODUCERS[v[7]], total_kblocks=v[8], kblocks_per_split=v[9], vec=v[10])
+
+
+def row_plan(C):
+    """The plan of the cluster row kernels for rows of ``C`` elements: (CTAs per row, True when each CTA's segment is cached in
+    registers, False when it is streamed)."""
+    lib = load_library()
+    cs, fits = ctypes.c_int32(), ctypes.c_int32()
+    _check(lib, lib.bre_debug_row_plan(int(C), ctypes.byref(cs), ctypes.byref(fits)), "bre_debug_row_plan")
+    return cs.value, bool(fits.value)
+
+
+ROW_OPS = {"softmax": 0, "softmax_chain": 1, "token_ce_fwd": 2, "token_ce_tan_bwd": 3, "token_label_grad": 4, "ce_fwd": 5,
+           "ce_label_grad": 6, "ce_tan_bwd": 7}
+
+
+def row_op(op, in0, in1=None, in2=None, labels=None, C=None, T=1, coef=0.0, round_out=False, out0=None, out1=None, out2=None):
+    """One row kernel of the label leaf or the cross-entropy seeds through the engine's launcher (``bre_row_op``; the operands
+    of each ``op`` are listed in include/breaching_b200.h).  CUDA fp32 tensors [rows, width]; logits-shaped tensors of the token
+    ops may be wider than ``C`` (row stride Vs = their width).  Outputs are written in place; missing ones are allocated like
+    ``in0`` ([rows] for the loss).  Returns (out0, out1, out2)."""
+    lib = load_library()
+    rows, Vs = in0.shape
+    C = Vs if C is None else int(C)
+    for t in (in0, in1, in2, out0, out1, out2):
+        assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous())
+    assert labels is None or (labels.is_cuda and labels.dtype == torch.int64 and labels.is_contiguous())
+    fwd = op in ("token_ce_fwd", "ce_fwd")
+    out0 = torch.empty_like(in0) if out0 is None else out0
+    out1 = torch.empty(rows, dtype=torch.float32, device=in0.device) if fwd and out1 is None else out1
+    out2 = torch.empty_like(in0) if fwd and out2 is None else out2
+    stream = torch.cuda.current_stream(in0.device).cuda_stream
+    with torch.cuda.device(in0.device):
+        rc = lib.bre_row_op(ROW_OPS[op], _ptr(in0), _ptr(in1), _ptr(in2), _ptr(labels), rows, C, Vs, int(T), float(coef), int(bool(round_out)),
+                            _ptr(out0), _ptr(out1), _ptr(out2), ctypes.c_void_p(stream))
+    _check(lib, rc, "bre_row_op")
+    return out0, out1, out2
 
 
 def token_layernorm(sweep, x, gamma, beta, stats, in1=None, in2=None, in3=None, v_gamma=None, v_beta=None, eps=1e-5, want_param_grad=False,

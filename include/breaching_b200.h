@@ -207,7 +207,8 @@ int bre_engine_debug_tensor(bre_engine* e, int32_t which, int32_t tensor, float*
 /* Candidate-side buffers of the optimiser step as the last iteration left them (tests), to host: which 0 = the candidate gradient
  * the step read (before noise / clip / sign), 1 = the separate task-loss gradient (BRE_ERR_STATE when the step reads none: no
  * task_regularization, or already folded into 0), 2 / 3 = the optimiser moments m / v (SGD: m = momentum buffer); candidate-shaped.
- * 4 / 5 / 6 = gradient, m, v of the label-logit leaf of a joint trial ([N, classes]). */
+ * 4 / 5 / 6 = gradient, m, v of the label-logit leaf of a joint trial ([N, classes]); 7 = the soft targets q = softmax(label logits)
+ * that the last joint iteration handed to the evaluation ([N, classes]). */
 int bre_engine_debug_step_state(bre_engine* e, int32_t which, float* out_host);
 /* What the engine did with op `op` (tests): bit 0 = it ran in the epilogue of the preceding tensor-core GEMM in the last forward
  * sweep (fuse_bnact), bit 1 = its input tangent was not stored in the last tangent-forward sweep (that fused case), bit 2 = the
@@ -368,6 +369,26 @@ int bre_conv_gemm(int32_t mode, int32_t backend, const float* a, const float* w,
  * 2 cp.async, 3 TMA per parity class), total k-blocks, k-blocks per split (32-wide on the tensor cores, 16-wide on SIMT), vector
  * flags (SIMT: bit 0 A loads, bit 1 B loads, bit 2 stores; dgrad_small_ci / linear_small fprop: vector loads). */
 int bre_debug_last_gemm_plan(int32_t* out);
+/* The plan of the cluster row kernels (row softmax, softmax chain, token cross-entropy, its tangent, token label gradient) for rows
+ * of C elements: *cs = CTAs per row (1, 2, 4 or 8), *fits = 1 when each CTA's segment is cached in registers, 0 when it is streamed. */
+int bre_debug_row_plan(int32_t C, int32_t* cs, int32_t* fits);
+/* The row kernels of the label leaf and of the cross-entropy seeds, stand-alone through the engine's own launchers (parity tests).
+ * fp32 device pointers; rows >= 1, 1 <= C <= Vs; logits-shaped buffers of the token ops have row stride Vs, every other buffer
+ * row stride C (the other ops need Vs == C).  T: sequence length of the token ops (rows % T == 0); labels: int64 class indices
+ * in [0, C) (not checked).
+ *   BRE_ROW_SOFTMAX          out0 [rows, C] = softmax(in0) per row
+ *   BRE_ROW_SOFTMAX_CHAIN    out0 [rows, C] <- in0 * (out0 - <in0, out0>) per row (in place; in0 = q)
+ *   BRE_ROW_TOKEN_CE_FWD     in0 = logits, in1 = soft targets [rows, C]; out0 = p, out1 = loss per row [rows], out2 = dlogits
+ *   BRE_ROW_TOKEN_CE_TAN_BWD in0 = p, in1 = logits tangent; out0 = tangent dlogits
+ *   BRE_ROW_TOKEN_LABEL_GRAD in0 = logits, in1 = p, in2 = logits tangent, coef = task_regularization; out0 [rows, C]
+ *   BRE_ROW_CE_FWD           in0 = logits, labels or in1 = soft targets; out0 = p, out1 = loss per row, out2 = dlogits
+ *   BRE_ROW_CE_LABEL_GRAD    in0 = logits, in1 = p, in2 = logits tangent, coef = task_regularization; out0
+ *   BRE_ROW_CE_TAN_BWD       in0 = p, in1 = logits tangent; out0 = tangent dlogits; with labels: plus coef (p - onehot) / rows
+ * round_out != 0 stores dlogits / tangent dlogits on the TF32 grid (token ops and the labelled tangent only). */
+enum { BRE_ROW_SOFTMAX = 0, BRE_ROW_SOFTMAX_CHAIN = 1, BRE_ROW_TOKEN_CE_FWD = 2, BRE_ROW_TOKEN_CE_TAN_BWD = 3, BRE_ROW_TOKEN_LABEL_GRAD = 4,
+       BRE_ROW_CE_FWD = 5, BRE_ROW_CE_LABEL_GRAD = 6, BRE_ROW_CE_TAN_BWD = 7 };
+int bre_row_op(int32_t op, const float* in0, const float* in1, const float* in2, const int64_t* labels, int32_t rows, int32_t C, int32_t Vs,
+               int32_t T, float coef, int32_t round_out, float* out0, float* out1, float* out2, void* stream);
 
 const char* bre_last_error(void);
 const char* bre_version(void);

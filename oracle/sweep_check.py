@@ -43,6 +43,28 @@ Token programs (``compiler.compile_transformer``: tensors are [rows = B x T, C, 
   * ``check_label_gradient``: d objective / d target probabilities, ``-(zdot - <p, zdot>) / M - tau (z - lse) / M`` of the
     source row (row (b, t - 1) for tokens, 0 at t = 0), bounded like the seeds.
 
+The label leaf of a joint iteration (``check_label_leaf``; the row kernels ``row_softmax`` and ``softmax_chain``), and the row
+kernels alone (``check_row_kernel``; every relation is a module function that ``SweepChecker`` uses as well):
+
+  * row softmax ``q = softmax(l)``: the kernel takes the exact fp32 row max m, forms ``expf(l_c - m)`` (the argument rounded
+    once, ``u |l_c - m|``, and CUDA's ``expf`` within 2 ulp, ``4u``), sums them -- on the register path in runs of four fp32
+    adds folded into a double (``4u`` of the run), on the streamed path in double -- and merges the per-thread (m, s) pairs as
+    ``s e^(m - M)`` over lanes, warps and CTAs: a partial is rescaled at most ``SOFTMAX_MERGES = 19`` times (5 lane steps, 7 warps,
+    7 CTAs), each rescale one ``expf`` (``4u``) of a rounded difference (the differences along one chain add up to at most the
+    row range ``R = max l - min l``, ``u R``).  So the sum carries ``e_S = (8 + 4 SOFTMAX_MERGES) u + u R`` relative, and
+    ``q_c = expf(l_c - m) (1 / S)`` (the reciprocal rounded to fp32, the product rounded) is within
+    ``q_c ((6 + |l_c - m|) u + e_S)`` plus ``2^-147`` for results that underflow to subnormals;
+  * chain ``g <- q (g - <q, g>)`` on the engine's own fp32 q and un-chained g: the products are exact in double, the double
+    sum costs ``n 2^-53 sum |q g|`` and its rounding to fp32 ``u |<q, g>|``; the difference and the product one ``u`` each:
+    ``|q| (u |g - d| + u |d| + n 2^-53 sum |q g|) + u |ref|``, doubled;
+  * the cross-entropy forward (vision ``ce_fwd`` with class indices or soft targets, token ``token_ce_fwd``): p by the softmax
+    relation, the seed by the seed bound above, each row's loss by the per-row task-loss bound below (tokens: times
+    ``rows / M`` through the fp32 ``1 / M``, ``2u`` more); the tangent seeds (``ce_tan_bwd``, ``token_ce_tan_bwd``, the
+    labelled ``ce_tan_bwd_seed`` with ``coef (p - y) / N`` fused in) by the tangent-seed bound of sweep TB, evaluated on the
+    p the kernel read; the label gradients (``ce_label_grad``, ``token_label_grad``) by the label-gradient bound.  Outputs
+    stored on the TF32 grid add half a TF32 ulp.  Unscored token rows (each sequence's last row; every row when T = 1) and
+    label-gradient rows at t = 0 must be exactly zero.
+
 Multi-step (FedAvg) evaluations (``MultiStepChecker``; the engine's ``evaluate_multistep``, ``MultiStepInterpreter``): every
 local step k is checked as a single step, with W_k as the parameters (the BN constants follow from it), step k's labels, the
 direction u_{k+1} that step k used as ``v``, and no priors or task term in its candidate-gradient relation (that buffer is the
@@ -121,6 +143,8 @@ TRAIN_C = 8.0           # stated constant of the composite train-mode BN / DeepI
 POW_C = 8.0             # stated constant of one fp32 power (powf: 4 ulp), in units of u
 D53 = 2.0 ** -53        # one double rounding
 MASK_VALUE = float(torch.tensor(1e-6, dtype=torch.float32))   # masked-cosine threshold as the kernels compare it
+SOFTMAX_MERGES = 19     # rescales of one (m, s) partial in the cluster softmax: 5 lane steps, 7 warps, 7 CTAs
+SUBNORMAL = 2.0 ** -147  # absolute error of an fp32 result that underflows to a subnormal
 TERMS = ("match", "task_loss", "total_variation", "norm", "deep_inversion", "features")
 
 
@@ -198,6 +222,142 @@ def on_grid(t):
     return bool((torch.bitwise_and(f.view(torch.int32), 0x1FFF) == 0).all())
 
 
+def softmax_relation(z):
+    """q = softmax(z) per row as the row kernels form it: (float64 reference, per-element bound); see the module docstring."""
+    m = z.max(dim=1, keepdim=True).values
+    d = (z - m).abs()
+    R = (z.max(dim=1, keepdim=True).values - z.min(dim=1, keepdim=True).values)
+    q = torch.softmax(z, dim=1)
+    e_s = (8 + 4 * SOFTMAX_MERGES) * U + U * R
+    return q, q * ((6 + d) * U + e_s) + SUBNORMAL
+
+
+def chain_relation(q, g):
+    """Softmax chain ``q (g - <q, g>)`` per row on the fp32 q and g the kernel read: (reference, bound)."""
+    dot = (q * g).sum(dim=1, keepdim=True)
+    ref = q * (g - dot)
+    n = q.shape[1]
+    A = (q * g).abs().sum(dim=1, keepdim=True)
+    return ref, 2 * (q.abs() * (U * (g - dot).abs() + U * dot.abs() + n * D53 * A) + U * ref.abs())
+
+
+def seed_relation(z, t, M, keep=1.0):
+    """Cross-entropy seed ``(softmax(z) - t) / M`` on scored rows (``keep``) against the aligned targets t: (reference, bound)."""
+    p = torch.softmax(z, dim=1)
+    rng = (z - z.max(dim=1, keepdim=True).values).abs()
+    return (p - t) * keep / M, (16 + 2 * rng) * U * (p + t.abs()) * keep / M
+
+
+def tangent_seed_relation(p, zd, rng, M, keep=1.0):
+    """Tangent of the cross-entropy seed ``p (zd - <p, zd>) / M`` on scored rows: (reference, bound).  ``rng``: |z - max z| when
+    p is the float64 softmax of the stored logits (the kernel read its own fp32 p), 0 when p is what the kernel read."""
+    ref = (p * zd - p * (p * zd).sum(dim=1, keepdim=True)) * keep / M
+    mag = (p * zd.abs() + p * (p * zd.abs()).sum(dim=1, keepdim=True)) * keep / M
+    return ref, (16 + 2 * rng) * U * mag
+
+
+def label_gradient_relation(z, zd, p, p_rng, tau, M):
+    """d objective / d target probabilities of each logits row, ``-(zd - <p, zd>) / M - tau (z - lse) / M``: (reference, bound).
+    ``p``: the probabilities the kernel read (``p_rng`` as for ``tangent_seed_relation``)."""
+    lse = torch.logsumexp(z, dim=1, keepdim=True)
+    rng = (z - z.max(dim=1, keepdim=True).values).abs()
+    dot = (p * zd).sum(dim=1, keepdim=True)
+    ref = -(zd - dot) / M - tau * (z - lse) / M
+    # <p, zdot> from the stored fp32 p (softmax bound) in double; lse in fp32 from a double sum of expf; a few roundings each
+    bound = (4 * U * (zd.abs() + (p * zd.abs()).sum(dim=1, keepdim=True)) + ((16 + 2 * p_rng) * U * p * zd.abs()).sum(dim=1, keepdim=True)
+             + abs(tau) * (8 * U * (z.abs() + lse.abs()) + (4 + 2 * rng.amax(dim=1, keepdim=True)) * U)) / M + U * ref.abs()
+    return ref, bound
+
+
+def to_target_rows(t, seq):
+    """Token programs: the relation of logits row (b, t - 1) belongs to target row (b, t); rows at t = 0 are exactly zero."""
+    first = (torch.arange(t.shape[0], device=t.device) % seq == 0).view(-1, 1)
+    return torch.cat([torch.zeros_like(t[:1]), t[:-1]]).masked_fill(first, 0.0)
+
+
+def task_loss_rows(z, q):
+    """Per-row cross-entropy ``-sum_c q_c (z_c - lse)`` against targets q [rows, C] (one-hot for class indices): (loss, bound)."""
+    mx = z.max(dim=1, keepdim=True).values
+    lse = torch.logsumexp(z, dim=1, keepdim=True)
+    rng = (z - mx).abs().amax(dim=1, keepdim=True)
+    ln = -(q * (z - lse)).sum(dim=1)
+    en = (q.abs() * ((16 + 2 * rng) * U + 4 * U * ((z - mx).abs() + mx.abs() + (lse - mx).abs()))).sum(dim=1) + 2 * U * ln.abs()
+    return ln, en
+
+
+def token_rows(rows, seq, device=None):
+    """Token programs: (scored-row mask [rows, 1], M = rows - rows / T; 1 when no row is scored)."""
+    keep = ((torch.arange(rows, device=device) % seq) != seq - 1).double().view(-1, 1)
+    return keep, max(rows - rows // seq, 1)
+
+
+def row_kernel_relations(kernel, z=None, q=None, g=None, p=None, zd=None, labels=None, T=1, coef=0.0, round_out=False):
+    """(reference, bound) of every output of one row kernel (``engine.row_op``) from float64 inputs [rows, C]: ``z`` logits, ``q``
+    soft targets / probabilities of the chain, ``g`` un-chained gradient, ``p`` probabilities the kernel read, ``zd`` logits
+    tangent, ``labels`` class indices.  Returns {output name: (reference, bound)}."""
+    tf = TF32_HALF if round_out else 0.0
+    if kernel == "softmax":
+        return {"q": softmax_relation(z)}
+    if kernel == "softmax_chain":
+        return {"g": chain_relation(q, g)}
+    rows, C = (z if z is not None else p).shape
+    if kernel in ("token_ce_fwd", "ce_fwd"):
+        token = kernel == "token_ce_fwd"
+        t = q if labels is None else F.one_hot(labels.view(-1).long(), C).to(z.dtype)
+        keep, M = token_rows(rows, T, z.device) if token else (1.0, rows)
+        if token:
+            t = torch.cat([t[1:], torch.zeros_like(t[:1])]) * keep   # row (b, t) is scored against target row (b, t + 1)
+        d, db = seed_relation(z, t, M, keep)
+        ln, en = task_loss_rows(z, t)
+        if token:
+            ln, en = ln * keep.view(-1) * rows / M, (en * rows / M + 2 * U * ln.abs() * rows / M) * keep.view(-1)
+        return {"p": softmax_relation(z), "loss": (ln, en), "dlogits": (d, db + tf * (d.abs() + db))}
+    if kernel in ("token_ce_tan_bwd", "ce_tan_bwd"):
+        keep, M = token_rows(rows, T, p.device) if kernel == "token_ce_tan_bwd" else (1.0, rows)
+        ref, bound = tangent_seed_relation(p, zd, 0.0, M, keep)
+        if labels is not None:   # the labelled tangent seed: coef (p - y) / N fused in
+            y = F.one_hot(labels.view(-1).long(), C).to(p.dtype)
+            ref = ref + coef * (p - y) / M
+            bound = bound + 4 * U * abs(coef) * (p + y) / M + 2 * U * ref.abs()
+        return {"tdlogits": (ref, bound + tf * (ref.abs() + bound))}
+    if kernel in ("token_label_grad", "ce_label_grad"):
+        token = kernel == "token_label_grad"
+        M = token_rows(rows, T)[1] if token else rows
+        ref, bound = label_gradient_relation(z, zd, p, 0.0, coef, M)
+        if token:
+            ref, bound = to_target_rows(ref, T), to_target_rows(bound, T)
+        return {"out": (ref, bound)}
+    raise ValueError(kernel)
+
+
+def worst_element(y, ref, bound):
+    """(worst error / bound ratio, flat index of that element); NaN counts as infinitely wrong, an exact match as 0."""
+    err = (y - ref).abs()
+    ratio = err / bound.clamp_min(TINY) if torch.is_tensor(bound) else err / max(bound, TINY)
+    ratio = torch.where(err == 0, torch.zeros_like(ratio), ratio)
+    ratio = torch.nan_to_num(ratio, nan=float("inf"))
+    if not ratio.numel():
+        return 0.0, 0
+    j = int(ratio.flatten().argmax())
+    return float(ratio.flatten()[j]), j
+
+
+def check_row_kernel(kernel, outputs, **inputs):
+    """Findings (kind = the kernel, sweep = the output name, index = the worst element) of one row kernel's ``outputs`` (dict of
+    fp32 or float64 tensors keyed like ``row_kernel_relations``) against its relations; also returns {output: worst ratio}."""
+    findings, ratios = [], {}
+    for name, (ref, bound) in row_kernel_relations(kernel, **inputs).items():
+        y = outputs[name].double().reshape(ref.shape)
+        worst, j = worst_element(y, ref, bound)
+        ratios[name] = worst
+        if not worst <= 1.0:
+            idx = tuple(int(v) for v in torch.unravel_index(torch.tensor(j), y.shape))
+            b = bound.expand_as(ref).flatten()[j] if torch.is_tensor(bound) else torch.tensor(bound)
+            e = (y - ref).abs().flatten()[j]
+            findings.append(Finding(-1, kernel, name, f"{kernel} {name}", idx, float(y.flatten()[j]), float(ref.flatten()[j]), float(e), float(b)))
+    return findings, ratios
+
+
 class Finding:
     def __init__(self, op, kind, sweep, what, index, value, ref, err, bound, step=None):
         self.op, self.kind, self.sweep, self.what = op, kind, sweep, what
@@ -267,13 +427,10 @@ class SweepChecker:
     def _cmp(self, i, sweep, what, y, ref, bound, kind=None):
         kind = kind or ("objective" if i < 0 else C.OP_NAMES[self.prog.ops[i].kind])
         err = (y - ref).abs()
-        ratio = err / bound.clamp_min(TINY) if torch.is_tensor(bound) else err / max(bound, TINY)
-        ratio = torch.where(err == 0, torch.zeros_like(ratio), ratio)
-        worst = float(ratio.max()) if ratio.numel() else 0.0
+        worst, j = worst_element(y, ref, bound)
         key = (kind, sweep)
         self.ratios[key] = max(self.ratios.get(key, 0.0), worst)
         if not worst <= 1.0:   # also catches NaN
-            j = int(torch.nan_to_num(ratio, nan=float("inf")).flatten().argmax())
             idx = tuple(int(v) for v in torch.unravel_index(torch.tensor(j), y.shape)) if y.dim() else ()
             b = bound.expand_as(ref).flatten()[j] if torch.is_tensor(bound) else torch.tensor(bound)
             self.findings.append(Finding(i, kind, sweep, what, idx, float(y.flatten()[j]), float(ref.flatten()[j]),
@@ -414,8 +571,7 @@ class SweepChecker:
 
     def _seed_rows(self, rows):
         """Token programs: (scored-row mask [rows, 1], M)."""
-        keep = ((torch.arange(rows) % self.seq) != self.seq - 1).double().view(-1, 1)
-        return keep, rows - rows // self.seq
+        return token_rows(rows, self.seq)
 
     def _targets(self, n):
         """Soft targets [n, classes] (float64) or the one-hot of class-index labels."""
@@ -534,17 +690,12 @@ class SweepChecker:
                 ref, bound = self._merge(O).view_as(y), self._merge(eO).view_as(y)
                 self._cmp(i, "F", f"val[t{op.tout}]", y, ref, bound + self._rounded(y, ref))
         z = self.T("val", prog.logits).flatten(1)
-        self.p = torch.softmax(z, dim=1)
         self._padding("val", len(prog.ops) - 1, "F")
         if self.seq:   # the next-token seed is checked with sweep B
             return
         # cross-entropy seed of sweep B (class indices or soft targets)
         n = z.shape[0]
-        p = self.p
-        q = self._targets(n)
-        ref = (p - q) / n
-        rng = (z - z.max(dim=1, keepdim=True).values).abs()
-        bound = (16 + 2 * rng) * U * (p + q.abs()) / n
+        ref, bound = seed_relation(z, self._targets(n), n)
         d = self.T("delta", prog.logits).flatten(1)
         self._cmp(len(prog.ops) - 1, "F", f"delta[t{prog.logits}] (cross-entropy seed)", d, ref, bound)
 
@@ -558,14 +709,10 @@ class SweepChecker:
         z = self.T("val", prog.logits).flatten(1)
         rows = z.shape[0]
         keep, M = self._seed_rows(rows)
-        p = self.p
         q = self._targets(rows)
         qn = torch.zeros_like(q)
         qn[:-1] = q[1:]
-        qn = qn * keep
-        ref = (p - qn) * keep / M
-        rng = (z - z.max(dim=1, keepdim=True).values).abs()
-        bound = (16 + 2 * rng) * U * (p + qn) * keep / M
+        ref, bound = seed_relation(z, qn * keep, M, keep)
         d = self.T("delta", prog.logits).flatten(1)
         self._cmp(len(prog.ops) - 1, "B", f"delta[t{prog.logits}] (next-token loss seed)", d, ref, bound + self._rounded(d, ref))
         self._padding("delta", len(prog.ops) - 1, "B")
@@ -953,13 +1100,10 @@ class SweepChecker:
         zd = self.T("tangent", prog.logits).flatten(1)
         n = z.shape[0]
         keep, M = self._seed_rows(n) if self.seq else (1.0, n)
-        p = torch.softmax(z, dim=1)
-        ref = (p * zd - p * (p * zd).sum(dim=1, keepdim=True)) * keep / M
         rng = (z - z.max(dim=1, keepdim=True).values).abs()
-        mag = (p * zd.abs() + p * (p * zd.abs()).sum(dim=1, keepdim=True)) * keep / M
+        ref, bound = tangent_seed_relation(torch.softmax(z, dim=1), zd, rng, M, keep)
         y = self.T("tangent_delta", prog.logits).flatten(1)
-        self._cmp(len(prog.ops) - 1, "TB", f"tangent_delta[t{prog.logits}] (cross-entropy seed)", y, ref,
-                  (16 + 2 * rng) * U * mag + self._rounded(y, ref))
+        self._cmp(len(prog.ops) - 1, "TB", f"tangent_delta[t{prog.logits}] (cross-entropy seed)", y, ref, bound + self._rounded(y, ref))
         self._padding("tangent_delta", len(prog.ops) - 1, "TB")
         contrib = self._check_deltas("TB", self._reverse("TB"))
         # the candidate gradient: first op's contribution + image priors + task term
@@ -995,22 +1139,28 @@ class SweepChecker:
         z = self.T("val", self.prog.logits).flatten(1)
         zd = self.T("tangent", self.prog.logits).flatten(1)
         n = z.shape[0]
-        tau = self.obj["task_regularization"]
-        p = torch.softmax(z, dim=1)
-        lse = torch.logsumexp(z, dim=1, keepdim=True)
-        rng = (z - z.max(dim=1, keepdim=True).values).abs()
         M = n - n // self.seq if self.seq else n
-        dot = (p * zd).sum(dim=1, keepdim=True)
-        ref = -(zd - dot) / M - tau * (z - lse) / M
-        # <p, zdot> from the stored fp32 p (softmax bound) in double; lse in fp32 from a double sum of expf; a few roundings each
-        bound = (4 * U * (zd.abs() + (p * zd.abs()).sum(dim=1, keepdim=True)) + ((16 + 2 * rng) * U * p * zd.abs()).sum(dim=1, keepdim=True)
-                 + abs(tau) * (8 * U * (z.abs() + lse.abs()) + (4 + 2 * rng.amax(dim=1, keepdim=True)) * U)) / M + U * ref.abs()
+        rng = (z - z.max(dim=1, keepdim=True).values).abs()
+        ref, bound = label_gradient_relation(z, zd, torch.softmax(z, dim=1), rng, self.obj["task_regularization"], M)
         if self.seq:
-            first = (torch.arange(n) % self.seq == 0).view(-1, 1)
-            ref = torch.cat([torch.zeros_like(ref[:1]), ref[:-1]]).masked_fill(first, 0.0)
-            bound = torch.cat([torch.zeros_like(bound[:1]), bound[:-1]]).masked_fill(first, 0.0)
+            ref, bound = to_target_rows(ref, self.seq), to_target_rows(bound, self.seq)
         y = lg.double().reshape(n, -1)
         self._cmp(len(self.prog.ops) - 1, "L", "label gradient", y, ref, bound, kind="label")
+        if raise_on_failure and self.findings:
+            raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
+        return self.findings
+
+    def check_label_leaf(self, ell, q, g_pre, g_chained, raise_on_failure=True):
+        """The label leaf of a joint iteration: ``q`` (the soft targets the evaluation read, ``debug_step_state("soft_q")``)
+        against softmax of the label logits ``ell`` the iteration started from, and ``g_chained`` (``debug_step_state("label_grad")``)
+        against the softmax chain of the engine's own q and un-chained gradient ``g_pre`` (``label_gradient``).  Reported with
+        the kernel's name as the kind, sweep "L"."""
+        n = ell.shape[0]
+        q64, g64 = q.double().reshape(n, -1), g_pre.double().reshape(n, -1)
+        ref, bound = softmax_relation(ell.double().reshape(n, -1))
+        self._cmp(-1, "L", "soft targets q = softmax(label logits)", q64, ref, bound, kind="row_softmax")
+        ref, bound = chain_relation(q64, g64)
+        self._cmp(-1, "L", "label-logit gradient q (g - <q, g>)", g_chained.double().reshape(n, -1), ref, bound, kind="softmax_chain")
         if raise_on_failure and self.findings:
             raise SweepCheckError("\n".join(repr(f) for f in self.findings[:20]))
         return self.findings
@@ -1025,12 +1175,7 @@ class SweepChecker:
 
     def _task_loss_term(self):
         z = self.T("val", self.prog.logits).flatten(1)
-        q = self._targets(z.shape[0])
-        mx = z.max(dim=1, keepdim=True).values
-        lse = torch.logsumexp(z, dim=1, keepdim=True)
-        rng = (z - mx).abs().amax(dim=1, keepdim=True)
-        ln = -(q * (z - lse)).sum(dim=1)
-        en = (q.abs() * ((16 + 2 * rng) * U + 4 * U * ((z - mx).abs() + mx.abs() + (lse - mx).abs()))).sum(dim=1) + 2 * U * ln.abs()
+        ln, en = task_loss_rows(z, self._targets(z.shape[0]))
         L = float(ln.mean())
         return L, float(en.mean()) + U * abs(L)
 

@@ -2,7 +2,8 @@
 multi-head attention, linears, residual adds, next-token loss with soft targets over a padded vocabulary) against a float64
 restatement of its own op (oracle/sweep_check.py), on both GEMM back ends; plus the label gradient, the padded logit columns
 (exactly zero), and the TF32 grid of every tensor-core operand on the tensor-core back end.  A soft-label vision case runs the
-same seed and label-gradient checks on a CNN."""
+same seed and label-gradient checks on a CNN.  One joint data + label iteration (``iteration_joint``) is checked end to end: the
+soft targets q = softmax(label logits), every sweep buffer on that q, the un-chained label gradient and its softmax chain."""
 import copy
 
 import pytest
@@ -26,6 +27,11 @@ TEXT_CASES = {
     "task-reg": (MULTI_SEQ, {"objective.task_regularization": 0.2}),
     "config5": "config5",                                 # full size: V = 50 257 -> 50 304, cluster CE kernels, tall decoder dgrad
 }
+# one vocabulary per plan of the cluster row kernels not reached above: 2 and 4 CTAs per row, BERT's 30 522 on 8, and 65 500 (65 536
+# padded) streaming its segments
+WIDE_VOCAB = dict(batch=2, seq_len=8, seed=23, ninp=16, nhead=2, nhid=32, nlayers=1)
+for _V in (5000, 12000, 30522, 65500):
+    TEXT_CASES[f"vocab-{_V}"] = (dict(WIDE_VOCAB, ntokens=_V), {})
 
 
 def text_case(name):
@@ -124,3 +130,86 @@ def test_soft_label_vision_seed_and_label_gradient(backend):
     finally:
         eng.close()
     assert ("label", "L") in chk.ratios and ("linear", "F") in chk.ratios
+
+
+class JointSource(EngineSource):
+    """The engine's buffers after one joint iteration.  Tensor 0's value is the candidate buffer itself, which the step has
+    already moved: the iteration evaluated ``x0``."""
+
+    def __init__(self, eng, x0):
+        super().__init__(eng)
+        self.x0 = x0.detach().double().cpu()
+
+    def tensor(self, which, tid):
+        if tid == 0 and which == "val":
+            return self.x0.view(self.eng.debug_tensor("val", 0).shape)
+        return super().tensor(which, tid)
+
+
+def check_joint_iteration(eng, params, bn, grads, cfg, x0, ell0, tag):
+    """begin_joint_trial(x0, l0), run(1); then q, the chained label gradient the step read, and last the un-chained gradient
+    (``label_gradient`` recomputes it into the same buffer)."""
+    eng.begin_joint_trial(x0.to(DEV), ell0.to(DEV), [1e-2])
+    eng.run(1)
+    eng.sync()
+    q = eng.debug_step_state("soft_q")
+    g_chained = eng.debug_step_state("label_grad")
+    g_pre = eng.label_gradient(tuple(ell0.shape)).cpu()
+    moved = not torch.equal(eng.debug_tensor("val", 0).view(-1), x0.cpu().view(-1))
+    chk = SweepChecker(eng.prog, params, bn, grads, q, sweep_objective(cfg), JointSource(eng, x0))
+    try:
+        chk.check(raise_on_failure=False)
+        chk.check_label_gradient(g_pre, raise_on_failure=False)
+        chk.check_label_leaf(ell0, q, g_pre, g_chained, raise_on_failure=False)
+        if not eng.prog.seq_len:
+            chk.check_terms(eng.last_terms(), raise_on_failure=False)
+    finally:
+        report(chk, f"joint {tag}; candidate moved by the step: {moved}")
+    assert not chk.findings, "\n".join(repr(f) for f in chk.findings[:20])
+    assert {("row_softmax", "L"), ("softmax_chain", "L"), ("label", "L")} <= set(chk.ratios)
+    return chk
+
+
+JOINT_TEXT = ["tag-mini", "vocab-5000", "vocab-12000", "vocab-30522", "vocab-65500", "config5"]
+
+
+@pytest.mark.parametrize("backend", ["simt", "tc"])
+@pytest.mark.parametrize("name", JOINT_TEXT)
+def test_joint_iteration_label_leaf_and_sweeps(name, backend):
+    if name == "config5" and backend == "simt":
+        pytest.skip("full size on the tensor-core back end, as bench.py --config 5 runs it")
+    model, B, T, grads, cfg = text_case(name)
+    params = [p.detach() for n, p in model.named_parameters() if n != "encoder.weight"]
+    d, V = model.decoder.in_features, model.decoder.out_features
+    prog = compiler.compile_transformer(model, B, T)
+    eng = Engine(None, (B * T, d, 1, 1), cfg, DEV, backend=backend, program=prog)
+    try:
+        eng.load_model(params=params)
+        L = len(grads)
+        eng.load_targets([g.to(DEV) for g in grads], torch.zeros(B * T, dtype=torch.long),
+                         tensor_weights=torch.arange(L, 0, -1, dtype=torch.float32) / L)
+        gen = torch.Generator().manual_seed(31)
+        x0, ell0 = torch.randn(B * T, d, 1, 1, generator=gen), torch.randn(B * T, V, generator=gen)
+        check_joint_iteration(eng, params, [None] * len(prog.ops), grads, cfg, x0, ell0, f"{name} / {backend}")
+    finally:
+        eng.close()
+
+
+@pytest.mark.parametrize("backend", ["simt", "tc"])
+def test_joint_iteration_vision_fixture(backend):
+    """The joint Adam fixture's ConvNet (10 classes): ``ce_label_grad`` under the chain."""
+    fx = load_golden("trial_joint_adam_convnet.pt")
+    model, _, _, shared, true = case_from_fixture(fx)
+    cfg = cfg_from_fixture(fx)
+    model.eval()
+    x0, ell0 = fx["x0"].float(), fx["l0"].float()
+    grads = shared[0]["gradients"]
+    eng = Engine(copy.deepcopy(model).to(DEV), tuple(x0.shape), cfg, DEV, backend=backend)
+    try:
+        eng.load_model()
+        eng.load_targets([g.to(DEV) for g in grads], true["labels"].to(DEV))
+        bn = [None if m is None or m.running_mean is None else (m.running_mean.double(), m.running_var.double())
+              for m in compiler.bn_modules(model, eng.prog)]
+        check_joint_iteration(eng, list(model.parameters()), bn, grads, cfg, x0, ell0, f"joint_adam_convnet / {backend}")
+    finally:
+        eng.close()
