@@ -3,12 +3,15 @@
 pipeline of ``csrc/augment.cu``.
 
 Supported, in config order: ``discrete_shift`` (``Jitter``), ``flip`` (``Flip``), ``colorjitter`` (``ColorJitter``; constants drawn
-once per attacker like the module's ``shuffled`` flag) and ``continuous_shift`` (``RandomTransform``: bilinear, ``align=True``,
-``padding`` ``circular`` / ``zeros``; must come after the shift / flip steps of its run), and the shape-changing ``zoom`` (``Zoom``),
+once per attacker like the module's ``shuffled`` flag) and ``continuous_shift`` (``RandomTransform``: ``align=True`` as the module forces,
+``mode`` bilinear / nearest / bicubic, ``padding`` reflection (the module's default) / border / zeros / circular, ``fliplr`` /
+``flipud`` grid flips drawn per image), and the shape-changing ``zoom`` (``Zoom``),
 ``centerzoom`` (``CenterZoom``), ``focus`` (``Focus``, its window corner drawn on the device every evaluation) and ``antialias``
 (``AntiAlias``).  A config with only the first four kinds is one pipeline of shape-keeping steps (``AugmentationPlan.steps`` and the
 colour / continuous-shift fields).  With any of the others the view is an ordered list of ``Stage`` s: each maximal run of the
 shape-keeping kinds is one ``PIXEL`` stage, each zoom / centerzoom / focus a ``RESAMPLE`` stage and each antialias a ``BLUR`` stage.
+The device applies a stage's continuous shift after its shift / flip steps, so a ``discrete_shift`` or ``flip`` after a
+``continuous_shift`` opens a new ``PIXEL`` stage; a config of the shape-keeping kinds in such an order is a list of ``PIXEL`` stages.
 The model then runs on the view's shape (``view_shape``), which may differ from the candidate's; the reference's objective and every
 regulariser see the view (``:161-162``), and the gradient is pulled back onto the candidate.  A stage that changes the shape needs
 ``differentiable_augmentations: True`` (the reference's non-differentiable mode would replace the candidate by its view and shrink or
@@ -25,6 +28,9 @@ from ..config import cfg_get
 SHIFT, FLIP = 1, 2
 PIXEL, RESAMPLE, BLUR = "pixel", "resample", "blur"
 _PIXEL_KINDS = ("discrete_shift", "flip", "colorjitter", "continuous_shift")
+_GRID_KINDS = ("discrete_shift", "flip", "continuous_shift")       # what a continuous shift must come after within one stage
+CS_MODES = {"bilinear": 0, "nearest": 1, "bicubic": 2}              # grid_sample mode / padding_mode -> bre_augment_view_ex codes
+CS_PADDINGS = {"zeros": 0, "border": 1, "reflection": 2}
 _VIEW_KINDS = ("zoom", "centerzoom", "focus", "antialias")
 _UNSUPPORTED = ("median",)
 MAX_STAGES = 8
@@ -40,6 +46,10 @@ class Stage:
     circular: bool = False
     colour_scale: Optional[torch.Tensor] = None
     colour_shift: Optional[torch.Tensor] = None
+    cs_mode: str = "bilinear"                                        # PIXEL: continuous_shift sampling, as AugmentationPlan
+    cs_padding: str = "zeros"
+    fliplr: bool = False
+    flipud: bool = False
     corner: Tuple[int, int] = (0, 0)                                 # RESAMPLE: window corner (row, column) and size
     window: Tuple[int, int] = (0, 0)
     focus_std: Optional[float] = None                                # RESAMPLE (focus): corner drawn per evaluation
@@ -58,6 +68,10 @@ class AugmentationPlan:
     seed: int = 0
     stages: List[Stage] = field(default_factory=list)               # empty: the fields above are the whole (shape-keeping) view
     candidate_shape: Optional[Tuple[int, int, int, int]] = None     # with stages: [N, C, H, W] of the candidate
+    cs_mode: str = "bilinear"                                       # grid_sample mode of the continuous shift
+    cs_padding: str = "zeros"                                       # its padding_mode ("circular": zeros after the wrap, circular=True)
+    fliplr: bool = False                                            # RandomTransform's grid flips
+    flipud: bool = False
 
 
 def _opts(aug, key):
@@ -96,6 +110,25 @@ def _geometry(key, opts, C, H, W):
     raise KeyError(key)
 
 
+def _stage_starts(aug):
+    """The keys that open a PIXEL stage: a shape-keeping kind at the start or after a shape-changing one, and a discrete_shift, flip or
+    continuous_shift after a continuous_shift of the same stage."""
+    starts, in_run, shifted = set(), False, False
+    for key in aug.keys():
+        if key in _VIEW_KINDS:
+            in_run = False
+        elif key in _PIXEL_KINDS:
+            if not in_run or (shifted and key in _GRID_KINDS):
+                starts.add(key)
+                in_run, shifted = True, False
+            shifted = shifted or key == "continuous_shift"
+    return starts
+
+
+def _needs_stages(aug):
+    return any(k in _VIEW_KINDS for k in aug.keys()) or len(_stage_starts(aug)) > 1
+
+
 def has_view_stages(cfg_attack):
     """Does the config contain a shape-changing kind (zoom, centerzoom, focus, antialias)?  Draws nothing."""
     aug = cfg_get(cfg_attack, "augmentations")
@@ -131,10 +164,11 @@ def build_plan(cfg_attack, batch, channels, setup, spatial=None):
     if aug is None or len(list(aug.keys())) == 0:
         return None
     plan = AugmentationPlan(differentiable=bool(cfg_get(cfg_attack, "differentiable_augmentations", False)))
-    staged = has_view_stages(cfg_attack)
+    staged = _needs_stages(aug)
+    starts = _stage_starts(aug)
     if staged:
         if spatial is None:
-            raise ValueError("shape-changing augmentations need the candidate's spatial shape")
+            raise ValueError("shape-changing augmentations and shift / flip steps after a continuous_shift need the candidate's spatial shape")
         view_shape(cfg_attack, (batch, channels, *spatial))       # shape refusals before anything is drawn
         H, W = int(spatial[0]), int(spatial[1])
     scale = torch.ones(batch, channels, device=setup["device"])
@@ -152,16 +186,13 @@ def build_plan(cfg_attack, batch, channels, setup, spatial=None):
 
     for key in aug.keys():
         opts = _opts(aug, key)
-        if key in _PIXEL_KINDS and staged and run is None:
+        if key in _PIXEL_KINDS and staged and (run is None or key in starts):
+            close_run()
             run = Stage(PIXEL, (H, W), (H, W))
         target = run if staged and key in _PIXEL_KINDS else plan
         if key == "discrete_shift":                        # Jitter(lim=32)
-            if target.continuous_shift is not None:
-                raise NotImplementedError("discrete_shift after continuous_shift is not implemented by the engine")
             target.steps.append((SHIFT, float(opts.get("lim", 32))))
         elif key == "flip":                                # Flip(p=0.5)
-            if target.continuous_shift is not None:
-                raise NotImplementedError("flip after continuous_shift is not implemented by the engine")
             target.steps.append((FLIP, float(opts.get("p", 0.5))))
         elif key == "colorjitter":                         # ColorJitter(mean=0.0, std=1.0): (img - mean) / std, drawn once (:77-83)
             if channels != 3:
@@ -177,15 +208,15 @@ def build_plan(cfg_attack, batch, channels, setup, spatial=None):
             else:
                 scale, shift = scale / sd, (shift - m) / sd
                 any_colour = True
-        elif key == "continuous_shift":                    # RandomTransform(shift=8, padding="reflection", ...)
-            if target.continuous_shift is not None:
-                raise NotImplementedError("two continuous_shift steps are not implemented by the engine")
-            if opts.get("fliplr", False) or opts.get("flipud", False) or opts.get("mode", "bilinear") != "bilinear":
-                raise NotImplementedError("continuous_shift: only bilinear sampling without grid flips is implemented")
-            padding = opts.get("padding", "reflection")
-            if padding not in ("circular", "zeros"):
-                raise NotImplementedError(f"continuous_shift padding {padding} is not implemented by the engine (circular / zeros)")
+        elif key == "continuous_shift":                    # RandomTransform(shift=8, fliplr=False, flipud=False, mode="bilinear", padding="reflection")
+            mode, padding = opts.get("mode", "bilinear"), opts.get("padding", "reflection")
+            if mode not in CS_MODES:                       # the errors of F.grid_sample
+                raise ValueError(f"continuous_shift: mode must be one of bilinear, nearest, bicubic, got {mode!r}")
+            if padding not in (*CS_PADDINGS, "circular"):
+                raise ValueError(f"continuous_shift: padding must be one of zeros, border, reflection, circular, got {padding!r}")
             target.continuous_shift, target.circular = float(opts.get("shift", 8)), padding == "circular"
+            target.cs_mode, target.cs_padding = mode, "zeros" if padding == "circular" else padding
+            target.fliplr, target.flipud = bool(opts.get("fliplr", False)), bool(opts.get("flipud", False))
         elif key in _VIEW_KINDS:
             close_run()
             st = _geometry(key, opts, channels, H, W)
@@ -216,13 +247,12 @@ def with_spatial(plan, cfg_attack, spatial):
     view_shape(cfg_attack, (N, C, H, W))
     aug = cfg_get(cfg_attack, "augmentations")
     runs = iter([st for st in plan.stages if st.kind == PIXEL])
-    stages, in_run = [], False
+    starts = _stage_starts(aug)
+    stages = []
     for key in aug.keys():
         if key in _VIEW_KINDS:
-            in_run = False
             stages.append(_geometry(key, _opts(aug, key), C, H, W))
             H, W = stages[-1].out_hw
-        elif not in_run:                                   # the next run of shape-keeping kinds, at this point's shape
-            in_run = True
+        elif key in starts:                                # the next PIXEL stage, at this point's shape
             stages.append(replace(next(runs), in_hw=(H, W), out_hw=(H, W)))
     return replace(plan, stages=stages, candidate_shape=(N, C, int(spatial[0]), int(spatial[1])))

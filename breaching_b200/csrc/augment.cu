@@ -4,10 +4,13 @@
 //   discrete_shift  (Jitter :9-18)            torch.roll by two random offsets in [-lim, lim), one draw per forward, whole batch
 //   flip            (Flip :57-64)             horizontal flip with probability p, one draw per forward
 //   colorjitter     (ColorJitter :70-89)      (x - mean[n, c]) / std[n, c], constants drawn once per attacker
-//   continuous_shift (RandomTransform :141-205) bilinear grid_sample (align_corners = True) on the grid
-//                                             g(i, j) = (lin[j] + sx[n], lin[i] + sy[n]), lin = linspace(-1, 1, S), per-image random shifts
-//                                             of at most shift / (S - 1); padding "circular" maps g -> ((g + 1) mod 1) - 1 as the
-//                                             reference does (which samples the top-left quadrant twice per axis -- reproduced)
+//   continuous_shift (RandomTransform :141-205) grid_sample (align_corners = True; bilinear, nearest or bicubic; zeros, border or
+//                                             reflection padding) on the grid g(i, j) = (lin[j] + sx[n], lin[i] + sy[n]),
+//                                             lin = linspace(-1, 1, S), per-image random shifts of at most shift / (S - 1), each
+//                                             coordinate negated per image by the fliplr / flipud grid flips; padding "circular" maps
+//                                             g -> ((g + 1) mod 1) - 1 and samples with zeros padding as the reference does (which samples
+//                                             the top-left quadrant twice per axis -- reproduced).  The grid is separable, so every output
+//                                             row / column reads at most 4 taps of its axis (cs_taps), and the pull-back is two 1-D gathers.
 // Shape-changing stages (each a stage of its own, see AugStage): RESAMPLE = a window resized bilinearly (Zoom :34-40, CenterZoom :43-55,
 // Focus :20-31), BLUR = binomial depthwise convolution (AntiAlias :198-226).  Their pull-backs are fixed-order gathers (no atomics).
 // Random draws come from Philox keyed by (seed, iteration, step), so the forward view and the transposed pull-back of one
@@ -70,12 +73,14 @@ __global__ void aug_draw_kernel(AugPipeline pipe, const Scalars* sc, AugDraws* d
         d->o1[s] = u01(r[0]) < plan.p0[s] ? 1 : 0;
       }
     }
-    // continuous shift: two uniforms per image
+    // continuous shift: two uniforms per image, and the grid flips from the third and fourth word (randgen[:, 2:4] > 0.5)
     for (int n = threadIdx.x; n < N; n += blockDim.x) {
       uint32_t r[4];
       philox4(plan.seed, (uint32_t)it, 0xC0FFEEu, (uint32_t)n, r);
       d->sx[n] = u01(r[0]);
       d->sy[n] = u01(r[1]);
+      d->flr[n] = plan.cs_fliplr && u01(r[2]) > 0.5f;
+      d->fud[n] = plan.cs_flipud && u01(r[3]) > 0.5f;
     }
   }
 }
@@ -99,47 +104,99 @@ __device__ __forceinline__ void map_forward(const AugPlan& plan, const AugDraws&
   }
 }
 
-// continuous shift: source coordinate of output index `o` along an axis of extent S, for the uniform u of this image
-__device__ __forceinline__ void cs_coord(const AugPlan& plan, float u, int o, int S, int& i0, float& frac) {
-  const float lin = S > 1 ? -1.f + 2.f * (float)o / (float)(S - 1) : -1.f;
-  const float delta = plan.cs_shift / (float)(S - 1);
-  float g = lin + (u - 0.5f) * 2.f * delta;
-  if (plan.cs_circular) g = (g + 1.f) - floorf(g + 1.f) - 1.f;     // python's (g + 1) % 1 - 1
-  const float pos = (g + 1.f) * 0.5f * (float)(S - 1);              // align_corners = True
-  const float fl = floorf(pos);
-  i0 = (int)fl;
-  frac = pos - fl;
+// continuous shift along one axis of extent S: the taps of output index o for the uniform u and flip bit of its image, following
+// ATen's grid sampler (GridSampler.h) with align_corners = True.  The coordinate is computed in double: the fp32 weights are then the
+// float64 reference's rounded once.  bilinear / nearest: the unnormalised coordinate is clipped (border) or reflected about 0 and
+// S - 1 and clipped (reflection), then sampled, and taps outside [0, S) read zero; nearest rounds half to even.  bicubic: four taps
+// floor - 1 .. floor + 2 of the raw coordinate with the cubic-convolution weights (A = -0.75), each tap index passed through the
+// padding rule on its own (several taps may land on one pixel).  idx = -1: a tap that reads zero.
+struct CsTaps { short idx[4]; float w[4]; };
+
+__device__ __forceinline__ double cs_reflect(double p, int S) {       // reflect_coordinates(p, 0, 2 (S - 1)), then clip
+  if (S <= 1) return 0.0;
+  const double span = (double)(S - 1);
+  p = fabs(p);
+  const double extra = fmod(p, span);
+  const double r = ((long long)floor(p / span)) % 2 == 0 ? extra : span - extra;
+  return fmin(fmax(r, 0.0), span);
+}
+__device__ __forceinline__ int cs_bound(int i, int S, int padding) {   // an integer tap under the padding rule (-1: zero)
+  if (padding == AUG_CS_BORDER) return i < 0 ? 0 : (i > S - 1 ? S - 1 : i);
+  if (padding == AUG_CS_REFLECTION) {
+    if (S <= 1) return 0;
+    const int period = 2 * (S - 1);
+    int m = (i < 0 ? -i : i) % period;
+    return m > S - 1 ? period - m : m;
+  }
+  return i >= 0 && i < S ? i : -1;
+}
+__device__ __forceinline__ double cubic1(double x) { const double A = -0.75; return ((A + 2.0) * x - (A + 3.0)) * x * x + 1.0; }
+__device__ __forceinline__ double cubic2(double x) { const double A = -0.75; return ((A * x - 5.0 * A) * x + 8.0 * A) * x - 4.0 * A; }
+
+__device__ CsTaps cs_taps(const AugPlan& plan, float u, int flip, int o, int S) {
+  const double lin = S > 1 ? -1.0 + 2.0 * (double)o / (double)(S - 1) : -1.0;
+  double g = lin + ((double)u - 0.5) * 2.0 * ((double)plan.cs_shift / (double)(S - 1));
+  if (flip) g = -g;
+  if (plan.cs_circular) g = (g + 1.0) - floor(g + 1.0) - 1.0;        // python's (g + 1) % 1 - 1
+  double pos = (g + 1.0) / 2.0 * (double)(S - 1);                    // grid_sampler_unnormalize, align_corners = True
+  CsTaps t;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) { t.idx[k] = -1; t.w[k] = 0.f; }
+  if (plan.cs_mode == AUG_CS_BICUBIC) {
+    const double fl = floor(pos), f = pos - fl;
+    const double c[4] = {cubic2(f + 1.0), cubic1(f), cubic1(1.0 - f), cubic2(2.0 - f)};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { t.idx[k] = (short)cs_bound((int)fl - 1 + k, S, plan.cs_padding); t.w[k] = (float)c[k]; }
+    return t;
+  }
+  if (plan.cs_padding == AUG_CS_BORDER) pos = fmin(fmax(pos, 0.0), (double)(S - 1));
+  else if (plan.cs_padding == AUG_CS_REFLECTION) pos = cs_reflect(pos, S);
+  if (plan.cs_mode == AUG_CS_NEAREST) {
+    const double r = rint(pos);
+    t.idx[0] = (short)(r >= 0.0 && r < (double)S ? (int)r : -1); t.w[0] = 1.f;
+    return t;
+  }
+  const double fl = floor(pos), f = pos - fl;
+  const int i0 = (int)fl;
+  t.idx[0] = (short)(i0 >= 0 && i0 < S ? i0 : -1);           t.w[0] = (float)(1.0 - f);
+  t.idx[1] = (short)(i0 + 1 >= 0 && i0 + 1 < S ? i0 + 1 : -1); t.w[1] = (float)f;
+  return t;
 }
 
-// forward view: permutation steps, then (optionally) the continuous shift, then the colour affine
-__global__ void __launch_bounds__(256) aug_view_kernel(const float* __restrict__ x, float* __restrict__ out, int N, int C, int H, int W,
+// forward view: permutation steps, then (optionally) the continuous shift, then the colour affine.  blockIdx.y = image; with the
+// continuous shift the block first tabulates the taps of its image's rows and columns in shared memory ([H] then [W]).
+__global__ void __launch_bounds__(256) aug_view_kernel(const float* __restrict__ x, float* __restrict__ out, int C, int H, int W,
                                                        AugPlan plan, const AugDraws* __restrict__ draws) {
+  extern __shared__ CsTaps taps[];
   pdl_prologue();
-  const long long total = (long long)N * C * H * W;
+  const int n = blockIdx.y;
+  const long long per = (long long)C * H * W;
   const AugDraws& d = *draws;   // read through the pointer (uniform addresses: served by the L1 / constant path)
-  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+  if (plan.cs_enabled) {
+    for (int k = threadIdx.x; k < H + W; k += blockDim.x)
+      taps[k] = k < H ? cs_taps(plan, d.sy[n], d.fud[n], k, H) : cs_taps(plan, d.sx[n], d.flr[n], k - H, W);
+    __syncthreads();
+  }
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < per; e += (long long)gridDim.x * blockDim.x) {
     const int j = (int)(e % W);
-    long long t = e / W;
-    const int i = (int)(t % H); t /= H;
-    const int c = (int)(t % C);
-    const int n = (int)(t / C);
+    const long long t = e / W;
+    const int i = (int)(t % H);
+    const int c = (int)(t / H);
     const float* src = x + ((long long)n * C + c) * H * W;
     float v;
-    if (plan.cs_enabled) {   // the continuous shift is the outermost spatial step: sample the permuted image bilinearly
-      int y0, x0; float fy, fx;
-      cs_coord(plan, d.sy[n], i, H, y0, fy);
-      cs_coord(plan, d.sx[n], j, W, x0, fx);
+    if (plan.cs_enabled) {   // the continuous shift is the outermost spatial step: sample the permuted image
+      const CsTaps& ty = taps[i];
+      const CsTaps& tx = taps[H + j];
       v = 0.f;
 #pragma unroll
-      for (int a = 0; a < 2; ++a)
+      for (int a = 0; a < 4; ++a)
 #pragma unroll
-        for (int b = 0; b < 2; ++b) {
-          const int yy = y0 + a, xx = x0 + b;
-          const float w = (a ? fy : 1.f - fy) * (b ? fx : 1.f - fx);
-          if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
+        for (int b = 0; b < 4; ++b) {
+          const int yy = ty.idx[a], xx = tx.idx[b];
+          if (yy >= 0 && xx >= 0 && ty.w[a] != 0.f && tx.w[b] != 0.f) {
             int sy, sx;
             map_back(plan, d, H, W, yy, xx, sy, sx);
-            v = fmaf(w, src[(long long)sy * W + sx], v);
+            v = fmaf(ty.w[a] * tx.w[b], src[(long long)sy * W + sx], v);
           }
         }
     } else {
@@ -148,7 +205,7 @@ __global__ void __launch_bounds__(256) aug_view_kernel(const float* __restrict__
       v = src[(long long)sy * W + sx];
     }
     if (plan.cj_scale != nullptr) v = fmaf(v, plan.cj_scale[n * C + c], plan.cj_shift[n * C + c]);
-    out[e] = v;
+    out[(long long)n * per + e] = v;
   }
 }
 
@@ -174,29 +231,33 @@ __global__ void __launch_bounds__(256) aug_pull_perm_kernel(const float* __restr
 
 // pull-back through the continuous shift, separable and deterministic (no atomics): first along x, then along y.
 //   tmp[n, c, i, xx] = sum_j wx(j -> xx) g[n, c, i, j]          out[n, c, yy, xx] = sum_i wy(i -> yy) tmp[n, c, i, xx]
-// (every thread walks the output index of its axis in order; O(S) per element, S <= a few hundred)
-__global__ void __launch_bounds__(256) aug_pull_cs_kernel(const float* __restrict__ g, float* __restrict__ out, int N, int C, int H, int W,
+// wx(j -> xx) sums the taps of output j that land on xx (bicubic taps may fold onto one pixel).  blockIdx.y = image; the block
+// tabulates its image's taps of the axis with the same cs_taps as the view, so both see bitwise the same weights.  Every thread walks
+// the output index of its axis in order (O(S) per element; the warp reads one table entry at a time, a shared-memory broadcast).
+__global__ void __launch_bounds__(256) aug_pull_cs_kernel(const float* __restrict__ g, float* __restrict__ out, int C, int H, int W,
                                                           AugPlan plan, const AugDraws* __restrict__ draws, int axis) {
+  extern __shared__ CsTaps taps[];
   pdl_prologue();
-  const long long total = (long long)N * C * H * W;
-  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+  const int n = blockIdx.y;
+  const int S = axis == 0 ? W : H;
+  for (int k = threadIdx.x; k < S; k += blockDim.x)
+    taps[k] = axis == 0 ? cs_taps(plan, draws->sx[n], draws->flr[n], k, S) : cs_taps(plan, draws->sy[n], draws->fud[n], k, S);
+  __syncthreads();
+  const long long per = (long long)C * H * W;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < per; e += (long long)gridDim.x * blockDim.x) {
     const int xq = (int)(e % W);
-    long long t = e / W;
-    const int yq = (int)(t % H); t /= H;
-    const int n = (int)(t / C);
-    const float* plane = g + (e - ((long long)yq * W + xq));
-    const float u = axis == 0 ? draws->sx[n] : draws->sy[n];
-    const int S = axis == 0 ? W : H, q = axis == 0 ? xq : yq;
+    const int yq = (int)((e / W) % H);
+    const float* plane = g + (long long)n * per + (e - ((long long)yq * W + xq));
+    const int q = axis == 0 ? xq : yq;
     float acc = 0.f;
     for (int o = 0; o < S; ++o) {
-      int i0; float fr;
-      cs_coord(plan, u, o, S, i0, fr);
+      const CsTaps& t = taps[o];
       float w = 0.f;
-      if (i0 == q) w = 1.f - fr;
-      else if (i0 + 1 == q) w = fr;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) w += t.idx[k] == q ? t.w[k] : 0.f;
       if (w != 0.f) acc = fmaf(w, axis == 0 ? plane[(long long)yq * W + o] : plane[(long long)o * W + xq], acc);
     }
-    out[e] = acc;
+    out[(long long)n * per + e] = acc;
   }
 }
 
@@ -356,8 +417,14 @@ int launch_aug_draws(const AugPipeline& pipe, const Scalars* sc, AugDraws* draws
   BRE_CHECK_LAUNCH();
   return 0;
 }
+// the continuous-shift kernels run one grid row per image (blockIdx.y), about as many blocks in all as grid_for gives the batch
+inline dim3 grid_per_image(int N, long long per) {
+  const int bx = grid_for((long long)N * per) / N;
+  return dim3(bx < 1 ? 1 : bx, N);
+}
 int launch_aug_view(const float* x, float* out, int N, int C, int H, int W, const AugPlan& plan, const AugDraws* draws, cudaStream_t s) {
-  BRE_KLAUNCH(aug_view_kernel, grid_for((long long)N * C * H * W), 256, 0, s, x, out, N, C, H, W, plan, draws);
+  const size_t smem = plan.cs_enabled ? (size_t)(H + W) * sizeof(CsTaps) : 0;
+  BRE_KLAUNCH(aug_view_kernel, grid_per_image(N, (long long)C * H * W), 256, smem, s, x, out, C, H, W, plan, draws);
   BRE_CHECK_LAUNCH();
   return 0;
 }
@@ -366,8 +433,9 @@ int launch_aug_pull(float* g, float* tmp, float* gx, int N, int C, int H, int W,
   const int grid = grid_for((long long)N * C * H * W);
   const float* src = g;
   if (plan.cs_enabled) {
-    BRE_KLAUNCH(aug_pull_cs_kernel, grid, 256, 0, s, (const float*)g, tmp, N, C, H, W, plan, draws, 0);
-    BRE_KLAUNCH(aug_pull_cs_kernel, grid, 256, 0, s, (const float*)tmp, g, N, C, H, W, plan, draws, 1);
+    const dim3 gi = grid_per_image(N, (long long)C * H * W);
+    BRE_KLAUNCH(aug_pull_cs_kernel, gi, 256, (size_t)W * sizeof(CsTaps), s, (const float*)g, tmp, C, H, W, plan, draws, 0);
+    BRE_KLAUNCH(aug_pull_cs_kernel, gi, 256, (size_t)H * sizeof(CsTaps), s, (const float*)tmp, g, C, H, W, plan, draws, 1);
   }
   BRE_KLAUNCH(aug_pull_perm_kernel, grid, 256, 0, s, src, gx, N, C, H, W, plan, draws);
   BRE_CHECK_LAUNCH();
@@ -398,14 +466,24 @@ using namespace bre;
 
 // ---- stand-alone entry points with explicit draws (parity tests against the reference modules) -----------------------------------
 static int fill_plan(AugPlan* plan, AugDraws* d, int32_t n_steps, const int32_t* kinds, const int32_t* o1, const int32_t* o2, float cs_shift,
-                     int32_t cs_circular, const float* sx, const float* sy, int32_t N, const float* cj_scale, const float* cj_shift) {
+                     int32_t cs_circular, int32_t cs_mode, int32_t cs_padding, const float* sx, const float* sy, const int32_t* flr,
+                     const int32_t* fud, int32_t N, int32_t H, int32_t W, const float* cj_scale, const float* cj_shift) {
   if (n_steps < 0 || n_steps > AUG_MAX_STEPS || N > AUG_MAX_BATCH) { set_error("bre_augment: too many steps / images"); return BRE_ERR_INVALID; }
+  if (cs_mode < AUG_CS_BILINEAR || cs_mode > AUG_CS_BICUBIC || cs_padding < AUG_CS_ZEROS || cs_padding > AUG_CS_REFLECTION ||
+      (cs_circular && cs_padding != AUG_CS_ZEROS)) {
+    set_error("bre_augment: unknown continuous_shift mode / padding (circular wraps the grid and pads with zeros)"); return BRE_ERR_INVALID;
+  }
+  if (sx != nullptr && (H > AUG_CS_MAX_SIDE || W > AUG_CS_MAX_SIDE)) { set_error("bre_augment: continuous_shift on a side over 1024"); return BRE_ERR_UNSUPPORTED; }
   memset(plan, 0, sizeof(*plan));
   memset(d, 0, sizeof(*d));
   plan->n_steps = n_steps;
   for (int s = 0; s < n_steps; ++s) { plan->kind[s] = kinds[s]; d->o1[s] = o1[s]; d->o2[s] = o2 ? o2[s] : 0; }
   plan->cs_enabled = sx != nullptr; plan->cs_shift = cs_shift; plan->cs_circular = cs_circular;
-  for (int n = 0; n < N && sx != nullptr; ++n) { d->sx[n] = sx[n]; d->sy[n] = sy[n]; }
+  plan->cs_mode = cs_mode; plan->cs_padding = cs_padding;
+  for (int n = 0; n < N && sx != nullptr; ++n) {
+    d->sx[n] = sx[n]; d->sy[n] = sy[n];
+    d->flr[n] = flr != nullptr && flr[n] != 0; d->fud[n] = fud != nullptr && fud[n] != 0;
+  }
   plan->cj_scale = cj_scale; plan->cj_shift = cj_shift;
   return 0;
 }
@@ -413,9 +491,19 @@ static int fill_plan(AugPlan* plan, AugDraws* d, int32_t n_steps, const int32_t*
 extern "C" int bre_augment_view(const float* x, float* out, int32_t N, int32_t C, int32_t H, int32_t W, int32_t n_steps, const int32_t* kinds,
                                 const int32_t* o1, const int32_t* o2, float cs_shift, int32_t cs_circular, const float* sx, const float* sy,
                                 const float* cj_scale, const float* cj_shift, int32_t transpose, float* scratch, void* stream) {
-  if (!x || !out || N <= 0 || C <= 0 || H <= 0 || W <= 0) { set_error("bre_augment_view: bad arguments"); return BRE_ERR_INVALID; }
+  return bre_augment_view_ex(x, out, N, C, H, W, n_steps, kinds, o1, o2, cs_shift, cs_circular, BRE_CS_BILINEAR, BRE_CS_ZEROS, sx, sy, nullptr,
+                             nullptr, cj_scale, cj_shift, transpose, scratch, stream);
+}
+
+extern "C" int bre_augment_view_ex(const float* x, float* out, int32_t N, int32_t C, int32_t H, int32_t W, int32_t n_steps, const int32_t* kinds,
+                                   const int32_t* o1, const int32_t* o2, float cs_shift, int32_t cs_circular, int32_t cs_mode, int32_t cs_padding,
+                                   const float* sx, const float* sy, const int32_t* fliplr, const int32_t* flipud, const float* cj_scale,
+                                   const float* cj_shift, int32_t transpose, float* scratch, void* stream) {
+  if (!x || !out || N <= 0 || C <= 0 || H <= 0 || W <= 0 || (sx != nullptr) != (sy != nullptr)) { set_error("bre_augment_view: bad arguments"); return BRE_ERR_INVALID; }
   AugPlan plan; AugDraws host;
-  { const int frc = fill_plan(&plan, &host, n_steps, kinds, o1, o2, cs_shift, cs_circular, sx, sy, N, cj_scale, cj_shift); if (frc != 0) return frc; }
+  const int frc = fill_plan(&plan, &host, n_steps, kinds, o1, o2, cs_shift, cs_circular, cs_mode, cs_padding, sx, sy, fliplr, flipud, N, H, W,
+                            cj_scale, cj_shift);
+  if (frc != 0) return frc;
   cudaStream_t s = (cudaStream_t)stream;
   AugDraws* dev = nullptr;
   BRE_CUDA_CHECK(cudaMallocAsync((void**)&dev, sizeof(AugDraws), s));

@@ -7,7 +7,11 @@ namespace bre {
 constexpr int AUG_MAX_STEPS = 4;     // permutation steps (discrete_shift / flip) in config order
 constexpr int AUG_MAX_BATCH = 64;    // per-image uniforms of the continuous shift
 constexpr int AUG_MAX_STAGES = 8;    // stages of the view pipeline (see AugStage)
+constexpr int AUG_CS_MAX_SIDE = 1024; // continuous_shift: the per-image tap tables of both axes fit 48 KB of shared memory
 enum AugKind { AUG_SHIFT = 1, AUG_FLIP = 2 };
+// continuous_shift sampling (grid_sample mode / padding_mode; "circular" is a zeros-padded wrap of the grid, cs_circular)
+enum AugCsMode { AUG_CS_BILINEAR = 0, AUG_CS_NEAREST = 1, AUG_CS_BICUBIC = 2 };
+enum AugCsPadding { AUG_CS_ZEROS = 0, AUG_CS_BORDER = 1, AUG_CS_REFLECTION = 2 };
 // A stage of the view pipeline.  PIXEL: a maximal run of the shape-keeping kinds (discrete_shift, flip, continuous_shift,
 // colorjitter) on the fused kernels below, described by its AugPlan.  RESAMPLE: a window of the input resized bilinearly
 // (zoom, centerzoom, focus).  BLUR: the binomial depthwise convolution of antialias.
@@ -22,10 +26,13 @@ struct AugPlan {
   const float* cj_scale;             // colour affine per (n, c): out = in * scale + shift (composite of all colorjitter steps), may be null
   const float* cj_shift;
   unsigned long long seed;
+  int cs_mode, cs_padding;           // AugCsMode, AugCsPadding
+  int cs_fliplr, cs_flipud;          // grid flips: each image negates its x (y) coordinate when its third (fourth) uniform is > 0.5
 };
 struct AugDraws {
   int o1[AUG_MAX_STEPS], o2[AUG_MAX_STEPS];   // discrete_shift: the two roll offsets ; flip: o1 = flipped? ; focus: o1[0], o2[0] = window corner
   float sx[AUG_MAX_BATCH], sy[AUG_MAX_BATCH]; // continuous_shift: uniforms in [0, 1) per image (randgen[:, 0], randgen[:, 1])
+  int flr[AUG_MAX_BATCH], fud[AUG_MAX_BATCH]; // continuous_shift: 1 = this image's grid is flipped left-right / up-down
 };
 struct AugStage {
   int kind;                          // AugStageKind

@@ -1797,7 +1797,7 @@ static int set_candidate_shape(bre_engine* e, int N, int C, int H, int W) {
 }
 
 // the ordered stage list -> e->aug_pipe; candidate shape [N, C, H, W]; n_stages = 0 switches augmentations off
-static int set_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage* stages, int32_t N, int32_t C, int32_t H, int32_t W,
+static int set_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage_ex* stages, int32_t N, int32_t C, int32_t H, int32_t W,
                       int32_t differentiable, uint64_t seed) {
   if (n_stages < 0 || n_stages > AUG_MAX_STAGES || (n_stages > 0 && !stages)) { set_error("augmentations: at most 8 stages"); return BRE_ERR_INVALID; }
   if (e->ms_steps > 0) { set_error("augmentations are not supported together with local steps"); return BRE_ERR_UNSUPPORTED; }
@@ -1813,7 +1813,8 @@ static int set_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage* stag
   int h = H, w = W, pixel_runs = 0;
   long long widest = (long long)N * C * H * W;
   for (int k = 0; k < n_stages; ++k) {
-    const bre_aug_stage& in = stages[k];
+    const bre_aug_stage& in = stages[k].stage;
+    const bre_aug_stage_ex& ex = stages[k];
     AugStage& st = pipe.st[k];
     st.kind = in.kind; st.C = C; st.Hi = h; st.Wi = w; st.Ho = h; st.Wo = w;
     if (in.kind == BRE_AUG_PIXEL) {
@@ -1827,6 +1828,12 @@ static int set_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage* stag
       plan.seed = pixel_runs == 0 ? seed : seed ^ (0x9E3779B97F4A7C15ull * (unsigned long long)pixel_runs);   // the first run: the plain plan's keys
       ++pixel_runs;
       if (in.cs_enabled && h != w) { set_error("continuous_shift needs square images (the reference builds an S x S grid from shape[2])"); return BRE_ERR_UNSUPPORTED; }
+      if (ex.cs_mode < AUG_CS_BILINEAR || ex.cs_mode > AUG_CS_BICUBIC || ex.cs_padding < AUG_CS_ZEROS || ex.cs_padding > AUG_CS_REFLECTION ||
+          (in.cs_circular && ex.cs_padding != AUG_CS_ZEROS)) {
+        set_error("augmentations: unknown continuous_shift mode / padding (circular wraps the grid and pads with zeros)"); return BRE_ERR_INVALID;
+      }
+      if (in.cs_enabled && h > AUG_CS_MAX_SIDE) { set_error("continuous_shift: images up to 1024 x 1024"); return BRE_ERR_UNSUPPORTED; }
+      plan.cs_mode = ex.cs_mode; plan.cs_padding = ex.cs_padding; plan.cs_fliplr = ex.cs_fliplr != 0; plan.cs_flipud = ex.cs_flipud != 0;
       if ((in.cj_scale != nullptr) != (in.cj_shift != nullptr)) { set_error("colour scale and shift go together"); return BRE_ERR_INVALID; }
     } else if (in.kind == BRE_AUG_RESAMPLE) {
       if (in.Ho <= 0 || in.Wo <= 0 || in.wh <= 0 || in.ww <= 0 || in.wh > h || in.ww > w || (!in.focus && (in.y0 < 0 || in.x0 < 0 || in.y0 + in.wh > h || in.x0 + in.ww > w))) {
@@ -1866,11 +1873,12 @@ static int set_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage* stag
       BRE_TRY(e->alloc(&e->cj, 2LL * AUG_MAX_STAGES * AUG_MAX_BATCH * C));
     }
     for (int k = 0; k < n_stages; ++k) {
-      if (stages[k].kind != BRE_AUG_PIXEL || stages[k].cj_scale == nullptr) continue;
+      const bre_aug_stage& in = stages[k].stage;
+      if (in.kind != BRE_AUG_PIXEL || in.cj_scale == nullptr) continue;
       float* sc_dev = e->cj + 2LL * k * AUG_MAX_BATCH * C;
       float* sh_dev = sc_dev + (long long)AUG_MAX_BATCH * C;
-      BRE_CUDA_CHECK(cudaMemcpyAsync(sc_dev, stages[k].cj_scale, (size_t)N * C * sizeof(float), cudaMemcpyDefault, e->stream));
-      BRE_CUDA_CHECK(cudaMemcpyAsync(sh_dev, stages[k].cj_shift, (size_t)N * C * sizeof(float), cudaMemcpyDefault, e->stream));
+      BRE_CUDA_CHECK(cudaMemcpyAsync(sc_dev, in.cj_scale, (size_t)N * C * sizeof(float), cudaMemcpyDefault, e->stream));
+      BRE_CUDA_CHECK(cudaMemcpyAsync(sh_dev, in.cj_shift, (size_t)N * C * sizeof(float), cudaMemcpyDefault, e->stream));
       pipe.plan[k].cj_scale = sc_dev; pipe.plan[k].cj_shift = sh_dev;
     }
     BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
@@ -1882,21 +1890,40 @@ static int set_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage* stag
 
 int bre_engine_set_augmentations(bre_engine* e, int32_t n_steps, const int32_t* kinds, const float* params, int32_t cs_enabled, float cs_shift,
                                  int32_t cs_circular, const float* cj_scale, const float* cj_shift, int32_t differentiable, uint64_t seed) {
+  return bre_engine_set_augmentations_ex(e, n_steps, kinds, params, cs_enabled, cs_shift, cs_circular, BRE_CS_BILINEAR, BRE_CS_ZEROS, 0, 0, cj_scale,
+                                         cj_shift, differentiable, seed);
+}
+
+int bre_engine_set_augmentations_ex(bre_engine* e, int32_t n_steps, const int32_t* kinds, const float* params, int32_t cs_enabled, float cs_shift,
+                                    int32_t cs_circular, int32_t cs_mode, int32_t cs_padding, int32_t cs_fliplr, int32_t cs_flipud,
+                                    const float* cj_scale, const float* cj_shift, int32_t differentiable, uint64_t seed) {
   if (!e || n_steps < 0 || n_steps > AUG_MAX_STEPS || (n_steps > 0 && (!kinds || !params))) { set_error("bre_engine_set_augmentations: bad arguments"); return BRE_ERR_INVALID; }
   if (e->ms_steps > 0) { set_error("augmentations are not supported together with local steps"); return BRE_ERR_UNSUPPORTED; }
   const bool any = n_steps > 0 || cs_enabled || cj_scale != nullptr;
-  bre_aug_stage st;            // one PIXEL stage at the program's shape
+  bre_aug_stage_ex st;         // one PIXEL stage at the program's shape
   memset(&st, 0, sizeof(st));
-  st.kind = BRE_AUG_PIXEL; st.n_steps = n_steps;
-  for (int s = 0; s < n_steps; ++s) { st.kinds[s] = kinds[s]; st.params[s] = params[s]; }
-  st.cs_enabled = cs_enabled; st.cs_shift = cs_shift; st.cs_circular = cs_circular;
-  st.cj_scale = cj_scale; st.cj_shift = cj_shift;
+  st.stage.kind = BRE_AUG_PIXEL; st.stage.n_steps = n_steps;
+  for (int s = 0; s < n_steps; ++s) { st.stage.kinds[s] = kinds[s]; st.stage.params[s] = params[s]; }
+  st.stage.cs_enabled = cs_enabled; st.stage.cs_shift = cs_shift; st.stage.cs_circular = cs_circular;
+  st.stage.cj_scale = cj_scale; st.stage.cj_shift = cj_shift;
+  st.cs_mode = cs_mode; st.cs_padding = cs_padding; st.cs_fliplr = cs_fliplr; st.cs_flipud = cs_flipud;
   const bre_tensor_desc& v = e->td(0);
   return set_stages(e, any ? 1 : 0, &st, v.N, v.C, v.H, v.W, differentiable, seed);
 }
 
 int bre_engine_set_augmentation_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage* stages, int32_t N, int32_t C, int32_t H, int32_t W,
                                        int32_t differentiable, uint64_t seed) {
+  if (!e) { set_error("bre_engine_set_augmentation_stages: bad arguments"); return BRE_ERR_INVALID; }
+  if (!e->model_loaded) { set_error("load the model first"); return BRE_ERR_STATE; }
+  if (n_stages < 0 || n_stages > AUG_MAX_STAGES || (n_stages > 0 && !stages)) { set_error("augmentations: at most 8 stages"); return BRE_ERR_INVALID; }
+  bre_aug_stage_ex ex[AUG_MAX_STAGES];   // the same stages without the continuous_shift options
+  memset(ex, 0, sizeof(ex));
+  for (int k = 0; k < n_stages; ++k) ex[k].stage = stages[k];
+  return bre_engine_set_augmentation_stages_ex(e, n_stages, ex, N, C, H, W, differentiable, seed);
+}
+
+int bre_engine_set_augmentation_stages_ex(bre_engine* e, int32_t n_stages, const bre_aug_stage_ex* stages, int32_t N, int32_t C, int32_t H,
+                                          int32_t W, int32_t differentiable, uint64_t seed) {
   if (!e) { set_error("bre_engine_set_augmentation_stages: bad arguments"); return BRE_ERR_INVALID; }
   if (!e->model_loaded) { set_error("load the model first"); return BRE_ERR_STATE; }
   return set_stages(e, n_stages, stages, N, C, H, W, differentiable, seed);
@@ -1929,6 +1956,16 @@ int bre_engine_augmentation_draws(bre_engine* e, int32_t* n_stages, int32_t* o1,
     for (int s = 0; s < AUG_MAX_STEPS; ++s) { if (o1) o1[k * AUG_MAX_STEPS + s] = h[k].o1[s]; if (o2) o2[k * AUG_MAX_STEPS + s] = h[k].o2[s]; }
     for (int n = 0; n < AUG_MAX_BATCH; ++n) { if (sx) sx[k * AUG_MAX_BATCH + n] = h[k].sx[n]; if (sy) sy[k * AUG_MAX_BATCH + n] = h[k].sy[n]; }
   }
+  return BRE_OK;
+}
+
+int bre_engine_augmentation_flips(bre_engine* e, int32_t* n_stages, int32_t* fliplr, int32_t* flipud) {
+  if (!e || !e->aug_draws) { set_error("bre_engine_augmentation_flips: no augmentations configured"); return BRE_ERR_STATE; }
+  AugDraws h[AUG_MAX_STAGES];
+  BRE_TRY(read_draws(e, h));
+  if (n_stages) *n_stages = e->aug_pipe.n_stages;
+  for (int k = 0; k < AUG_MAX_STAGES; ++k)
+    for (int n = 0; n < AUG_MAX_BATCH; ++n) { if (fliplr) fliplr[k * AUG_MAX_BATCH + n] = h[k].flr[n]; if (flipud) flipud[k * AUG_MAX_BATCH + n] = h[k].fud[n]; }
   return BRE_OK;
 }
 

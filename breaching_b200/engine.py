@@ -42,6 +42,10 @@ class AugStage(ctypes.Structure):   # bre_aug_stage
                [("focus_std", ctypes.c_float), ("width", ctypes.c_int32), ("stride", ctypes.c_int32)]
 
 
+class AugStageEx(ctypes.Structure):   # bre_aug_stage_ex
+    _fields_ = [("stage", AugStage)] + [(n, ctypes.c_int32) for n in ("cs_mode", "cs_padding", "cs_fliplr", "cs_flipud")]
+
+
 class StepScalars(ctypes.Structure):   # bre_step_scalars
     _fields_ = [(n, ctypes.c_double) for n in ("match", "task_loss", "tv", "norm", "di", "feat", "fmin")] + \
                [(n, ctypes.c_int32) for n in ("it", "recorded", "stopped", "trial")] + \
@@ -100,6 +104,7 @@ EXPORTS = [
     "bre_engine_begin_joint_trial", "bre_engine_get_joint_labels", "bre_resize_bilinear",
     "bre_engine_set_augmentations", "bre_engine_last_augmentation", "bre_augment_view",
     "bre_engine_set_augmentation_stages", "bre_engine_augmentation_draws", "bre_augment_resample", "bre_augment_blur",
+    "bre_engine_set_augmentations_ex", "bre_engine_set_augmentation_stages_ex", "bre_augment_view_ex", "bre_engine_augmentation_flips",
     "bre_engine_set_trial_index", "bre_engine_debug_step_state", "bre_optimizer_step", "bre_langevin_noise",
     "bre_debug_last_gemm_plan", "bre_debug_row_plan", "bre_row_op",
 ]
@@ -164,6 +169,11 @@ def load_library(path=None):
     lib.bre_engine_set_augmentation_stages.argtypes = [vp, i32, P(AugStage), i32, i32, i32, i32, i32, ctypes.c_uint64]
     lib.bre_engine_augmentation_draws.argtypes = [vp, P(i32), P(i32), P(i32), P(f32), P(f32)]
     lib.bre_augment_resample.argtypes = [vp, vp] + [i32] * 11 + [vp]
+    lib.bre_engine_set_augmentations_ex.argtypes = [vp, i32, P(i32), P(f32), i32, f32, i32, i32, i32, i32, i32, vp, vp, i32, ctypes.c_uint64]
+    lib.bre_engine_set_augmentation_stages_ex.argtypes = [vp, i32, P(AugStageEx), i32, i32, i32, i32, i32, ctypes.c_uint64]
+    lib.bre_augment_view_ex.argtypes = [vp, vp, i32, i32, i32, i32, i32, P(i32), P(i32), P(i32), f32, i32, i32, i32, P(f32), P(f32), P(i32), P(i32),
+                                        vp, vp, i32, vp, vp]
+    lib.bre_engine_augmentation_flips.argtypes = [vp, P(i32), P(i32), P(i32)]
     lib.bre_augment_blur.argtypes = [vp, vp] + [i32] * 7 + [vp]
     lib.bre_resize_bilinear.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, vp]
     lib.bre_image_mse.argtypes = [vp, vp, i32, i32, i32, vp, vp, i32, P(ctypes.c_double), vp]
@@ -428,6 +438,8 @@ class Engine:
         candidate then has the plan's candidate shape and ``input_shape`` / ``numel`` follow it."""
         if plan is not None and plan.stages:
             return self._set_augmentation_stages(plan)
+        from .attacks import augment as A
+
         if plan is None:
             _check(self.lib, self.lib.bre_engine_set_augmentations(self.h, 0, None, None, 0, 0.0, 0, None, None, 0, 0), "bre_engine_set_augmentations")
             self._candidate_shape(None)
@@ -439,10 +451,11 @@ class Engine:
         shift = None if plan.colour_shift is None else _f32c(plan.colour_shift, self.device)
         torch.cuda.synchronize(self.device)
         self._aug_keep = (scale, shift)
-        _check(self.lib, self.lib.bre_engine_set_augmentations(self.h, n, kinds, params, int(plan.continuous_shift is not None),
-                                                               float(plan.continuous_shift or 0.0), int(plan.circular), _ptr(scale), _ptr(shift),
-                                                               int(plan.differentiable), int(plan.seed) & 0xFFFFFFFFFFFFFFFF),
-               "bre_engine_set_augmentations")
+        _check(self.lib, self.lib.bre_engine_set_augmentations_ex(self.h, n, kinds, params, int(plan.continuous_shift is not None),
+                                                                  float(plan.continuous_shift or 0.0), int(plan.circular), A.CS_MODES[plan.cs_mode],
+                                                                  A.CS_PADDINGS[plan.cs_padding], int(plan.fliplr), int(plan.flipud), _ptr(scale),
+                                                                  _ptr(shift), int(plan.differentiable), int(plan.seed) & 0xFFFFFFFFFFFFFFFF),
+               "bre_engine_set_augmentations_ex")
         self._candidate_shape(None)
 
     def _candidate_shape(self, shape):
@@ -459,11 +472,14 @@ class Engine:
     def _set_augmentation_stages(self, plan):
         from .attacks import augment as A
 
-        arr = (AugStage * len(plan.stages))()
+        arr = (AugStageEx * len(plan.stages))()
         keep = []
-        for st, cs in zip(plan.stages, arr):
+        for st, ex in zip(plan.stages, arr):
+            cs = ex.stage
             cs.Ho, cs.Wo = st.out_hw
             if st.kind == A.PIXEL:
+                ex.cs_mode, ex.cs_padding = A.CS_MODES[st.cs_mode], A.CS_PADDINGS[st.cs_padding]
+                ex.cs_fliplr, ex.cs_flipud = int(st.fliplr), int(st.flipud)
                 cs.kind, cs.n_steps = 0, len(st.steps)
                 for i, (k, p) in enumerate(st.steps):
                     cs.kinds[i], cs.params[i] = int(k), float(p)
@@ -481,8 +497,8 @@ class Engine:
         torch.cuda.synchronize(self.device)
         self._aug_keep = tuple(keep)
         N, Cc, H, W = plan.candidate_shape
-        _check(self.lib, self.lib.bre_engine_set_augmentation_stages(self.h, len(plan.stages), arr, N, Cc, H, W, int(plan.differentiable),
-                                                                     int(plan.seed) & 0xFFFFFFFFFFFFFFFF), "bre_engine_set_augmentation_stages")
+        _check(self.lib, self.lib.bre_engine_set_augmentation_stages_ex(self.h, len(plan.stages), arr, N, Cc, H, W, int(plan.differentiable),
+                                                                        int(plan.seed) & 0xFFFFFFFFFFFFFFFF), "bre_engine_set_augmentation_stages_ex")
         self._candidate_shape(plan.candidate_shape)
 
     def last_augmentation(self):
@@ -502,6 +518,14 @@ class Engine:
         n = self.input_shape[0]
         return [dict(o1=list(o1[4 * k:4 * k + 4]), o2=list(o2[4 * k:4 * k + 4]), sx=list(sx[64 * k:64 * k + n]), sy=list(sy[64 * k:64 * k + n]))
                 for k in range(n_st.value)]
+
+    def augmentation_flips(self):
+        """The continuous shift's grid flips of the last evaluation, per stage: list of dicts (fliplr, flipud: 0 / 1 per image)."""
+        n_st = ctypes.c_int32()
+        lr, ud = (ctypes.c_int32 * 512)(), (ctypes.c_int32 * 512)()
+        _check(self.lib, self.lib.bre_engine_augmentation_flips(self.h, ctypes.byref(n_st), lr, ud), "bre_engine_augmentation_flips")
+        n = self.input_shape[0]
+        return [dict(fliplr=list(lr[64 * k:64 * k + n]), flipud=list(ud[64 * k:64 * k + n])) for k in range(n_st.value)]
 
     def run(self, n_iters):
         _check(self.lib, self.lib.bre_engine_run(self.h, int(n_iters)), "bre_engine_run")
@@ -725,9 +749,15 @@ def total_variation(x, scale=0.1, inner_exp=1.0, outer_exp=1.0, eps=1e-8, double
 
 
 def augment_view(x, steps=(), offsets=(), continuous_shift=None, circular=True, uniforms=None, colour_scale=None, colour_shift=None,
-                 transpose=False):
+                 transpose=False, mode="bilinear", padding="zeros", flips=None):
     """Stand-alone augmentation view (or its transpose) with explicit draws: ``steps`` = [(kind, param)], ``offsets`` = [(o1, o2)] per
-    step (roll offsets; flip: (flag, 0)), ``uniforms`` = (sx, sy) lists per image for the continuous shift."""
+    step (roll offsets; flip: (flag, 0)), ``uniforms`` = (sx, sy) lists per image for the continuous shift, sampled with grid_sample's
+    ``mode`` and ``padding`` (zeros / border / reflection; ``circular`` wraps the grid first and needs zeros); ``flips`` = (fliplr,
+    flipud) lists of 0 / 1 per image: that image's x / y grid coordinate is negated."""
+    from .attacks.augment import CS_MODES, CS_PADDINGS
+
+    if mode not in CS_MODES or padding not in CS_PADDINGS:
+        raise ValueError(f"continuous_shift: unknown mode {mode!r} or padding {padding!r}")
     lib = load_library()
     x = _f32c(x).clone()
     N, C, H, W = x.shape
@@ -736,17 +766,20 @@ def augment_view(x, steps=(), offsets=(), continuous_shift=None, circular=True, 
     kinds = (ctypes.c_int32 * max(n, 1))(*[k for k, _ in steps])
     o1 = (ctypes.c_int32 * max(n, 1))(*[int(a) for a, _ in offsets])
     o2 = (ctypes.c_int32 * max(n, 1))(*[int(b) for _, b in offsets])
-    sx = sy = None
+    sx = sy = lr = ud = None
     if continuous_shift is not None:
         sx, sy = (ctypes.c_float * N)(*[float(v) for v in uniforms[0]]), (ctypes.c_float * N)(*[float(v) for v in uniforms[1]])
+        if flips is not None:
+            lr, ud = (ctypes.c_int32 * N)(*[int(v) for v in flips[0]]), (ctypes.c_int32 * N)(*[int(v) for v in flips[1]])
     scratch = torch.empty_like(x)
     cs, csh = (None if colour_scale is None else _f32c(colour_scale, x.device)), (None if colour_shift is None else _f32c(colour_shift, x.device))
     stream = torch.cuda.current_stream(x.device).cuda_stream
     with torch.cuda.device(x.device):
         torch.cuda.synchronize(x.device)
-        rc = lib.bre_augment_view(_ptr(x), _ptr(out), N, C, H, W, n, kinds, o1, o2, float(continuous_shift or 0.0), int(circular), sx, sy, _ptr(cs),
-                                  _ptr(csh), int(transpose), _ptr(scratch), ctypes.c_void_p(stream))
-    _check(lib, rc, "bre_augment_view")
+        rc = lib.bre_augment_view_ex(_ptr(x), _ptr(out), N, C, H, W, n, kinds, o1, o2, float(continuous_shift or 0.0), int(circular),
+                                     CS_MODES[mode], CS_PADDINGS[padding], sx, sy, lr, ud, _ptr(cs), _ptr(csh), int(transpose), _ptr(scratch),
+                                     ctypes.c_void_p(stream))
+    _check(lib, rc, "bre_augment_view_ex")
     return out
 
 

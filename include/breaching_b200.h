@@ -245,6 +245,19 @@ int bre_engine_last_augmentation(bre_engine* e, int32_t* o1, int32_t* o2, float*
 int bre_augment_view(const float* x, float* out, int32_t N, int32_t C, int32_t H, int32_t W, int32_t n_steps, const int32_t* kinds,
                      const int32_t* o1, const int32_t* o2, float cs_shift, int32_t cs_circular, const float* sx, const float* sy,
                      const float* cj_scale, const float* cj_shift, int32_t transpose, float* scratch, void* stream);
+/* continuous_shift with every option of the reference's RandomTransform (the entry points above sample bilinearly with zeros
+ * padding, or "circular" = cs_circular, without grid flips): grid_sample mode cs_mode and padding_mode cs_padding (cs_circular
+ * needs BRE_CS_ZEROS), and per-image grid flips: fliplr[n] / flipud[n] != 0 negates image n's x / y coordinate (NULL = none).
+ * Sides up to 1024. */
+enum { BRE_CS_BILINEAR = 0, BRE_CS_NEAREST = 1, BRE_CS_BICUBIC = 2 };
+enum { BRE_CS_ZEROS = 0, BRE_CS_BORDER = 1, BRE_CS_REFLECTION = 2 };
+int bre_engine_set_augmentations_ex(bre_engine* e, int32_t n_steps, const int32_t* kinds, const float* params, int32_t cs_enabled,
+                                    float cs_shift, int32_t cs_circular, int32_t cs_mode, int32_t cs_padding, int32_t cs_fliplr,
+                                    int32_t cs_flipud, const float* cj_scale, const float* cj_shift, int32_t differentiable, uint64_t seed);
+int bre_augment_view_ex(const float* x, float* out, int32_t N, int32_t C, int32_t H, int32_t W, int32_t n_steps, const int32_t* kinds,
+                        const int32_t* o1, const int32_t* o2, float cs_shift, int32_t cs_circular, int32_t cs_mode, int32_t cs_padding,
+                        const float* sx, const float* sy, const int32_t* fliplr, const int32_t* flipud, const float* cj_scale,
+                        const float* cj_shift, int32_t transpose, float* scratch, void* stream);
 
 /* The view as an ordered list of up to 8 stages, each with its own input and output shape (augment.cu):
  *   BRE_AUG_PIXEL     a run of the shape-keeping kinds with the parameters of bre_engine_set_augmentations (n_steps, kinds,
@@ -271,9 +284,20 @@ typedef struct bre_aug_stage {
 } bre_aug_stage;
 int bre_engine_set_augmentation_stages(bre_engine* e, int32_t n_stages, const bre_aug_stage* stages, int32_t N, int32_t C, int32_t H,
                                        int32_t W, int32_t differentiable, uint64_t seed);
+/* The same with the continuous_shift options of bre_engine_set_augmentations_ex per PIXEL stage (cs_fliplr / cs_flipud != 0: each
+ * image's grid is flipped when its third / fourth uniform is > 0.5). */
+typedef struct bre_aug_stage_ex {
+  bre_aug_stage stage;
+  int32_t cs_mode, cs_padding, cs_fliplr, cs_flipud;
+} bre_aug_stage_ex;
+int bre_engine_set_augmentation_stages_ex(bre_engine* e, int32_t n_stages, const bre_aug_stage_ex* stages, int32_t N, int32_t C, int32_t H,
+                                          int32_t W, int32_t differentiable, uint64_t seed);
 /* All draws of the last evaluation, per stage k (8 x 4 offsets, 8 x 64 uniforms): PIXEL stages as bre_engine_last_augmentation,
  * focus stages their window corner (o1[4 k], o2[4 k]) = (row, column). */
 int bre_engine_augmentation_draws(bre_engine* e, int32_t* n_stages, int32_t* o1, int32_t* o2, float* sx, float* sy);
+/* The grid flips of the last evaluation, per stage k and image n (8 x 64): fliplr[64 k + n], flipud[64 k + n] = 1 when image n's grid
+ * was flipped (0 for stages without flips). */
+int bre_engine_augmentation_flips(bre_engine* e, int32_t* n_stages, int32_t* fliplr, int32_t* flipud);
 /* Stand-alone RESAMPLE / BLUR stage with an explicit window: transpose = 0 maps x [N, C, Hi, Wi] to the view, transpose = 1 pulls
  * x = the gradient at the view back to out [N, C, Hi, Wi] (fixed-order gathers, bitwise reproducible). */
 int bre_augment_resample(const float* x, float* out, int32_t N, int32_t C, int32_t Hi, int32_t Wi, int32_t y0, int32_t x0, int32_t wh,

@@ -2,7 +2,9 @@
 
   (a) a 224 x 224 candidate without augmentations,
   (b) a 112 x 112 candidate with ``zoom: {out_size: 224}`` (the model runs at 224; RESAMPLE view and pull-back),
-  (c) a 224 x 224 candidate with ``antialias: {width: 5}`` (BLUR view and pull-back).
+  (c) a 224 x 224 candidate with ``antialias: {width: 5}`` (BLUR view and pull-back),
+  (d) - (g) a 224 x 224 candidate with ``continuous_shift: {shift: 8}`` sampled bilinearly with the module's default reflection padding,
+      bicubically with reflection padding, nearest with reflection padding, and bilinearly with the circular wrap of multiscale_ghiasi.
 
 Each arm is one engine with its captured CUDA graph; after a warm-up (capture included) the arms are timed in turn, ``--repeats``
 rounds of ``--steps`` iterations each, with CUDA events on the engine's stream around the graph launches (``Engine.run_timed``).
@@ -29,6 +31,10 @@ ARMS = {   # name: (candidate size, augmentations)
     "a_224_plain": (224, None),
     "b_112_zoom_224": (112, {"zoom": {"out_size": 224}}),
     "c_224_antialias5": (224, {"antialias": {"width": 5}}),
+    "d_224_cshift_reflection_bilinear": (224, {"continuous_shift": {"shift": 8}}),
+    "e_224_cshift_reflection_bicubic": (224, {"continuous_shift": {"shift": 8, "mode": "bicubic"}}),
+    "f_224_cshift_reflection_nearest": (224, {"continuous_shift": {"shift": 8, "mode": "nearest"}}),
+    "g_224_cshift_circular_bilinear": (224, {"continuous_shift": {"shift": 8, "padding": "circular"}}),
 }
 
 
