@@ -189,7 +189,7 @@ struct bre_engine {
     a.g = ConvGeom{to.N, to.H, to.W, stem_Kp, to.H, to.W, to.C, 1, 1, 1, 0};
     a.x_sN = (long long)to.H * to.W * stem_Kp; a.x_sP = stem_Kp; a.x_sC = 1;
     a.nsrc = 1;
-    a.ws = ws; a.counters = gemm_counters; a.ws_tiles = ws_tiles; a.splits = 0;
+    a.ws = ws; a.counters = gemm_counters; a.ws_tiles = ws_tiles;
     return a;
   }
   int stem_unfold(const bre_op_desc& op) {            // candidate -> xcol
@@ -392,7 +392,7 @@ struct bre_engine {
       else { a.x_sN = (long long)ti.H * ti.W * ti.C; a.x_sP = ti.C; a.x_sC = 1; }                         // NHWC internal
     }
     a.nsrc = 1;
-    a.ws = ws; a.counters = gemm_counters; a.ws_tiles = ws_tiles; a.splits = 0;
+    a.ws = ws; a.counters = gemm_counters; a.ws_tiles = ws_tiles;
     a.force_fp32 = is_precise(op_index(op)) ? 1 : 0;
     return a;
   }
@@ -415,14 +415,9 @@ struct bre_engine {
     return mask;
   }
   int gemm_on(const GemmArgs& a, cudaStream_t st) {
-    if (linear_tall_supported(a)) return launch_linear_tall(a, st);
-    if (linear_small_preferred(a)) return launch_linear_small(a, st);
-    if (gemm_backend == 1 && !a.force_fp32 && igemm_tc_supported(a)) {
-      GemmArgs b = a;
-      b.wgt_static = static_weights(a);
-      return launch_igemm_tc(b, st);
-    }
-    return launch_igemm_simt(a, st);
+    GemmArgs b = a;
+    b.wgt_static = static_weights(a);
+    return launch_gemm(b, gemm_backend == 1 && !a.force_fp32 ? 2 : 0, st);
   }
 
   // The BN/residual/ReLU op that directly follows conv `i` and reads its output can run in the GEMM epilogue (tensor-core back end).
@@ -1090,6 +1085,29 @@ int bre_engine::refresh_bn_constants(int k) {
   ++launch_count;
   return 0;
 }
+
+namespace {
+// bre_conv_gemm's contraction: NHWC activations, OHWI weights, a 1024-tile split-K workspace
+GemmArgs conv_gemm_args(int mode, const float* a, const float* w, const float* a2, const float* w2, float* out, int N, int H, int W, int Ci,
+                        int Co, int R, int S, int stride, int pad, float* ws, int* counters) {
+  GemmArgs g;
+  memset(&g, 0, sizeof(g));
+  g.mode = mode;
+  g.g = ConvGeom{N, H, W, Ci, (H + 2 * pad - R) / stride + 1, (W + 2 * pad - S) / stride + 1, Co, R, S, stride, pad};
+  g.nsrc = (a2 && w2) ? 2 : 1;
+  g.act[0] = a; g.wgt[0] = w; g.act[1] = a2; g.wgt[1] = w2;
+  g.x_sN = (long long)H * W * Ci; g.x_sP = Ci; g.x_sC = 1;
+  g.out = out;
+  g.ws = ws; g.counters = counters; g.ws_tiles = 1024;
+  return g;
+}
+
+void plan_fields(const GemmPlan& p, int32_t* out) {
+  const int32_t v[GEMM_PLAN_FIELDS] = {p.family, p.mode, p.nsrc, p.tile_rows, p.tile_width, p.splits, p.stages, p.producer,
+                                       p.total_kblocks, p.kblocks_per_split, p.vec};
+  memcpy(out, v, sizeof(v));
+}
+}  // namespace
 
 // ======================================================================================================
 // C ABI
@@ -2174,35 +2192,29 @@ int bre_conv_gemm(int32_t mode, int32_t backend, const float* a, const float* w,
                   int32_t N, int32_t H, int32_t W, int32_t Ci, int32_t Co, int32_t R, int32_t S, int32_t stride, int32_t pad,
                   void* stream) {
   if (!a || !w || !out || mode < 0 || mode > 2) { set_error("bre_conv_gemm: bad arguments"); return BRE_ERR_INVALID; }
-  cudaStream_t s = (cudaStream_t)stream;
-  GemmArgs g;
-  memset(&g, 0, sizeof(g));
-  g.mode = mode;
-  g.g = ConvGeom{N, H, W, Ci, (H + 2 * pad - R) / stride + 1, (W + 2 * pad - S) / stride + 1, Co, R, S, stride, pad};
-  g.nsrc = (a2 && w2) ? 2 : 1;
-  g.act[0] = a; g.wgt[0] = w; g.act[1] = a2; g.wgt[1] = w2;
-  g.x_sN = (long long)H * W * Ci; g.x_sP = Ci; g.x_sC = 1;
-  g.out = out;
   static thread_local float* ws = nullptr;
   static thread_local int* counters = nullptr;
   if (!ws) { BRE_TRY(dev_alloc(&ws, 1024LL * IG_BM * IG_BN)); BRE_TRY(dev_alloc(&counters, 1 << 16)); }
-  g.ws = ws; g.counters = counters; g.ws_tiles = 1024;
-  if (linear_tall_supported(g)) return launch_linear_tall(g, s) == 0 ? BRE_OK : BRE_ERR_CUDA;   // the engine's dispatch rule (gemm_on)
-  if (backend == 1) {
-    if (!igemm_tc_supported(g)) { set_error("tensor-core back end does not cover this shape"); return BRE_ERR_UNSUPPORTED; }
-    return launch_igemm_tc(g, s);
-  }
-  if (backend == 2 && linear_small_preferred(g)) return launch_linear_small(g, s) == 0 ? BRE_OK : BRE_ERR_CUDA;
-  if (backend == 2 && igemm_tc_supported(g)) return launch_igemm_tc(g, s);  // the engine's own dispatch rule
-  return launch_igemm_simt(g, s);
+  const GemmArgs g = conv_gemm_args(mode, a, w, a2, w2, out, N, H, W, Ci, Co, R, S, stride, pad, ws, counters);
+  return launch_gemm(g, backend, (cudaStream_t)stream);
+}
+
+int bre_gemm_plan(int32_t mode, int32_t backend, int32_t N, int32_t H, int32_t W, int32_t Ci, int32_t Co, int32_t R, int32_t S,
+                  int32_t stride, int32_t pad, int32_t nsrc, int32_t* out) {
+  const bool empty = N < 1 || H < 1 || W < 1 || pad < 0 || Ci < 1 || Co < 1 || R < 1 || S < 1 || stride < 1 || H + 2 * pad < R || W + 2 * pad < S;
+  if (!out || mode < 0 || mode > 2 || nsrc < 1 || nsrc > 2 || empty) { set_error("bre_gemm_plan: bad arguments"); return BRE_ERR_INVALID; }
+  // stands for 16-byte aligned operands and workspace: the plan reads their alignment, never their contents
+  alignas(16) static float operand[4];
+  static int counter;
+  const GemmArgs g = conv_gemm_args(mode, operand, operand, nsrc == 2 ? operand : nullptr, nsrc == 2 ? operand : nullptr, operand, N, H, W,
+                                    Ci, Co, R, S, stride, pad, operand, &counter);
+  plan_fields(plan_gemm(g, backend), out);
+  return BRE_OK;
 }
 
 int bre_debug_last_gemm_plan(int32_t* out) {
   if (!out) { set_error("bre_debug_last_gemm_plan: null output"); return BRE_ERR_INVALID; }
-  const GemmPlan& p = last_gemm_plan();
-  const int32_t v[GEMM_PLAN_FIELDS] = {p.family, p.mode, p.nsrc, p.tile_rows, p.tile_width, p.splits, p.stages, p.producer,
-                                       p.total_kblocks, p.kblocks_per_split, p.vec};
-  memcpy(out, v, sizeof(v));
+  plan_fields(last_gemm_plan(), out);
   return BRE_OK;
 }
 

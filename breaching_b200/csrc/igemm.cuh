@@ -52,7 +52,6 @@ struct GemmArgs {
   float* ws;              // split-K workspace (>= ws_tiles * 4096 floats)
   int* counters;          // >= max tiles ints, zero-initialised, self-resetting
   int ws_tiles;
-  int splits;             // 0 = choose automatically
   int force_fp32;         // engine: run this contraction on the fp32 kernels even on the tensor-core back end (precision knob)
   // bit s: wgt[s] (fprop / dgrad) was fully written before the *predecessor* kernel of this launch started, so the tensor-core back end
   // may start loading it before griddepcontrol.wait (model weights; the direction v once a serialised launch follows make_v)
@@ -61,12 +60,12 @@ struct GemmArgs {
 
 constexpr int IG_BM = 64, IG_BN = 64, IG_BK = 16, IG_THREADS = 256;
 
-// What the launchers chose for the last GEMM issued by the calling host thread (bre_debug_last_gemm_plan): the kernel family,
-// tiles, split, ring depth and operand producer.  Host side only: written just before the launch, never passed to a kernel.
+// The launch plan of one GEMM: the kernel family, tiles, split, ring depth, operand producer and vector flags.  plan_gemm decides
+// it from the arguments alone; the family launchers run it as given.  Host side only, never passed to a kernel.
 enum GemmFamily { GEMM_FAM_SIMT = 0, GEMM_FAM_DGRAD_SMALL_CI = 1, GEMM_FAM_LINEAR_SMALL = 2, GEMM_FAM_LINEAR_TALL = 3, GEMM_FAM_TC = 4 };
 enum GemmProducer { GEMM_PROD_NONE = 0, GEMM_PROD_TMA = 1, GEMM_PROD_CP_ASYNC = 2, GEMM_PROD_CLASSES = 3 };
 struct GemmPlan {
-  int family = -1, mode = -1, nsrc = 0;
+  int family = -1, mode = -1, nsrc = 0;   // family -1: no kernel of the back end covers the contraction
   int tile_rows = 0, tile_width = 0;   // output tile (SIMT / tensor core); linear_small: rows of the kernel instance
   int splits = 1, stages = 0;          // split-K factor (grid z; linear_tall: reduction chunks), ring depth
   int producer = GEMM_PROD_NONE;
@@ -75,21 +74,52 @@ struct GemmPlan {
                                        // linear_small fprop: vector loads
 };
 constexpr int GEMM_PLAN_FIELDS = 11;
-void record_gemm_plan(const GemmPlan& p);
+// what launch_gemm ran last on the calling host thread (bre_debug_last_gemm_plan)
 const GemmPlan& last_gemm_plan();
 
-int launch_igemm_simt(const GemmArgs& a, cudaStream_t stream);
-// linear layers on <= 16 rows (the classification head at small batch): dedicated fp32 kernels (linear_small.cu)
+// Switches of the GEMM launch rules (experiments, and the references of the bitwise tests), read from the environment once per
+// process: BRE_TC_* (tensor-core plans), BRE_LINEAR_* (which contractions the small-row linear kernels take).
+struct GemmSwitches {
+  int tc_tma;              // BRE_TC_TMA=0: the cp.async producer everywhere
+  int tc_strided_tma;      // BRE_TC_STRIDED_TMA=0: strided dgrad on the cp.async producer instead of per-class tensor maps
+  int tc_narrow;           // BRE_TC_NARROW=0: 128 x 64 tiles wherever the width allows
+  int tc_stream;           // BRE_TC_STREAM=0: 128-row tiles also where the m-tile holds <= 64 rows
+  int tc_stages;           // BRE_TC_STAGES=2|4|8: forced ring depth (anything else: by rule)
+  int tc_shortk_stages;    // BRE_TC_SHORTK_STAGES (default 2: short reductions on many tiles run a 2-deep ring; 4 turns it off)
+  int tc_max_splits;       // BRE_TC_MAX_SPLITS: cap of the split-K factor (0: none)
+  int tc_target_ctas;      // BRE_TC_TARGET_CTAS: CTAs the split-K rule aims at (0: one per SM)
+  int tc_proxy_fence;      // BRE_TC_PROXY_FENCE=1: async-proxy fence before every wgmma k-block also after TMA writes
+  int tc_prefetch;         // BRE_TC_PREFETCH=0: no prefetch.tensormap
+  int tc_producers;        // BRE_TC_PRODUCERS=1..4: TMA issuing lanes (default 2)
+  int linear_small;        // BRE_LINEAR_SMALL=0: linear layers on <= 16 rows on the SIMT GEMM
+  int linear_small_rows;   // BRE_LINEAR_SMALL_ROWS=1: linear layers on <= 32 rows with a short reduction on the small-row kernels
+  int linear_tall;         // BRE_LINEAR_TALL=0: the tall-K linear dgrad on the GEMM back ends
+};
+const GemmSwitches& gemm_switches();
+
+// One GEMM: the plan and its launch.  backend 0 = SIMT fp32 kernels, 1 = tensor cores only (empty plan where they do not cover the
+// shape), 2 = the engine's dispatch (tensor cores where covered, the fp32 kernels otherwise).  plan_gemm allocates, encodes and
+// launches nothing.  launch_gemm returns BRE_ERR_UNSUPPORTED (-4) for an empty plan.
+GemmPlan plan_gemm(const GemmArgs& a, int backend);
+int launch_gemm(const GemmArgs& a, int backend, cudaStream_t stream);
+
+// The family launchers (called by launch_gemm) run the plan they are given.
+// linear layers on <= 32 rows (the classification head at small batch): dedicated fp32 kernels (linear_small.cu)
 bool linear_small_supported(const GemmArgs& a);
-int launch_linear_small(const GemmArgs& a, cudaStream_t stream);
-bool linear_small_preferred(const GemmArgs& a);   // engine dispatch: small-row linear with a short reduction -> these kernels, not the GEMM
+bool linear_small_preferred(const GemmArgs& a);   // small-row linear with a short reduction -> these kernels, not the GEMM
+GemmPlan linear_small_plan(const GemmArgs& a);
+int launch_linear_small(const GemmArgs& a, const GemmPlan& p, cudaStream_t stream);
 // dgrad of a linear layer with <= 32 rows, <= 128 inputs and >= 8192 outputs (the token models' decoder): chunked reduction in
 // fp32 registers + a fixed-order fold (linear_small.cu); uses a.ws for the per-chunk partial sums
 bool linear_tall_supported(const GemmArgs& a);
-int launch_linear_tall(const GemmArgs& a, cudaStream_t stream);
-// TF32 tensor-core back end (igemm_tc.cu); returns BRE_ERR_UNSUPPORTED (-4) for shapes it does not cover.
-int launch_igemm_tc(const GemmArgs& a, cudaStream_t stream);
+GemmPlan linear_tall_plan(const GemmArgs& a);
+int launch_linear_tall(const GemmArgs& a, const GemmPlan& p, cudaStream_t stream);
+// TF32 tensor-core back end (igemm_tc.cu).  tc_plan: the plan of a covered shape, on the TMA producers where allow_tma and the
+// geometry allow them; empty where no plan without them exists (widths that are only a multiple of 32).  launch_igemm_tc replaces
+// `p` by tc_plan(a, false) when a tensor map of the plan does not encode.
 bool igemm_tc_supported(const GemmArgs& a);
+GemmPlan tc_plan(const GemmArgs& a, bool allow_tma);
+int launch_igemm_tc(const GemmArgs& a, GemmPlan& p, cudaStream_t stream);
 
 inline void gemm_dims(const GemmArgs& a, int& M, int& Nc, int& K) {
   const ConvGeom& g = a.g;

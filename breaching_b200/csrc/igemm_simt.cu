@@ -488,13 +488,25 @@ __global__ void __launch_bounds__(128) dgrad_small_ci_kernel(GemmArgs a, int n_r
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-int launch_dgrad_small_ci(const GemmArgs& a, cudaStream_t stream) {
+bool dgrad_small_ci_fits(const GemmArgs& a) {
+  const ConvGeom& g = a.g;
+  return a.mode == GEMM_DGRAD && g.Ci <= 4 && g.Co <= 16 * SC_KCH && g.H <= 65535 && g.N <= 65535 &&
+         (size_t)a.nsrc * ((g.R + g.stride - 1) / g.stride) * g.S * g.Co * g.Ci * 4 <= 200 * 1024;
+}
+
+GemmPlan dgrad_small_ci_plan(const GemmArgs& a) {
+  bool vec = a.g.Co % 4 == 0;
+  for (int q = 0; q < a.nsrc; ++q) vec = vec && aligned16(a.act[q]);
+  GemmPlan p;
+  p.family = GEMM_FAM_DGRAD_SMALL_CI; p.mode = a.mode; p.nsrc = a.nsrc;
+  p.tile_rows = 32 * SC_PX; p.tile_width = a.g.Ci; p.vec = vec ? 1 : 0;
+  return p;
+}
+
+int launch_dgrad_small_ci(const GemmArgs& a, const GemmPlan& p, cudaStream_t stream) {
   const ConvGeom& g = a.g;
   const int Wc = (g.W + g.stride - 1) / g.stride;
   const int n_r = (g.R + g.stride - 1) / g.stride;   // filter rows that can hit one image row
-  bool vecb = (g.Co % 4 == 0);
-  for (int q = 0; q < a.nsrc; ++q) vecb = vecb && aligned16(a.act[q]);
-  const int vec = vecb ? 1 : 0;
   const int wfloats = a.nsrc * n_r * g.S * g.Co * g.Ci;
   const int rfloats = 4 * 32 * SC_PX * g.Ci;
   const int smem_floats = (wfloats + 3) & ~3;   // weights, then the reduction scratch
@@ -502,10 +514,6 @@ int launch_dgrad_small_ci(const GemmArgs& a, cudaStream_t stream) {
   if (smem > 200 * 1024) { set_error("dgrad_small_ci: filter too large for shared memory"); return -4; }
   const int Wcp = ((Wc + SC_PX - 1) / SC_PX) * SC_PX;
   dim3 grid(ceil_div((long long)Wcp * g.stride, 32 * SC_PX), g.H, g.N), block(128);
-  GemmPlan plan;
-  plan.family = GEMM_FAM_DGRAD_SMALL_CI; plan.mode = a.mode; plan.nsrc = a.nsrc;
-  plan.tile_rows = 32 * SC_PX; plan.tile_width = g.Ci; plan.vec = vec;
-  record_gemm_plan(plan);
 #define BRE_LAUNCH_SC(CI_)                                                                                              \
   do {                                                                                                                  \
     static size_t cap = 0;                                                                                              \
@@ -513,7 +521,7 @@ int launch_dgrad_small_ci(const GemmArgs& a, cudaStream_t stream) {
       BRE_CUDA_CHECK(cudaFuncSetAttribute(dgrad_small_ci_kernel<CI_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
       cap = smem;                                                                                                       \
     }                                                                                                                   \
-    BRE_KLAUNCH((dgrad_small_ci_kernel<CI_>), grid, block, smem, stream, a, n_r, smem_floats, vec);                                     \
+    BRE_KLAUNCH((dgrad_small_ci_kernel<CI_>), grid, block, smem, stream, a, n_r, smem_floats, p.vec);                                   \
   } while (0)
   switch (g.Ci) {
     case 1: BRE_LAUNCH_SC(1); break;
@@ -526,74 +534,123 @@ int launch_dgrad_small_ci(const GemmArgs& a, cudaStream_t stream) {
   return 0;
 }
 
-thread_local GemmPlan g_last_plan;
-
-}  // namespace
-
-void record_gemm_plan(const GemmPlan& p) { g_last_plan = p; }
-const GemmPlan& last_gemm_plan() { return g_last_plan; }
-
-int launch_igemm_simt(const GemmArgs& a, cudaStream_t stream) {
-  Dims d;
-  gemm_dims(a, d.M, d.Nc, d.K);
+GemmPlan simt_plan(const GemmArgs& a) {
   const ConvGeom& g = a.g;
-  if (d.M <= 0 || d.Nc <= 0 || d.K <= 0) { set_error("igemm: empty problem"); return -1; }
-  if (a.nsrc < 1 || a.nsrc > 2) { set_error("igemm: bad nsrc"); return -1; }
-  static const bool small_linear = [] { const char* e = getenv("BRE_LINEAR_SMALL"); return e ? atoi(e) != 0 : true; }();
-  if (small_linear && linear_small_supported(a) && (a.g.N <= 16 || linear_small_preferred(a))) return launch_linear_small(a, stream);
-  if (a.mode == GEMM_DGRAD && g.Ci <= 4 && g.Co <= 16 * SC_KCH && g.H <= 65535 && g.N <= 65535 &&
-      (size_t)a.nsrc * ((g.R + g.stride - 1) / g.stride) * g.S * g.Co * g.Ci * 4 <= 200 * 1024)
-    return launch_dgrad_small_ci(a, stream);
-  d.steps_per_src = ceil_div(d.K, IG_BK);
-  d.total_steps = d.steps_per_src * a.nsrc;
-
+  int M, Nc, K;
+  gemm_dims(a, M, Nc, K);
   bool ptr_ok = true;
   for (int s = 0; s < a.nsrc; ++s) ptr_ok = ptr_ok && aligned16(a.act[s]) && aligned16(a.wgt[s]);
   const bool x_vec = (a.x_sC == 1) && (g.Ci % 4 == 0) && (a.x_sP % 4 == 0) && (a.x_sN % 4 == 0);
+  bool vecA, vecB, vecOut;
   if (a.mode == GEMM_FPROP) {
-    d.vecA = ptr_ok && x_vec;
-    d.vecB = ptr_ok && (d.K % 4 == 0);
-    d.vecOut = aligned16(a.out) && (d.Nc % 4 == 0);
+    vecA = ptr_ok && x_vec;
+    vecB = ptr_ok && (K % 4 == 0);
+    vecOut = aligned16(a.out) && (Nc % 4 == 0);
   } else if (a.mode == GEMM_DGRAD) {
-    d.vecA = ptr_ok && (g.Co % 4 == 0);
-    d.vecB = ptr_ok && (g.Ci % 4 == 0);
-    d.vecOut = aligned16(a.out) && x_vec;
+    vecA = ptr_ok && (g.Co % 4 == 0);
+    vecB = ptr_ok && (g.Ci % 4 == 0);
+    vecOut = aligned16(a.out) && x_vec;
   } else {
-    d.vecA = ptr_ok && (g.Co % 4 == 0);
-    d.vecB = ptr_ok && x_vec;
-    d.vecOut = aligned16(a.out) && (d.Nc % 4 == 0);
+    vecA = ptr_ok && (g.Co % 4 == 0);
+    vecB = ptr_ok && x_vec;
+    vecOut = aligned16(a.out) && (Nc % 4 == 0);
   }
-
-  const int tm = ceil_div(d.M, IG_BM), tn = ceil_div(d.Nc, IG_BN);
-  const long long tiles = (long long)tm * tn;
-  int splits = a.splits;
-  if (splits <= 0) {
-    splits = 1;
-    if (tiles < 2 * kNumSMs) {
-      splits = ceil_div(2 * kNumSMs, tiles);
-      const int max_by_k = d.total_steps / 4 > 0 ? d.total_steps / 4 : 1;
-      if (splits > max_by_k) splits = max_by_k;
-    }
+  const int total = ceil_div(K, IG_BK) * a.nsrc;
+  const long long tiles = (long long)ceil_div(M, IG_BM) * ceil_div(Nc, IG_BN);
+  int splits = 1;
+  if (tiles < 2 * kNumSMs) {
+    splits = ceil_div(2 * kNumSMs, tiles);
+    const int max_by_k = total / 4 > 0 ? total / 4 : 1;
+    if (splits > max_by_k) splits = max_by_k;
   }
-  if (splits > d.total_steps) splits = d.total_steps;
+  if (splits > total) splits = total;
   if (splits > 1 && (a.ws == nullptr || a.counters == nullptr)) splits = 1;
   if (splits > 1 && tiles * splits > a.ws_tiles) splits = (int)(a.ws_tiles / tiles) > 1 ? (int)(a.ws_tiles / tiles) : 1;
-  d.steps_per_split = ceil_div(d.total_steps, splits);
-  splits = ceil_div(d.total_steps, d.steps_per_split);  // no empty splits
-  if (tn > 65535 || splits > 65535) { set_error("igemm: grid too large"); return -1; }
+  GemmPlan p;
+  p.family = GEMM_FAM_SIMT; p.mode = a.mode; p.nsrc = a.nsrc;
+  p.tile_rows = IG_BM; p.tile_width = IG_BN; p.stages = 2;
+  p.total_kblocks = total; p.kblocks_per_split = ceil_div(total, splits);
+  p.splits = ceil_div(total, p.kblocks_per_split);  // no empty splits
+  p.vec = (vecA ? 1 : 0) | (vecB ? 2 : 0) | (vecOut ? 4 : 0);
+  return p;
+}
 
-  dim3 grid(tm, tn, splits), block(IG_THREADS);
-  GemmPlan plan;
-  plan.family = GEMM_FAM_SIMT; plan.mode = a.mode; plan.nsrc = a.nsrc;
-  plan.tile_rows = IG_BM; plan.tile_width = IG_BN; plan.splits = splits; plan.stages = 2;
-  plan.total_kblocks = d.total_steps; plan.kblocks_per_split = d.steps_per_split;
-  plan.vec = (d.vecA ? 1 : 0) | (d.vecB ? 2 : 0) | (d.vecOut ? 4 : 0);
-  record_gemm_plan(plan);
+int launch_igemm_simt(const GemmArgs& a, const GemmPlan& p, cudaStream_t stream) {
+  Dims d;
+  gemm_dims(a, d.M, d.Nc, d.K);
+  d.steps_per_src = ceil_div(d.K, IG_BK);
+  d.total_steps = p.total_kblocks;
+  d.steps_per_split = p.kblocks_per_split;
+  d.vecA = p.vec & 1; d.vecB = (p.vec >> 1) & 1; d.vecOut = (p.vec >> 2) & 1;
+  const int tm = ceil_div(d.M, IG_BM), tn = ceil_div(d.Nc, IG_BN);
+  if (tn > 65535 || p.splits > 65535) { set_error("igemm: grid too large"); return -1; }
+  dim3 grid(tm, tn, p.splits), block(IG_THREADS);
   if (a.mode == GEMM_FPROP) BRE_KLAUNCH((igemm_simt_kernel<GEMM_FPROP>), grid, block, 0, stream, a, d);
   else if (a.mode == GEMM_DGRAD) BRE_KLAUNCH((igemm_simt_kernel<GEMM_DGRAD>), grid, block, 0, stream, a, d);
   else BRE_KLAUNCH((igemm_simt_kernel<GEMM_WGRAD>), grid, block, 0, stream, a, d);
   BRE_CHECK_LAUNCH();
   return 0;
+}
+
+thread_local GemmPlan g_last_plan;
+
+}  // namespace
+
+const GemmPlan& last_gemm_plan() { return g_last_plan; }
+
+const GemmSwitches& gemm_switches() {
+  static const GemmSwitches sw = [] {
+    auto getenv_or = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
+    GemmSwitches s;
+    s.tc_tma = getenv_or("BRE_TC_TMA", 1);
+    s.tc_strided_tma = getenv_or("BRE_TC_STRIDED_TMA", 1);
+    s.tc_narrow = getenv_or("BRE_TC_NARROW", 1);
+    s.tc_stream = getenv_or("BRE_TC_STREAM", 1);
+    s.tc_stages = getenv_or("BRE_TC_STAGES", 0);
+    s.tc_shortk_stages = getenv_or("BRE_TC_SHORTK_STAGES", 2);
+    s.tc_max_splits = getenv_or("BRE_TC_MAX_SPLITS", 0);
+    s.tc_target_ctas = getenv_or("BRE_TC_TARGET_CTAS", 0);
+    s.tc_proxy_fence = getenv_or("BRE_TC_PROXY_FENCE", 0);
+    s.tc_prefetch = getenv_or("BRE_TC_PREFETCH", 1);
+    s.tc_producers = getenv_or("BRE_TC_PRODUCERS", 2);
+    if (s.tc_producers < 1 || s.tc_producers > 4) s.tc_producers = 2;
+    s.linear_small = getenv_or("BRE_LINEAR_SMALL", 1);
+    s.linear_small_rows = getenv_or("BRE_LINEAR_SMALL_ROWS", 0);
+    s.linear_tall = getenv_or("BRE_LINEAR_TALL", 1);
+    return s;
+  }();
+  return sw;
+}
+
+// The family order of every GEMM, for all back ends: the tall-K linear dgrad, the small-row linear kernels where they are
+// preferred, the tensor cores where they cover the shape, then the fp32 kernels -- the small-row linear kernels, the small-channel
+// dgrad, the SIMT implicit GEMM.
+GemmPlan plan_gemm(const GemmArgs& a, int backend) {
+  if (linear_tall_supported(a)) return linear_tall_plan(a);
+  if (backend != 1 && linear_small_preferred(a)) return linear_small_plan(a);
+  if (backend != 0 && igemm_tc_supported(a)) return tc_plan(a, true);
+  if (backend == 1) return GemmPlan();
+  if (gemm_switches().linear_small && a.g.N <= 16 && linear_small_supported(a)) return linear_small_plan(a);
+  if (dgrad_small_ci_fits(a)) return dgrad_small_ci_plan(a);
+  return simt_plan(a);
+}
+
+int launch_gemm(const GemmArgs& a, int backend, cudaStream_t stream) {
+  int M, Nc, K;
+  gemm_dims(a, M, Nc, K);
+  if (M <= 0 || Nc <= 0 || K <= 0 || a.nsrc < 1 || a.nsrc > 2) { set_error("igemm: empty problem or bad nsrc"); return -1; }
+  GemmPlan p = plan_gemm(a, backend);
+  int rc;
+  switch (p.family) {
+    case GEMM_FAM_LINEAR_TALL: rc = launch_linear_tall(a, p, stream); break;
+    case GEMM_FAM_LINEAR_SMALL: rc = launch_linear_small(a, p, stream); break;
+    case GEMM_FAM_TC: rc = launch_igemm_tc(a, p, stream); break;
+    case GEMM_FAM_DGRAD_SMALL_CI: rc = launch_dgrad_small_ci(a, p, stream); break;
+    case GEMM_FAM_SIMT: rc = launch_igemm_simt(a, p, stream); break;
+    default: set_error("tensor-core back end does not cover this shape"); return -4;
+  }
+  g_last_plan = p;
+  return rc;
 }
 
 }  // namespace bre

@@ -943,14 +943,16 @@ bool tiled_map(CUtensorMap* out, const float* base, int rank, const long long* d
 
 // Does the TMA producer cover this contraction?  (strided dgrad does not: see the header of this file.)
 bool tma_eligible(const GemmArgs& a) {
-  static const int tma_env = [] { const char* e = getenv("BRE_TC_TMA"); return e ? atoi(e) : 1; }();
-  if (!tma_env || !tma_api().ok) return false;
+  if (!gemm_switches().tc_tma || !tma_api().ok) return false;
   const ConvGeom& g = a.g;
   if (g.stride > 8 || g.pad > 127 || g.R - 1 - g.pad > 127 || g.S - 1 - g.pad > 127 || g.R > 128 || g.S > 128) return false;
   if (a.mode == GEMM_DGRAD) return g.stride == 1;
   if (a.mode == GEMM_WGRAD) return g.Ci % 32 == 0;
   return true;
 }
+
+// 128 x 32 / 64 x 32 tiles exist for the TMA producer only
+bool narrow_tiles_ok(const GemmArgs& a) { return gemm_switches().tc_narrow && tma_eligible(a); }
 
 // BM: pixels per im2col box (the tile's rows; part of the map's cache key)
 bool build_maps(const GemmArgs& a, int BN, TcMaps* maps, int BM = TC_BM) {
@@ -1005,11 +1007,10 @@ inline AxisPlan axis_plan(int H, int Ho, int R, int stride, int pad, int e) {
 }
 
 bool cls_eligible(const GemmArgs& a) {
-  static const int env = [] { const char* e = getenv("BRE_TC_STRIDED_TMA"); return e ? atoi(e) : 1; }();
+  const GemmSwitches& sw = gemm_switches();
   const ConvGeom& g = a.g;
-  if (!env || a.mode != GEMM_DGRAD || g.stride != 2 || !tma_api().ok) return false;
-  static const int tma_env = [] { const char* e = getenv("BRE_TC_TMA"); return e ? atoi(e) : 1; }();
-  if (!tma_env || g.R > 16 || g.S > 16) return false;
+  if (!sw.tc_strided_tma || !sw.tc_tma || a.mode != GEMM_DGRAD || g.stride != 2 || !tma_api().ok) return false;
+  if (g.R > 16 || g.S > 16) return false;
   for (int ey = 0; ey < 2; ++ey)
     for (int horiz = 0; horiz < 2; ++horiz) {
       const AxisPlan p = horiz ? axis_plan(g.W, g.Wo, g.S, 2, g.pad, ey) : axis_plan(g.H, g.Ho, g.R, 2, g.pad, ey);
@@ -1018,8 +1019,8 @@ bool cls_eligible(const GemmArgs& a) {
   return true;
 }
 
-bool build_cls(const GemmArgs& a, ClsPlan* plan, TcMapsCls* maps) {
-  const ConvGeom& g = a.g;
+// The classes of a strided dgrad: pixel grids, taps, tap corners and m-tile ranges (host arithmetic only)
+bool class_plan(const ConvGeom& g, ClsPlan* plan) {
   memset(plan, 0, sizeof(*plan));
   plan->stride = g.stride;
   int tiles = 0, n = 0;
@@ -1036,114 +1037,82 @@ bool build_cls(const GemmArgs& a, ClsPlan* plan, TcMapsCls* maps) {
       plan->Ly[n] = py.L; plan->Lx[n] = px.L; plan->ey[n] = ey; plan->ex[n] = ex;
       plan->tile0[n] = tiles;
       tiles += ceil_div((long long)g.N * py.Hc * px.Hc, TC_BM);
-      for (int s = 0; s < a.nsrc && taps; ++s)
-        if (!im2col_map(&maps->act[2 * n + s], a.act[s], g.N, g.Ho, g.Wo, g.Co, (long long)g.Ho * g.Wo * g.Co, g.Co, px.L, py.L, px.U, py.U, 1,
-                        TC_BK, TC_BM, CU_TENSOR_MAP_SWIZZLE_128B))
-          return false;
-      if (!taps)   // never dereferenced (the class has no k-blocks), but a valid descriptor keeps prefetch.tensormap well defined
-        for (int s = 0; s < a.nsrc; ++s) maps->act[2 * n + s] = maps->act[s];
       ++n;
     }
   }
   plan->ncls = n;
   plan->tile0[n] = tiles;
+  return n > 0;
+}
+
+bool build_cls_maps(const GemmArgs& a, const ClsPlan& plan, TcMapsCls* maps) {
+  const ConvGeom& g = a.g;
+  for (int c = 0; c < plan.ncls; ++c) {
+    if (plan.Ty[c] == 0) {   // never dereferenced (the class has no k-blocks), but a valid descriptor keeps prefetch.tensormap well defined
+      for (int s = 0; s < a.nsrc; ++s) maps->act[2 * c + s] = maps->act[s];
+      continue;
+    }
+    const int Uy = plan.Hc[c] - g.Ho + plan.Ly[c], Ux = plan.Wc[c] - g.Wo + plan.Lx[c];
+    for (int s = 0; s < a.nsrc; ++s)
+      if (!im2col_map(&maps->act[2 * c + s], a.act[s], g.N, g.Ho, g.Wo, g.Co, (long long)g.Ho * g.Wo * g.Co, g.Co, plan.Lx[c], plan.Ly[c], Ux, Uy,
+                      1, TC_BK, TC_BM, CU_TENSOR_MAP_SWIZZLE_128B))
+        return false;
+  }
   for (int s = 0; s < a.nsrc; ++s) {
     const long long dims[3] = {g.Ci, (long long)g.R * g.S, g.Co}, strides[2] = {g.Ci, (long long)g.R * g.S * g.Ci};
     const int box[3] = {32, 1, TC_BK};
     if (!tiled_map(&maps->wgt[s], a.wgt[s], 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return false;
   }
-  return n > 0;
+  return true;
 }
 
 template <int MODE, int BN, bool TMA, bool CLS = false, int BM = TC_BM>
-int launch_tc(const GemmArgs& a, const TcDims& d0, const std::conditional_t<CLS, TcMapsCls, TcMaps>& maps, cudaStream_t stream,
-              const ClsPlan* plan_in = nullptr) {
-  TcDims d = d0;
+int launch_tc(const GemmArgs& a, const GemmPlan& p, const std::conditional_t<CLS, TcMapsCls, TcMaps>& maps, cudaStream_t stream,
+              const ClsPlan* cls = nullptr) {
+  TcDims d;
+  gemm_dims(a, d.M, d.Nc, d.K);
+  d.kblocks_per_src = ceil_div(d.K, TC_BK);
+  d.total_kblocks = p.total_kblocks;
+  d.kblocks_per_split = p.kblocks_per_split;
+  d.stage_shift = p.stages == 8 ? 3 : (p.stages == 2 ? 1 : 2);
   ClsPlan plan;
   memset(&plan, 0, sizeof(plan));
-  if (CLS) plan = *plan_in;
-  // CLS: the m-tiles of all classes side by side; the k extent that sizes the split is the largest class's
+  if (CLS) plan = *cls;
   const int tm = CLS ? plan.tile0[plan.ncls] : ceil_div(d.M, BM), tn = d.Nc / BN;
-  if (CLS) {
-    int kmax = 0;
-    for (int c = 0; c < plan.ncls; ++c) kmax = kmax > plan.Ty[c] * plan.Tx[c] ? kmax : plan.Ty[c] * plan.Tx[c];
-    d.total_kblocks = kmax * (a.g.Co / TC_BK) * a.nsrc;
-    if (d.total_kblocks < 1) d.total_kblocks = 1;
-  }
-  const long long tiles = (long long)tm * tn;
-  // split-K factor = cluster size along z: a power of two <= 8 (portable cluster limit) that brings the grid to ~100 CTAs
-  static const int max_splits_env = [] { const char* e = getenv("BRE_TC_MAX_SPLITS"); return e ? atoi(e) : 0; }();
-  static const int target_ctas_env = [] { const char* e = getenv("BRE_TC_TARGET_CTAS"); return e ? atoi(e) : 0; }();
-  const int target = target_ctas_env > 0 ? target_ctas_env : kNumSMs;   // about one wave of CTAs
-  constexpr int kMaxCluster = 8;  // portable cluster size
-  int splits = a.splits;
-  if (splits <= 0) {
-    splits = 1;
-    while (splits < kMaxCluster && tiles * splits < target && d.total_kblocks / (splits * 2) >= 2) splits *= 2;
-  }
-  if (max_splits_env > 0 && splits > max_splits_env) splits = max_splits_env;
-  int pow2 = 1;
-  while (pow2 * 2 <= splits && pow2 < kMaxCluster) pow2 *= 2;
-  splits = pow2;
-  while (splits > 1 && splits > d.total_kblocks) splits /= 2;
-  d.kblocks_per_split = ceil_div(d.total_kblocks, splits);
   if (tn > 65535) { set_error("igemm_tc: grid too large"); return -1; }
-  // Ring depth: 4 stages (96 KB: two CTAs per SM within the 227 KB an SM offers, and the next kernel's CTAs can become
-  // resident during this one's tail -- what programmatic dependent launch needs).  BRE_TC_STAGES=2|4|8 forces a depth for
-  // experiments (8 stages = 192 KB, one CTA per SM).
-  static const int stages_env = [] { const char* e = getenv("BRE_TC_STAGES"); return e ? atoi(e) : 0; }();
-  // Short reductions on many tiles (the token models' decoder fprop: 786 tiles x 3-6 k-blocks): a 2-deep ring halves the shared
-  // memory so more CTAs share an SM and the per-CTA prologue / epilogue overlap (BRE_TC_SHORTK_STAGES=4 turns it off)
-  static const int shortk_env = [] { const char* e = getenv("BRE_TC_SHORTK_STAGES"); return e ? atoi(e) : 2; }();
-  const bool shortk = shortk_env == 2 && d.kblocks_per_split <= 6 && tm == 1 && tiles * splits > 2LL * kNumSMs;
-  // 64-row tiles stage half the bytes per k-block, so an 8-deep ring (fprop 128 KB, 128 x 32 dgrad 96 KB) still leaves room for one
-  // 96 KB CTA of the successor.  It pays on launches that are one wave or less and whose CTAs walk long k-ranges: there the k-loop
-  // is the latency of the ring round trip divided by the k-blocks in flight.
-  const bool deep = BM == 64 && tiles * splits <= kNumSMs && d.kblocks_per_split >= 16;
-  const int stages = (stages_env == 8 || stages_env == 2 || stages_env == 4) ? stages_env : (shortk ? 2 : (deep ? 8 : TC_STAGES));
-  d.stage_shift = stages == 8 ? 3 : (stages == 2 ? 1 : 2);
-  const size_t smem = (size_t)stages * (BM + BN) * TC_BK * 4;
+  const size_t smem = (size_t)p.stages * (BM + BN) * TC_BK * 4;
   const size_t smem_max = (size_t)TC_MAX_STAGES * (BM + BN) * TC_BK * 4;
   static bool attr_done = false;
   if (!attr_done) {
     BRE_CUDA_CHECK(cudaFuncSetAttribute(igemm_tc_kernel<MODE, BN, TMA, CLS, BM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
     attr_done = true;
   }
-  static const int proxy_fence_env = [] {
-    const char* e = getenv("BRE_TC_PROXY_FENCE");
-    const char* pf = getenv("BRE_TC_PREFETCH");
-    const char* np = getenv("BRE_TC_PRODUCERS");
-    int nprod = np ? atoi(np) : 2;
-    if (nprod < 1 || nprod > 4) nprod = 2;
-    return (e && atoi(e) ? 1 : 0) | ((pf ? atoi(pf) : 1) ? 2 : 0) | (nprod << 2);
-  }();
   // At most one producer lane per ring stage: a lane that shares a stage with another one could wait on the "empty" parity of a
   // phase two rounds old, which reads as complete, and overwrite a stage still in use (BRE_TC_PRODUCERS=4 with a 2-deep ring).
-  int proxy_fence = proxy_fence_env;
-  if (((proxy_fence >> 2) & 7) > stages) proxy_fence = (proxy_fence & 3) | (stages << 2);
-  GemmPlan rec;
-  rec.family = GEMM_FAM_TC; rec.mode = MODE; rec.nsrc = a.nsrc; rec.tile_rows = BM; rec.tile_width = BN; rec.splits = splits;
-  rec.stages = stages; rec.producer = CLS ? GEMM_PROD_CLASSES : (TMA ? GEMM_PROD_TMA : GEMM_PROD_CP_ASYNC);
-  rec.total_kblocks = d.total_kblocks; rec.kblocks_per_split = d.kblocks_per_split;
-  record_gemm_plan(rec);
-  {
-    cudaError_t lerr = launch_kernel(igemm_tc_kernel<MODE, BN, TMA, CLS, BM>, dim3(tm, tn, splits), dim3(TC_BLOCK), smem, stream, splits, a, d,
-                                     proxy_fence, maps, plan);
-    if (lerr != cudaSuccess) { set_error(std::string("igemm_tc launch failed: ") + cudaGetErrorString(lerr)); return -2; }
-  }
+  const GemmSwitches& sw = gemm_switches();
+  const int nprod = sw.tc_producers < p.stages ? sw.tc_producers : p.stages;
+  const int flags = (sw.tc_proxy_fence ? 1 : 0) | (sw.tc_prefetch ? 2 : 0) | (nprod << 2);
+  cudaError_t lerr = launch_kernel(igemm_tc_kernel<MODE, BN, TMA, CLS, BM>, dim3(tm, tn, p.splits), dim3(TC_BLOCK), smem, stream, p.splits, a,
+                                   d, flags, maps, plan);
+  if (lerr != cudaSuccess) { set_error(std::string("igemm_tc launch failed: ") + cudaGetErrorString(lerr)); return -2; }
   BRE_CHECK_LAUNCH();
   return 0;
 }
 
-}  // namespace
-
-static bool narrow_tiles_ok(const GemmArgs& a) {
-  static const int env = [] { const char* e = getenv("BRE_TC_NARROW"); return e ? atoi(e) : 1; }();
-  if (!env || !tma_eligible(a)) return false;
-  if (a.mode == GEMM_DGRAD && a.g.stride != 1) return false;
-  if (a.mode == GEMM_WGRAD && (a.g.Ci % 32 != 0)) return false;
-  return true;
+template <int MODE, int BN>
+int launch_tma(const GemmArgs& a, const GemmPlan& p, const TcMaps& maps, cudaStream_t stream) {
+  if constexpr (MODE != GEMM_WGRAD)
+    if (p.tile_rows == 64) return launch_tc<MODE, BN, true, false, 64>(a, p, maps, stream);
+  return launch_tc<MODE, BN, true>(a, p, maps, stream);
 }
+
+template <int MODE>
+int launch_mode(const GemmArgs& a, const GemmPlan& p, const TcMaps& maps, cudaStream_t stream) {
+  if (p.producer == GEMM_PROD_CP_ASYNC) return launch_tc<MODE, 64, false>(a, p, maps, stream);
+  return p.tile_width == 32 ? launch_tma<MODE, 32>(a, p, maps, stream) : launch_tma<MODE, 64>(a, p, maps, stream);
+}
+
+}  // namespace
 
 bool igemm_tc_supported(const GemmArgs& a) {
   const ConvGeom& g = a.g;
@@ -1151,10 +1120,9 @@ bool igemm_tc_supported(const GemmArgs& a) {
   gemm_dims(a, M, Nc, K);
   for (int s = 0; s < a.nsrc; ++s)
     if (!aligned16(a.act[s]) || !aligned16(a.wgt[s])) return false;
-  if (!aligned16(a.out) || (a.splits == 0 && a.ws == nullptr)) return false;
+  if (!aligned16(a.out) || a.ws == nullptr) return false;
   const bool x_nhwc = a.x_sC == 1 && a.x_sP % 4 == 0 && a.x_sN % 4 == 0;
-  // output tiles are 128 x 64; widths that are only a multiple of 32 (token models: d = 96, 3 d = 288) run 128 x 32 tiles, which
-  // exist for the TMA producer only
+  // output tiles are 128 x 64; widths that are only a multiple of 32 (token models: d = 96, 3 d = 288) run 128 x 32 tiles
   if (Nc % 64 != 0 && !(Nc % 32 == 0 && narrow_tiles_ok(a))) return false;
   switch (a.mode) {
     case GEMM_FPROP: return x_nhwc && g.Ci % TC_BK == 0 && g.R * g.S <= 64;  // k-block inside one (r, s) cell
@@ -1164,58 +1132,95 @@ bool igemm_tc_supported(const GemmArgs& a) {
   }
 }
 
-int launch_igemm_tc(const GemmArgs& a, cudaStream_t stream) {
-  if (!igemm_tc_supported(a)) { set_error("igemm_tc: unsupported shape"); return -4; }
-  TcDims d;
-  gemm_dims(a, d.M, d.Nc, d.K);
-  d.kblocks_per_src = ceil_div(d.K, TC_BK);
-  d.total_kblocks = d.kblocks_per_src * a.nsrc;
-  d.kblocks_per_split = d.total_kblocks;
-  // TMA producer where the geometry allows it and the driver encodes the maps; otherwise the cp.async producer of the same
-  // kernel (same consumer, still on the GPU: a different loader, not a fallback to another implementation)
-  TcMaps maps;
-  memset(&maps, 0, sizeof(maps));
-  if (cls_eligible(a)) {   // strided dgrad: per-parity-class gathers through im2col tensor maps
-    ClsPlan plan;
-    TcMapsCls cmaps;
-    memset(&cmaps, 0, sizeof(cmaps));
-    if (build_cls(a, &plan, &cmaps)) return launch_tc<GEMM_DGRAD, 64, true, true>(a, d, cmaps, stream, &plan);
+// Every launch rule of the tensor-core back end.  The producer: TMA where the geometry allows it (and allow_tma), per-class tensor maps
+// for the stride-2 dgrad, otherwise the cp.async producer of the same kernel (same consumer, still on the GPU: a different loader, not
+// a fallback to another implementation).
+GemmPlan tc_plan(const GemmArgs& a, bool allow_tma) {
+  const GemmSwitches& sw = gemm_switches();
+  int M, Nc, K;
+  gemm_dims(a, M, Nc, K);
+  GemmPlan p;
+  p.family = GEMM_FAM_TC; p.mode = a.mode; p.nsrc = a.nsrc;
+  int kb = ceil_div(K, TC_BK) * a.nsrc;
+  long long tm = ceil_div(M, TC_BM);
+  ClsPlan cls;
+  if (allow_tma && cls_eligible(a) && class_plan(a.g, &cls)) {
+    // strided dgrad: the m-tiles of all classes side by side; the k extent that sizes the split is the largest class's
+    int kmax = 0;
+    for (int c = 0; c < cls.ncls; ++c) kmax = kmax > cls.Ty[c] * cls.Tx[c] ? kmax : cls.Ty[c] * cls.Tx[c];
+    kb = kmax * (a.g.Co / TC_BK) * a.nsrc;
+    if (kb < 1) kb = 1;
+    tm = cls.tile0[cls.ncls];
+    p.tile_rows = TC_BM; p.tile_width = 64; p.producer = GEMM_PROD_CLASSES;
+  } else {
+    const bool tma = allow_tma && tma_eligible(a), narrow = allow_tma && narrow_tiles_ok(a);
+    if (Nc % 64 != 0 && !narrow) return GemmPlan();
+    // 128 x 32 tiles: widths that are only a multiple of 32, and data / weight gradients whose 128 x 64 tiles would fill at most
+    // half the SMs even at the full 8-CTA split while every CTA walks a long k-range (batch 1: ResNet-18's layer-3 / layer-4 dgrad,
+    // 8 tiles x 8 = 64 CTAs over 9-36 k-blocks each; the stem's column wgrad, 3 tiles x 49).  Their mma.sync consumer (fragments
+    // loaded with ld.shared) bounds the k-loop; halving the tile width doubles the CTAs and halves each CTA's MMA and fragment-load
+    // work per k-block, while every output element keeps the same k-blocks per split, the same MMA accumulation chain and the same
+    // fixed-order cluster reduction: the result is bitwise the one of 128 x 64 tiles.  Both grids stay <= kNumSMs, so the split-K
+    // rule picks the same 8-way split for either.  Measured per launch on the H100 (scripts/profile_gemms.py, DESIGN.md section 6):
+    // dgrad 15-44 -> 10-32 us, the stem wgrad 44 -> 34 us; the wgmma fprop of the same shapes gained 0-2 us on some and lost 2 us on
+    // layer 4's, so it keeps 128 x 64 tiles.
+    const bool underfilled = a.mode != GEMM_FPROP && Nc % 64 == 0 && tm * (Nc / 64) * 16 <= kNumSMs && kb >= 64 && narrow;
+    p.tile_width = Nc % 64 != 0 || underfilled ? 32 : 64;
+    // 64-row tiles for an m-tile of <= 64 GEMM rows (batch 1: every 7 x 7 layer-4 launch, M = 49): a 128-row im2col box would stage
+    // 64+ rows past the end of the tensor every k-block.  Rows 0-63 see the same wgmma / mma.sync instructions on the same operands,
+    // the tile count, split and k-ranges do not change (ceil(M / 64) = ceil(M / 128) = 1), so the result is bitwise that of
+    // 128-row tiles.  BRE_TC_STREAM=0 keeps 128-row tiles.
+    p.tile_rows = sw.tc_stream && M <= 64 && a.mode != GEMM_WGRAD && tma ? 64 : TC_BM;
+    p.producer = tma ? GEMM_PROD_TMA : GEMM_PROD_CP_ASYNC;
   }
-  // 128 x 32 tiles: widths that are only a multiple of 32 (TMA producer only, see igemm_tc_supported), and data / weight gradients
-  // whose 128 x 64 tiles would fill at most half the SMs even at the full 8-CTA split while every CTA walks a long k-range (batch 1:
-  // ResNet-18's layer-3 / layer-4 dgrad, 8 tiles x 8 = 64 CTAs over 9-36 k-blocks each; the stem's column wgrad, 3 tiles x 49).
-  // Their mma.sync consumer (fragments loaded with ld.shared) bounds the k-loop; halving the tile width doubles the CTAs and halves
-  // each CTA's MMA and fragment-load work per k-block, while every output element keeps the same k-blocks per split, the same MMA
-  // accumulation chain and the same fixed-order cluster reduction: the result is bitwise the one of 128 x 64 tiles.  Both grids stay
-  // <= kNumSMs, so the split-K rule picks the same 8-way split for either.  Measured per launch on the H100 (scripts/profile_gemms.py,
-  // DESIGN.md section 6): dgrad 15-44 -> 10-32 us, the stem wgrad 44 -> 34 us; the wgmma fprop of the same shapes gained 0-2 us on
-  // some and lost 2 us on layer 4's, so it keeps 128 x 64 tiles.
-  const long long wide_tiles = (long long)ceil_div(d.M, TC_BM) * (d.Nc / 64);
-  const bool underfilled = a.mode != GEMM_FPROP && d.Nc % 64 == 0 && wide_tiles * 16 <= kNumSMs && d.total_kblocks >= 64 &&
-                           narrow_tiles_ok(a);
-  // 64-row tiles for an m-tile of <= 64 GEMM rows (batch 1: every 7 x 7 layer-4 launch, M = 49): a 128-row im2col box would stage
-  // 64+ rows past the end of the tensor every k-block.  Rows 0-63 see the same wgmma / mma.sync instructions on the same operands,
-  // the tile count, split and k-ranges do not change (ceil(M / 64) = ceil(M / 128) = 1), so the result is bitwise that of
-  // 128-row tiles.  BRE_TC_STREAM=0 keeps 128-row tiles.
-  static const int stream_env = [] { const char* e = getenv("BRE_TC_STREAM"); return e ? atoi(e) : 1; }();
-  const bool rows64 = stream_env && d.M <= 64 && (a.mode == GEMM_FPROP || a.mode == GEMM_DGRAD) && tma_eligible(a);
-  if (d.Nc % 64 != 0 || (underfilled && build_maps(a, 32, &maps, rows64 ? 64 : TC_BM))) {
-    if (d.Nc % 64 != 0 && !build_maps(a, 32, &maps, rows64 ? 64 : TC_BM)) {
-      set_error("igemm_tc: tensor-map encoding failed for a narrow-tile shape");
-      return -4;
+  // split-K factor = cluster size along z: a power of two <= 8 (portable cluster limit) that brings the grid to about one wave
+  const long long tiles = tm * (Nc / p.tile_width);
+  const int target = sw.tc_target_ctas > 0 ? sw.tc_target_ctas : kNumSMs;
+  constexpr int kMaxCluster = 8;  // portable cluster size
+  int splits = 1;
+  while (splits < kMaxCluster && tiles * splits < target && kb / (splits * 2) >= 2) splits *= 2;
+  if (sw.tc_max_splits > 0 && splits > sw.tc_max_splits) splits = sw.tc_max_splits;
+  int pow2 = 1;
+  while (pow2 * 2 <= splits && pow2 < kMaxCluster) pow2 *= 2;
+  splits = pow2;
+  while (splits > 1 && splits > kb) splits /= 2;
+  p.splits = splits;
+  p.total_kblocks = kb;
+  p.kblocks_per_split = ceil_div(kb, splits);
+  // Ring depth: 4 stages (96 KB: two CTAs per SM within the 227 KB an SM offers, and the next kernel's CTAs can become resident
+  // during this one's tail -- what programmatic dependent launch needs).  BRE_TC_STAGES=2|4|8 forces a depth for experiments
+  // (8 stages = 192 KB, one CTA per SM).
+  // Short reductions on many tiles (the token models' decoder fprop: 786 tiles x 3-6 k-blocks): a 2-deep ring halves the shared
+  // memory so more CTAs share an SM and the per-CTA prologue / epilogue overlap (BRE_TC_SHORTK_STAGES=4 turns it off).
+  const bool shortk = sw.tc_shortk_stages == 2 && p.kblocks_per_split <= 6 && tm == 1 && tiles * splits > 2LL * kNumSMs;
+  // 64-row tiles stage half the bytes per k-block, so an 8-deep ring (fprop 128 KB, 128 x 32 dgrad 96 KB) still leaves room for one
+  // 96 KB CTA of the successor.  It pays on launches that are one wave or less and whose CTAs walk long k-ranges: there the k-loop
+  // is the latency of the ring round trip divided by the k-blocks in flight.
+  const bool deep = p.tile_rows == 64 && tiles * splits <= kNumSMs && p.kblocks_per_split >= 16;
+  const int forced = sw.tc_stages;
+  p.stages = (forced == 8 || forced == 2 || forced == 4) ? forced : (shortk ? 2 : (deep ? 8 : TC_STAGES));
+  return p;
+}
+
+int launch_igemm_tc(const GemmArgs& a, GemmPlan& p, cudaStream_t stream) {
+  if (p.producer == GEMM_PROD_CLASSES) {
+    ClsPlan cls;
+    TcMapsCls maps;
+    memset(&maps, 0, sizeof(maps));
+    if (class_plan(a.g, &cls) && build_cls_maps(a, cls, &maps)) return launch_tc<GEMM_DGRAD, 64, true, true>(a, p, maps, stream, &cls);
+  } else {
+    TcMaps maps;
+    memset(&maps, 0, sizeof(maps));
+    if (p.producer == GEMM_PROD_CP_ASYNC || build_maps(a, p.tile_width, &maps, p.tile_rows)) {
+      if (a.mode == GEMM_FPROP) return launch_mode<GEMM_FPROP>(a, p, maps, stream);
+      if (a.mode == GEMM_DGRAD) return launch_mode<GEMM_DGRAD>(a, p, maps, stream);
+      return launch_mode<GEMM_WGRAD>(a, p, maps, stream);
     }
-    if (a.mode == GEMM_FPROP) return rows64 ? launch_tc<GEMM_FPROP, 32, true, false, 64>(a, d, maps, stream) : launch_tc<GEMM_FPROP, 32, true>(a, d, maps, stream);
-    if (a.mode == GEMM_DGRAD) return rows64 ? launch_tc<GEMM_DGRAD, 32, true, false, 64>(a, d, maps, stream) : launch_tc<GEMM_DGRAD, 32, true>(a, d, maps, stream);
-    return launch_tc<GEMM_WGRAD, 32, true>(a, d, maps, stream);
   }
-  if (rows64 && build_maps(a, 64, &maps, 64)) {
-    if (a.mode == GEMM_FPROP) return launch_tc<GEMM_FPROP, 64, true, false, 64>(a, d, maps, stream);
-    return launch_tc<GEMM_DGRAD, 64, true, false, 64>(a, d, maps, stream);
-  }
-  const bool tma = tma_eligible(a) && build_maps(a, 64, &maps);
-  if (a.mode == GEMM_FPROP) return tma ? launch_tc<GEMM_FPROP, 64, true>(a, d, maps, stream) : launch_tc<GEMM_FPROP, 64, false>(a, d, maps, stream);
-  if (a.mode == GEMM_DGRAD) return tma ? launch_tc<GEMM_DGRAD, 64, true>(a, d, maps, stream) : launch_tc<GEMM_DGRAD, 64, false>(a, d, maps, stream);
-  return tma ? launch_tc<GEMM_WGRAD, 64, true>(a, d, maps, stream) : launch_tc<GEMM_WGRAD, 64, false>(a, d, maps, stream);
+  // a tensor map of the plan did not encode: the plan of the cp.async producer, which exists unless the width is only a multiple of 32
+  p = tc_plan(a, false);
+  if (p.family < 0) { set_error("igemm_tc: tensor-map encoding failed for a narrow-tile shape"); return -4; }
+  return launch_igemm_tc(a, p, stream);
 }
 
 }  // namespace bre

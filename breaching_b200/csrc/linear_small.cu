@@ -125,24 +125,15 @@ __global__ void __launch_bounds__(256) linear_small_wgrad_kernel(GemmArgs a) {
 }
 
 template <int NB>
-int launch_nb(const GemmArgs& a, cudaStream_t stream) {
+int launch_nb(const GemmArgs& a, int vec, cudaStream_t stream) {
   const int Co = a.g.Co, Ci = a.g.Ci;
-  GemmPlan plan;
-  plan.family = GEMM_FAM_LINEAR_SMALL; plan.mode = a.mode; plan.nsrc = a.nsrc; plan.tile_rows = NB;
   if (a.mode == GEMM_FPROP) {
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-    int vec = (Ci % 4 == 0) && (a.x_sN % 4 == 0);
-    for (int s = 0; s < a.nsrc; ++s) vec = vec && al16(a.act[s]) && al16(a.wgt[s]);
-    plan.vec = vec;
-    record_gemm_plan(plan);
     BRE_KLAUNCH((linear_small_fprop_kernel<NB>), ceil_div((long long)Co * 32, 256), 256, 0, stream, a, vec);
   } else if (a.mode == GEMM_DGRAD) {
-    record_gemm_plan(plan);
     BRE_KLAUNCH((linear_small_dgrad_kernel<NB>), ceil_div(Ci, 32), 32 * (NB >= 16 ? 8 : (NB >= 8 ? 16 : 32)), 0, stream, a);
   } else {
     long long blocks = ((long long)Co * Ci + 255) / 256;
     if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
-    record_gemm_plan(plan);
     BRE_KLAUNCH((linear_small_wgrad_kernel<NB>), (int)blocks, 256, 0, stream, a);
   }
   BRE_CHECK_LAUNCH();
@@ -265,9 +256,8 @@ inline int tall_chunk(int Co) {   // ~4 blocks per SM, an even number of output 
 }  // namespace
 
 bool linear_tall_supported(const GemmArgs& a) {
-  static const bool env = [] { const char* e = getenv("BRE_LINEAR_TALL"); return e ? atoi(e) != 0 : true; }();
   const ConvGeom& g = a.g;
-  if (!env || a.mode != GEMM_DGRAD) return false;
+  if (!gemm_switches().linear_tall || a.mode != GEMM_DGRAD) return false;
   if (!(g.R == 1 && g.S == 1 && g.H == 1 && g.W == 1 && g.Ho == 1 && g.Wo == 1 && g.stride == 1 && g.pad == 0)) return false;
   if (g.N < 1 || g.N > LT_ROWS || g.Ci % 32 != 0 || g.Ci > 128 || g.Co < 8192 || a.x_sC != 1 || a.epi.kind != 0) return false;
   if (a.nsrc < 1 || a.nsrc > 2 || a.ws == nullptr) return false;
@@ -277,13 +267,17 @@ bool linear_tall_supported(const GemmArgs& a) {
   return need <= (long long)a.ws_tiles * IG_BM * IG_BN;
 }
 
-int launch_linear_tall(const GemmArgs& a, cudaStream_t stream) {
-  const int Co = a.g.Co, Ci = a.g.Ci;
-  const int chunk = tall_chunk(Co), chunks = ceil_div(Co, chunk);
-  GemmPlan plan;
-  plan.family = GEMM_FAM_LINEAR_TALL; plan.mode = a.mode; plan.nsrc = a.nsrc; plan.tile_rows = LT_ROWS; plan.tile_width = Ci;
-  plan.splits = chunks; plan.total_kblocks = Co; plan.kblocks_per_split = chunk;
-  record_gemm_plan(plan);
+GemmPlan linear_tall_plan(const GemmArgs& a) {
+  const int chunk = tall_chunk(a.g.Co);
+  GemmPlan p;
+  p.family = GEMM_FAM_LINEAR_TALL; p.mode = a.mode; p.nsrc = a.nsrc; p.tile_rows = LT_ROWS; p.tile_width = a.g.Ci;
+  p.splits = ceil_div(a.g.Co, chunk); p.total_kblocks = a.g.Co; p.kblocks_per_split = chunk;
+  return p;
+}
+
+int launch_linear_tall(const GemmArgs& a, const GemmPlan& p, cudaStream_t stream) {
+  const int Ci = a.g.Ci;
+  const int chunk = p.kblocks_per_split, chunks = p.splits;
   auto go = [&](auto cj_tag) -> int {
     constexpr int CJ = decltype(cj_tag)::value;
     const size_t smem = (size_t)(LT_MAXC * CJ * 32 + LT_MAXC * LT_PITCH) * sizeof(float);
@@ -317,22 +311,37 @@ bool linear_small_supported(const GemmArgs& a) {
          a.x_sC == 1 && a.epi.kind == 0 && a.nsrc >= 1 && a.nsrc <= 2 && !(a.mode == GEMM_FPROP && a.accumulate);
 }
 
-int launch_linear_small(const GemmArgs& a, cudaStream_t stream) {
-  const int N = a.g.N;
-  if (N <= 1) return launch_nb<1>(a, stream);
-  if (N <= 2) return launch_nb<2>(a, stream);
-  if (N <= 4) return launch_nb<4>(a, stream);
-  if (N <= 8) return launch_nb<8>(a, stream);
-  if (N <= 16) return launch_nb<16>(a, stream);
-  return launch_nb<32>(a, stream);
+// Kernel instance: the smallest row count NB >= N; fprop loads 16-byte vectors where the rows and both operands allow.
+GemmPlan linear_small_plan(const GemmArgs& a) {
+  GemmPlan p;
+  p.family = GEMM_FAM_LINEAR_SMALL; p.mode = a.mode; p.nsrc = a.nsrc;
+  p.tile_rows = 1;
+  while (p.tile_rows < a.g.N) p.tile_rows *= 2;
+  if (a.mode == GEMM_FPROP) {
+    auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    bool vec = (a.g.Ci % 4 == 0) && (a.x_sN % 4 == 0);
+    for (int s = 0; s < a.nsrc; ++s) vec = vec && al16(a.act[s]) && al16(a.wgt[s]);
+    p.vec = vec ? 1 : 0;
+  }
+  return p;
+}
+
+int launch_linear_small(const GemmArgs& a, const GemmPlan& p, cudaStream_t stream) {
+  switch (p.tile_rows) {
+    case 1: return launch_nb<1>(a, p.vec, stream);
+    case 2: return launch_nb<2>(a, p.vec, stream);
+    case 4: return launch_nb<4>(a, p.vec, stream);
+    case 8: return launch_nb<8>(a, p.vec, stream);
+    case 16: return launch_nb<16>(a, p.vec, stream);
+    default: return launch_nb<32>(a, p.vec, stream);
+  }
 }
 
 // Experiment switch (BRE_LINEAR_SMALL_ROWS=1): send linear layers on <= 32 rows with a short reduction (token models at batch 1:
 // 96 -> 288 / 96 / 1536 projections) to the matrix-vector kernels even where the tensor-core kernel covers the shape.  At 32 rows
 // 32 accumulators per thread and 32 broadcast loads per weight element are no match for one MMA, so the default is off.
 bool linear_small_preferred(const GemmArgs& a) {
-  static const int env = [] { const char* e = getenv("BRE_LINEAR_SMALL_ROWS"); return e ? atoi(e) : 0; }();
-  if (!env || a.mode == GEMM_WGRAD || !linear_small_supported(a)) return false;
+  if (!gemm_switches().linear_small_rows || a.mode == GEMM_WGRAD || !linear_small_supported(a)) return false;
   const int K = (a.mode == GEMM_FPROP ? a.g.Ci : a.g.Co) * a.nsrc;
   return K <= 512;
 }

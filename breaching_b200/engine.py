@@ -106,7 +106,7 @@ EXPORTS = [
     "bre_engine_set_augmentation_stages", "bre_engine_augmentation_draws", "bre_augment_resample", "bre_augment_blur",
     "bre_engine_set_augmentations_ex", "bre_engine_set_augmentation_stages_ex", "bre_augment_view_ex", "bre_engine_augmentation_flips",
     "bre_engine_set_trial_index", "bre_engine_debug_step_state", "bre_optimizer_step", "bre_langevin_noise",
-    "bre_debug_last_gemm_plan", "bre_debug_row_plan", "bre_row_op",
+    "bre_debug_last_gemm_plan", "bre_gemm_plan", "bre_debug_row_plan", "bre_row_op",
 ]
 
 
@@ -182,6 +182,7 @@ def load_library(path=None):
     lib.bre_optimizer_step.argtypes = [vp] * 7 + [i32, vp, vp, i64, i32, i32, P(AttackCfg), vp, i32, P(StepScalars), vp]
     lib.bre_langevin_noise.argtypes = [ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64, i64, vp, vp]
     lib.bre_debug_last_gemm_plan.argtypes = [P(i32)]
+    lib.bre_gemm_plan.argtypes = [i32] * 12 + [P(i32)]
     lib.bre_debug_row_plan.argtypes = [i32, P(i32), P(i32)]
     lib.bre_row_op.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, vp, vp, vp, vp]
     for name in EXPORTS:
@@ -862,15 +863,28 @@ GEMM_FAMILIES = {-1: None, 0: "igemm_simt", 1: "dgrad_small_ci", 2: "linear_smal
 GEMM_PRODUCERS = {0: None, 1: "tma", 2: "cp.async", 3: "classes"}
 
 
+def _plan_dict(buf):
+    v = list(buf)
+    return dict(family=GEMM_FAMILIES[v[0]], mode=v[1], nsrc=v[2], tile_rows=v[3], tile_width=v[4], splits=v[5], stages=v[6],
+                producer=GEMM_PRODUCERS[v[7]], total_kblocks=v[8], kblocks_per_split=v[9], vec=v[10])
+
+
 def last_gemm_plan():
     """The launch plan of the last GEMM issued by this host thread (bre_debug_last_gemm_plan): kernel family, mode, nsrc, tile rows /
     width, split-K factor, ring depth, operand producer, k-blocks in all and per split, and the SIMT vector-loader flags."""
     lib = load_library()
     buf = (ctypes.c_int32 * 11)()
     _check(lib, lib.bre_debug_last_gemm_plan(buf), "bre_debug_last_gemm_plan")
-    v = list(buf)
-    return dict(family=GEMM_FAMILIES[v[0]], mode=v[1], nsrc=v[2], tile_rows=v[3], tile_width=v[4], splits=v[5], stages=v[6],
-                producer=GEMM_PRODUCERS[v[7]], total_kblocks=v[8], kblocks_per_split=v[9], vec=v[10])
+    return _plan_dict(buf)
+
+
+def gemm_plan(mode, backend, N, H, W, Ci, Co, R, S, stride, pad, nsrc=1):
+    """The launch plan conv_gemm would run for this contraction (bre_gemm_plan), in the form of last_gemm_plan(); family None where
+    backend 1 does not cover the shape.  Nothing is allocated or launched."""
+    lib = load_library()
+    buf = (ctypes.c_int32 * 11)()
+    _check(lib, lib.bre_gemm_plan(mode, backend, N, H, W, Ci, Co, R, S, stride, pad, nsrc, buf), "bre_gemm_plan")
+    return _plan_dict(buf)
 
 
 def row_plan(C):

@@ -393,6 +393,11 @@ int bre_conv_gemm(int32_t mode, int32_t backend, const float* a, const float* w,
  * 2 cp.async, 3 TMA per parity class), total k-blocks, k-blocks per split (32-wide on the tensor cores, 16-wide on SIMT), vector
  * flags (SIMT: bit 0 A loads, bit 1 B loads, bit 2 stores; dgrad_small_ci / linear_small fprop: vector loads). */
 int bre_debug_last_gemm_plan(int32_t* out);
+/* The launch plan bre_conv_gemm would run for this contraction with nsrc sources (1 or 2) on `backend`, in the 11 fields of
+ * bre_debug_last_gemm_plan (family -1: backend 1 does not cover the shape).  Assumes bre_conv_gemm's operands (NHWC / OHWI,
+ * 16-byte aligned) and its 1024-tile workspace.  Host only: allocates, encodes and launches nothing. */
+int bre_gemm_plan(int32_t mode, int32_t backend, int32_t N, int32_t H, int32_t W, int32_t Ci, int32_t Co, int32_t R, int32_t S,
+                  int32_t stride, int32_t pad, int32_t nsrc, int32_t* out);
 /* The plan of the cluster row kernels (row softmax, softmax chain, token cross-entropy, its tangent, token label gradient) for rows
  * of C elements: *cs = CTAs per row (1, 2, 4 or 8), *fits = 1 when each CTA's segment is cached in registers, 0 when it is streamed. */
 int bre_debug_row_plan(int32_t C, int32_t* cs, int32_t* fits);

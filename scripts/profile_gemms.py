@@ -11,8 +11,8 @@
    table (launches, total and mean device time per iteration).
 
 Both tables go to DIR/gemm_launches.json and DIR/iteration_kernels.json.  The split plan is computed here from the shapes by
-the same rules as launch_igemm_tc / launch_tc in breaching_b200/csrc/igemm_tc.cu (honouring BRE_TC_MAX_SPLITS); it is a label of the rows, the
-times are measured.
+the same rules as tc_plan in breaching_b200/csrc/igemm_tc.cu (honouring BRE_TC_MAX_SPLITS); it is a label of the rows, the times are
+measured.
 """
 import argparse
 import json
@@ -112,12 +112,12 @@ def _tc_split(mode, g, nsrc):
 
 
 def split_plan(mode, g, nsrc):
-    """(tiles, tile width, split-K factor, k-blocks per CTA) as launch_igemm_tc / launch_tc choose them."""
+    """(tiles, tile width, split-K factor, k-blocks per CTA) as tc_plan in igemm_tc.cu chooses them."""
     return _tc_split(mode, g, nsrc)[:4]
 
 
 def ring_plan(mode, g, nsrc):
-    """(tile rows, ring depth) as launch_igemm_tc / launch_tc choose them (honouring BRE_TC_STREAM and BRE_TC_STAGES)."""
+    """(tile rows, ring depth) as tc_plan in igemm_tc.cu chooses them (honouring BRE_TC_STREAM and BRE_TC_STAGES)."""
     N, H, W, Ci, Co, R, st, pd = g
     M, Nc, K = gemm_shape(mode, g)
     tiles, bn, splits, kbc = split_plan(mode, g, nsrc)
@@ -130,7 +130,7 @@ def ring_plan(mode, g, nsrc):
 
 
 def tc_plan(mode, g, nsrc):
-    """The whole tensor-core launch plan, in the form engine.last_gemm_plan() reports it."""
+    """The whole tensor-core launch plan (tc_plan in igemm_tc.cu), in the form engine.last_gemm_plan() reports it."""
     tiles, bn, splits, kbc, kb, cls = _tc_split(mode, g, nsrc)
     bm, stages = ring_plan(mode, g, nsrc)
     producer = "classes" if cls else "tma" if bm == 64 or bn == 32 or tma_ok(mode, g) else "cp.async"
@@ -167,16 +167,23 @@ def linear_small_preferred(mode, g, nsrc):
     return (Ci if mode == 0 else Co) * nsrc <= 512
 
 
+def linear_small_plan(mode, g, nsrc):
+    """linear_small_plan in linear_small.cu for 16-byte aligned operands."""
+    N, H, W, Ci, Co, R, st, pd = g
+    nb = next(b for b in (1, 2, 4, 8, 16, 32) if N <= b)
+    return dict(family="linear_small", mode=mode, nsrc=nsrc, tile_rows=nb, tile_width=0, splits=1, stages=0, producer=None, total_kblocks=0,
+                kblocks_per_split=0, vec=int(mode == 0 and Ci % 4 == 0))
+
+
 def simt_plan(mode, g, nsrc):
-    """launch_igemm_simt in igemm_simt.cu (linear_small / dgrad_small_ci / the SIMT implicit GEMM) for NHWC / OHWI operands on 16-byte
-    aligned buffers, in the form engine.last_gemm_plan() reports it."""
+    """The fp32 kernels of plan_gemm in igemm_simt.cu (linear_small / dgrad_small_ci / the SIMT implicit GEMM) for NHWC / OHWI operands
+    on 16-byte aligned buffers, in the form engine.last_gemm_plan() reports it."""
     N, H, W, Ci, Co, R, st, pd = g
     M, Nc, K = gemm_shape(mode, g)
     base = dict(mode=mode, nsrc=nsrc, tile_rows=0, tile_width=0, splits=1, stages=0, producer=None, total_kblocks=0, kblocks_per_split=0,
                 vec=0)
-    if _env("BRE_LINEAR_SMALL", 1) and _linear(g) and 1 <= N <= 32 and (N <= 16 or linear_small_preferred(mode, g, nsrc)):
-        nb = next(b for b in (1, 2, 4, 8, 16, 32) if N <= b)
-        return dict(base, family="linear_small", tile_rows=nb, vec=int(mode == 0 and Ci % 4 == 0))
+    if _env("BRE_LINEAR_SMALL", 1) and _linear(g) and 1 <= N <= 16:
+        return linear_small_plan(mode, g, nsrc)
     if mode == 1 and Ci <= 4 and Co <= 16 * SC_KCH and nsrc * -(-R // st) * R * Co * Ci * 4 <= 200 * 1024:
         return dict(base, family="dgrad_small_ci", tile_rows=32 * SC_PX, tile_width=Ci, vec=int(Co % 4 == 0))
     total = -(-K // SIMT_BK) * nsrc
@@ -196,18 +203,20 @@ def simt_plan(mode, g, nsrc):
 
 
 def gemm_plan(mode, g, nsrc, backend):
-    """The plan bre_conv_gemm launches for `backend` (0 SIMT, 1 tensor cores, 2 the engine's dispatch), None if it refuses the shape."""
+    """plan_gemm in igemm_simt.cu: the plan bre_conv_gemm launches for `backend` (0 SIMT, 1 tensor cores, 2 the engine's dispatch), None
+    if it refuses the shape.  Family order: linear_tall, linear_small where preferred (not on backend 1), the tensor cores where they
+    cover the shape (not on backend 0), then the fp32 kernels."""
     if linear_tall_ok(mode, g, nsrc):
         N, H, W, Ci, Co, R, st, pd = g
         chunk = _tall_chunk(Co)
         return dict(family="linear_tall", mode=mode, nsrc=nsrc, tile_rows=32, tile_width=Ci, splits=-(-Co // chunk), stages=0, producer=None,
                     total_kblocks=Co, kblocks_per_split=chunk, vec=0)
-    if backend == 1:
-        return tc_plan(mode, g, nsrc) if tc_supported(mode, g) else None
-    if backend == 2 and linear_small_preferred(mode, g, nsrc):
-        return simt_plan(mode, g, nsrc)
-    if backend == 2 and tc_supported(mode, g):
+    if backend != 1 and linear_small_preferred(mode, g, nsrc):
+        return linear_small_plan(mode, g, nsrc)
+    if backend != 0 and tc_supported(mode, g):
         return tc_plan(mode, g, nsrc)
+    if backend == 1:
+        return None
     return simt_plan(mode, g, nsrc)
 
 

@@ -48,7 +48,7 @@ def test_table_reaches_every_plan():
 
 
 def test_64_row_tiles_need_the_tma_producer():
-    """A fprop of M <= 64 that no tensor map covers (stride 10) runs 128-row cp.async tiles, as launch_igemm_tc decides."""
+    """A fprop of M <= 64 that no tensor map covers (stride 10) runs 128-row cp.async tiles, as tc_plan decides."""
     g = (1, 20, 20, 64, 64, 1, 10, 0)
     assert P.gemm_shape(0, g)[0] == 4
     assert P.ring_plan(0, g, 1) == (128, 4)

@@ -6,7 +6,8 @@ float64.  Per case:
     are still NaN bit for bit (no store outside the output) and the output holds no NaN (every element written, no load outside
     the operands multiplied in);
   * bound: |out - ref| <= (K_total + 2) 2^-23 (|A| * |B|) for every element, ref and |A| * |B| in float64;
-  * plan: what the launcher recorded (engine.last_gemm_plan) is the table's plan and the restated one (scripts/profile_gemms.py);
+  * plan: what the launch recorded (engine.last_gemm_plan) is the table's plan, the restated one (scripts/profile_gemms.py) and the
+    one the planner gave before the launch (engine.gemm_plan);
   * a second launch gives the same bits.
 Then one case per mode with off-grid tensor-core operands (the bound widened by the 2^-10 operand truncation), and the tensor-core
 cases once more on the cp.async producer (BRE_TC_TMA=0, read once per process, hence a subprocess)."""
@@ -135,10 +136,13 @@ def reference(case, ops, absolute=False):
 def check(case, want_plan, on_grid=True):
     """Run one case with every check of the module docstring; returns (output on the host, largest error / bound ratio)."""
     mode, geom, nsrc, backend, _ = case
+    N, H, W, Ci, Co, R, st, pd = geom
+    planned = E.gemm_plan(mode, backend, N, H, W, Ci, Co, R, R, st, pd, nsrc)
     ops = operands(case, on_grid)
     obuf, out, bufs = launch(case, ops)
     rec = E.last_gemm_plan()
     assert rec == want_plan, (rec, want_plan)
+    assert planned == rec, (planned, rec)
     assert guards_intact(obuf), "a store outside the output"
     assert all(guards_intact(b) for b in bufs), "an operand's guard changed"
     assert not torch.isnan(out).any(), "an output element not written, or a load outside the operands"

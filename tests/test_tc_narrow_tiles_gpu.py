@@ -1,4 +1,4 @@
-"""128 x 32 tiles for the under-filled data / weight gradients of the tensor-core GEMM (csrc/igemm_tc.cu, launch_igemm_tc): at batch 1
+"""128 x 32 tiles for the under-filled data / weight gradients of the tensor-core GEMM (csrc/igemm_tc.cu, tc_plan): at batch 1
 ResNet-18's layer-3 / layer-4 dgrad and the stem's column wgrad have so few 128 x 64 tiles that even the 8-CTA split leaves half the
 H100 idle, and they run on twice as many 128 x 32 tiles instead.  Every output element keeps its k-ranges, MMA chain and cluster
 reduction order, so the results must be bitwise those of 128 x 64 tiles (BRE_TC_NARROW=0, read once per process, hence a

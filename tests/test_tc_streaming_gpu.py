@@ -1,4 +1,4 @@
-"""64-row tiles for m-tiles of <= 64 GEMM rows (csrc/igemm_tc.cu, launch_igemm_tc): at batch 1 every 7 x 7 layer-4 launch of ResNet-18
+"""64-row tiles for m-tiles of <= 64 GEMM rows (csrc/igemm_tc.cu, tc_plan): at batch 1 every 7 x 7 layer-4 launch of ResNet-18
 stages a 64-pixel im2col box instead of a 128-pixel one whose upper 79 rows lie past the end of the tensor, and the launches that are
 one wave or less and walk >= 16 k-blocks per CTA spend the freed shared memory on an 8-deep ring.  Every output element keeps its
 k-ranges, MMA instruction sequence and cluster reduction order, so the results must be bitwise those of 128-row tiles
