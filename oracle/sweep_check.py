@@ -18,7 +18,8 @@ rounding-error bound derived for that element:
     ``TRAIN_C (P + 8) 2^-24`` times the magnitudes, with the conditioning of the variance / norm differences as a factor;
   * a tensor-core layer (weights read from the TF32 shadow) whose activation operand is stored off the TF32 grid has that
     operand truncated by the tensor core: its bound is widened by 2^-10 of the magnitudes and the op is listed in
-    ``off_grid`` (this contradicts the intent of the engine's rounding flags; today: convolutions fed by a max-pool);
+    ``off_grid`` (this contradicts the intent of the engine's rounding flags; today: GEMMs fed by a max-pool, and linear
+    layers fed by an average pool whose weight gradient runs on the tensor cores);
   * a stored tensor whose every element lies on the TF32 grid (13 low mantissa bits zero) was rounded on store: half a
     TF32 ulp of the reference (per accumulation for deltas summed over several consumers) is added.
 

@@ -100,7 +100,15 @@ def check_evaluation(eng, x, model, grads, labels, cfg, feats, label):
         # largest error / bound ratio per op kind and sweep (headroom of the bounds)
         print(f"\n[{label}] " + ", ".join(f"{k}/{s}: {r:.3g}" for (k, s), r in sorted(chk.ratios.items())) +
               f"; tensor-core ops reading an off-grid activation: {sorted(chk.off_grid)}; fused BN ops: {chk.fused}; stem columns: {chk.stem}")
+    # the activations of tensor-core GEMMs are stored on the TF32 grid, except the pooling outputs (not rounded on store)
+    assert chk.off_grid <= pool_fed(eng.prog), sorted(chk.off_grid)
     return chk
+
+
+def pool_fed(prog):
+    """The conv / linear ops whose input is a max-pool or average-pool output."""
+    pooled = {op.tout for op in prog.ops if op.kind in (C.OP_MAXPOOL, C.OP_AVGPOOL)}
+    return {i for i, op in enumerate(prog.ops) if op.kind in (C.OP_CONV, C.OP_LINEAR) and op.tin in pooled}
 
 
 def check_engine(name, backend, options=(), env=None, monkeypatch=None):

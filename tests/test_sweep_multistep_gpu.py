@@ -96,10 +96,11 @@ class EngineGlue:
         return not torch.equal(self.W_operand[0][j], self.W[0][j])
 
 
-def check_engine(name, backend, options=(), env=None, monkeypatch=None):
+def check_engine(name, backend, options=(), env=None, monkeypatch=None, case=None):
+    """``case``: a tuple as build_case returns it, instead of the named one."""
     for k, v in (env or {}).items():
         monkeypatch.setenv(k, v)
-    case = build_case(name)
+    case = build_case(name) if case is None else case
     model, shared, local, cfg, x, _ = case
     K, dps = local["steps"], local["data_per_step"]
     eng = make_engine(case, backend, options)
