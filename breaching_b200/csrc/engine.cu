@@ -57,6 +57,8 @@ struct BnBuf {
   // train-mode BN reuses di_mean / di_var for the batch statistics and di_cm / di_cv for the tangent-forward means; the
   // tangent-backward means live here
   float *tb1 = nullptr, *tb2 = nullptr;
+  // FedAvg: the current step's copies of its gamma / beta gradient sums (G_gamma, G_beta of its sweep B), null without local steps
+  float *keep_duxh = nullptr, *keep_du = nullptr;
 };
 
 #define BRE_TRY(call)            \
@@ -159,6 +161,10 @@ struct bre_engine {
     std::vector<float*> val, d;
     std::vector<int*> idx;
     std::vector<float*> bn_scale, bn_shift;
+    // train-mode BN layers: this step's batch-statistics constants and its sweep-B sums G_gamma / G_beta (the G arena is
+    // overwritten by the later steps and by the tangent parameter gradients of the reverse pass); eval-mode layers share step 0's
+    // inv / nrm and keep no sums
+    std::vector<float*> bn_inv, bn_nrm, bn_keep_duxh, bn_keep_du;
     float* p = nullptr; float* loss_n = nullptr; long long* labels = nullptr;
   };
   int ms_steps = 0;                 // 0 = single gradient (objectives.py:40-46)
@@ -172,6 +178,7 @@ struct bre_engine {
   struct BnPrep { int gamma_off, beta_off, C; const float* inv; const float* nrm; float* scale; float* shift; };
   std::vector<BnPrep*> ms_bnprep_dev;  // per step (k >= 1): device table for the batched BN-constant refresh
   int n_bn_layers = 0;
+  int n_bn_refresh = 0;                // entries of each refresh table: the eval-mode BN layers
   bool want_tangent_G = false;
   // option "debug_multistep_stop" (tests): 0 = off; s in 1..K = the evaluation returns after step s-1's forward and backward
   // sweeps and its W / D updates; s = K + 1 + k = it returns after step k's tangent sweeps, before its candidate-gradient axpy
@@ -605,6 +612,8 @@ struct bre_engine {
             BRE_LAUNCH(launch_bnact_bwd(r, stream));
             BnTrainArgs ta = bn_train_args(op);
             ta.dst = t[op.tin].d; ta.acc = op.acc_in != 0; ta.round_out = round_d(op.tin);
+            const BnBuf& bb = bn[op.bn_buffer];
+            ta.keep_du = bb.keep_du; ta.keep_duxh = bb.keep_duxh;
             BRE_LAUNCH(launch_bn_train_bwd(ta, stream));
             break;
           }
@@ -640,6 +649,9 @@ struct bre_engine {
     if (forked) {
       BRE_CUDA_CHECK(cudaEventRecord(ev_join, side));
       BRE_CUDA_CHECK(cudaStreamWaitEvent(stream, ev_join, 0));
+      // the next kernel reads the side stream's weight gradients: a programmatic launch may begin before the joined side-stream
+      // work has completed (its griddepcontrol.wait covers only the predecessor on this stream)
+      serialize_next_launch();
     }
     return 0;
   }
@@ -857,7 +869,10 @@ struct bre_engine {
           if (op.has_bn && op.bn_train) {
             BnBuf& b = bn[op.bn_buffer];
             BnTrainArgs ta = bn_train_args(op);
+            if (b.keep_du != nullptr) { ta.sum_du = b.keep_du; ta.sum_duxh = b.keep_duxh; }   // FedAvg: this step's sweep-B sums
+            if (want_tangent_G) { ta.tg_gamma = Gp(op.gamma); ta.tg_beta = Gp(op.beta); }
             BRE_LAUNCH(launch_bn_train_tanbwd_stats(ta, b.tb1, b.tb2, red_partials, red_counters, stream));
+            ta.tg_gamma = ta.tg_beta = nullptr;
             ta.dst = t[op.tin].td; ta.acc = op.acc_in != 0; ta.round_out = round_d(op.tin);
             ta.dres = op.res >= 0 ? t[op.res].td : nullptr; ta.acc_res = op.acc_res != 0;
             BRE_LAUNCH(launch_bn_train_tan_bwd(ta, stream));
@@ -901,6 +916,9 @@ struct bre_engine {
     if (forked) {
       BRE_CUDA_CHECK(cudaEventRecord(ev_join, side));
       BRE_CUDA_CHECK(cudaStreamWaitEvent(stream, ev_join, 0));
+      // the next kernel reads the side stream's weight gradients: a programmatic launch may begin before the joined side-stream
+      // work has completed (its griddepcontrol.wait covers only the predecessor on this stream)
+      serialize_next_launch();
     }
     return 0;
   }
@@ -912,7 +930,10 @@ struct bre_engine {
     pool_idx = b.idx;
     p = b.p; loss_n = b.loss_n; labels = b.labels;
     W = ms_W[k]; Wt = ms_Wt[k];
-    for (int j = 0; j < n_bn_layers; ++j) { bn[j].scale = b.bn_scale[j]; bn[j].shift = b.bn_shift[j]; }
+    for (int j = 0; j < n_bn_layers; ++j) {
+      bn[j].scale = b.bn_scale[j]; bn[j].shift = b.bn_shift[j]; bn[j].inv = b.bn_inv[j]; bn[j].nrm = b.bn_nrm[j];
+      bn[j].keep_duxh = b.bn_keep_duxh[j]; bn[j].keep_du = b.bn_keep_du[j];
+    }
     t[0].val = x + ms_offset[k];
     t[0].td = gradx_step;
   }
@@ -1080,8 +1101,8 @@ __global__ void bn_refresh_kernel(const bre_engine::BnPrep* table, const float* 
 }  // namespace
 
 int bre_engine::refresh_bn_constants(int k) {
-  if (n_bn_layers == 0) return 0;
-  BRE_KLAUNCH(bn_refresh_kernel, n_bn_layers, 128, 0, stream, (const BnPrep*)ms_bnprep_dev[k], (const float*)ms_W[k]);
+  if (n_bn_refresh == 0) return 0;
+  BRE_KLAUNCH(bn_refresh_kernel, n_bn_refresh, 128, 0, stream, (const BnPrep*)ms_bnprep_dev[k], (const float*)ms_W[k]);
   ++launch_count;
   return 0;
 }
@@ -1432,8 +1453,16 @@ int bre_engine_set_local_steps(bre_engine* e, int32_t total_images, int32_t step
   if (!e || steps < 1 || total_images < 1 || !labels) { set_error("bre_engine_set_local_steps: bad arguments"); return BRE_ERR_INVALID; }
   if (!e->model_loaded) { set_error("load the model first"); return BRE_ERR_STATE; }
   if (e->ms_steps > 0) { set_error("local steps already configured"); return BRE_ERR_STATE; }
-  for (const bre_op_desc& o : e->ops)
-    if (o.kind == BRE_OP_BNACT && o.has_bn && o.bn_train) { set_error("multi-step updates with train-mode BatchNorm are not implemented"); return BRE_ERR_UNSUPPORTED; }
+  for (size_t i = 0; i < e->ops.size(); ++i) {   // torch refuses such a training step as well
+    const bre_op_desc& o = e->ops[i];
+    const bre_tensor_desc& to = e->td(o.tout);
+    if (o.kind == BRE_OP_BNACT && o.has_bn && o.bn_train && (long long)to.N * to.H * to.W == 1) {
+      set_error("train-mode BatchNorm layer at op " + std::to_string(i) + " (" + std::to_string(to.C) + " channels at " +
+                std::to_string(to.H) + "x" + std::to_string(to.W) + ") sees one value per channel with " + std::to_string(to.N) +
+                " image(s) per local step: its batch statistics are undefined");
+      return BRE_ERR_UNSUPPORTED;
+    }
+  }
   if (e->cfg.feat_scale > 0.f) {
     set_error("the feature prior is not defined for multi-step updates: its target W_g[y] / b_g[y] is the input feature of one "
               "forward pass only when the shared update is a single gradient; W_K - W_0 sums K local steps with different "
@@ -1477,6 +1506,15 @@ int bre_engine_set_local_steps(bre_engine* e, int32_t total_images, int32_t step
     bre_engine::StepBufs& b = e->ms_bufs[k];
     b.val.assign(e->t.size(), nullptr); b.d.assign(e->t.size(), nullptr); b.idx.assign(e->ops.size(), nullptr);
     b.bn_scale.assign(e->bn.size(), nullptr); b.bn_shift.assign(e->bn.size(), nullptr);
+    b.bn_inv.assign(e->bn.size(), nullptr); b.bn_nrm.assign(e->bn.size(), nullptr);
+    b.bn_keep_duxh.assign(e->bn.size(), nullptr); b.bn_keep_du.assign(e->bn.size(), nullptr);
+    for (size_t j = 0; j < e->bn.size(); ++j) { b.bn_inv[j] = e->bn[j].inv; b.bn_nrm[j] = e->bn[j].nrm; }
+    for (const bre_op_desc& op : e->ops) {
+      if (op.kind != BRE_OP_BNACT || !op.has_bn || !op.bn_train) continue;
+      const int j = op.bn_buffer;
+      if (k > 0) { rc |= e->alloc(&b.bn_inv[j], e->bn[j].C); rc |= e->alloc(&b.bn_nrm[j], e->bn[j].C); }
+      rc |= e->alloc(&b.bn_keep_duxh[j], e->bn[j].C); rc |= e->alloc(&b.bn_keep_du[j], e->bn[j].C);
+    }
     if (k == 0) {
       for (size_t i = 1; i < e->t.size(); ++i) { b.val[i] = e->t[i].val; b.d[i] = e->t[i].d; }
       b.idx = e->pool_idx; b.p = e->p; b.loss_n = e->loss_n; b.labels = e->labels;
@@ -1490,11 +1528,12 @@ int bre_engine_set_local_steps(bre_engine* e, int32_t total_images, int32_t step
       for (size_t j = 0; j < e->bn.size(); ++j) { rc |= e->alloc(&b.bn_scale[j], e->bn[j].C); rc |= e->alloc(&b.bn_shift[j], e->bn[j].C); }
       std::vector<bre_engine::BnPrep> table;
       for (const bre_op_desc& op : e->ops) {
-        if (op.kind != BRE_OP_BNACT || !op.has_bn) continue;
+        if (op.kind != BRE_OP_BNACT || !op.has_bn || op.bn_train) continue;   // train-mode constants: each step's bn_train_prepare
         const BnBuf& bb = e->bn[op.bn_buffer];
         table.push_back({(int)e->params[op.gamma].off, (int)e->params[op.beta].off, bb.C, bb.inv, bb.nrm, b.bn_scale[op.bn_buffer],
                          b.bn_shift[op.bn_buffer]});
       }
+      e->n_bn_refresh = (int)table.size();
       rc |= e->alloc(&e->ms_bnprep_dev[k], (long long)table.size());
       if (rc == 0 && !table.empty())
         BRE_CUDA_CHECK(cudaMemcpy(e->ms_bnprep_dev[k], table.data(), table.size() * sizeof(bre_engine::BnPrep), cudaMemcpyHostToDevice));

@@ -701,6 +701,7 @@ __global__ void bn_train_bwd_kernel(BnTrainArgs a, long long total) {
     float di = __ldg(a.scale + c) * (du - __ldg(a.sum_du + c) * invP - xh * __ldg(a.sum_duxh + c) * invP);
     if (a.acc) di += a.dst[i];
     a.dst[i] = a.round_out ? tf32_rna(di) : di;
+    if (a.keep_du != nullptr && i < a.C) { a.keep_du[i] = a.sum_du[i]; a.keep_duxh[i] = a.sum_duxh[i]; }
   }
 }
 
@@ -763,6 +764,7 @@ __global__ void bn_train_tanbwd_stats_kernel(BnTrainArgs a, float* b1, float* b2
   if (slab_reduce<2>(v, partials, counters, Cpad, tot) && cv) {
     b1[c] = tot[0] / (float)a.P;
     b2[c] = tot[1] / (float)a.P;
+    if (a.tg_beta != nullptr) { a.tg_beta[c] = tot[0]; a.tg_gamma[c] = tot[1]; }
   }
 }
 

@@ -96,6 +96,11 @@ struct BnTrainArgs {
   const float* tres;                                  // tangent of the residual branch (may be null)
   float* dst; bool acc; bool round_out;               // result of the pass (din / tout / tdin)
   float* dres; bool acc_res;                          // TB: tangent delta of the residual branch (may be null)
+  // FedAvg (multi-step) only, null otherwise.  B: copies of sum_du / sum_duxh that outlive the G arena (the step's reverse pass
+  // reads them after later steps have overwritten G).  TB statistics: the tangents of the gamma / beta gradients,
+  // tg_gamma = sum(du' xh + du xh'), tg_beta = sum(du') -- the undivided sums behind b2 / b1.
+  float *keep_du, *keep_duxh;
+  float *tg_gamma, *tg_beta;
 };
 int launch_bn_train_prepare(const float* mean, const float* var, const float* gamma, const float* beta, float eps, int C, float* scale,
                             float* shift, float* inv, float* nrm, cudaStream_t s);

@@ -389,9 +389,11 @@ class Engine:
         """FedAvg: ``labels_per_step`` = list of ``steps`` LongTensors of length ``data_per_step`` (the program batch).
 
         Supported with the matching objectives, TV / norm / orthogonality on the whole candidate, and ``task_regularization`` and
-        DeepInversion on the last local step (its task loss, the BN-input statistics of its forward; both need ``lr != 0``).  The
-        feature prior (its target is the input feature of no forward pass once the update spans several steps) and train-mode BN
-        raise ``EngineError``."""
+        DeepInversion on the last local step (its task loss, the BN-input statistics of its forward; both need ``lr != 0``).
+        Train-mode BN (no BN buffers shared) normalises every local step with its own batch statistics.  The feature prior (its
+        target is the input feature of no forward pass once the update spans several steps) and a train-mode BN layer that would
+        normalise one value per channel (``data_per_step * H * W == 1``; torch refuses that training step too) raise
+        ``EngineError``."""
         labels = torch.cat([l.detach().to(torch.int64).flatten().cpu() for l in labels_per_step]).contiguous()
         if labels.numel() != steps * self.input_shape[0]:
             raise EngineError("labels_per_step must hold data_per_step labels for every local step")

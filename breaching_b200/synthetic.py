@@ -160,10 +160,14 @@ def make_case(model_name="resnet18", data="imagenet", batch=1, seed=233, provide
 
 
 def make_fedavg_case(model_name="resnet18", data="imagenet", num_data_points=4, steps=4, data_per_step=1, lr=1e-3, seed=233,
-                     bn_random=False, image_size=None, classes=None):
+                     bn_random=False, image_size=None, classes=None, no_buffers=False):
     """Multi-step user (cases/users.py:336-413 ``UserMultiStep`` with ``local_updates.yaml``): ``steps`` SGD steps of size
     ``lr`` on consecutive slices of ``data_per_step`` images, eval-mode BN with the server's public buffers; the shared
-    "gradient" is ``W_local - W_server`` and the local hyper-parameters (incl. the per-step labels) are shared."""
+    "gradient" is ``W_local - W_server`` and the local hyper-parameters (incl. the per-step labels) are shared.
+
+    ``no_buffers=True``: the server publishes no BN buffers (``provide_public_buffers=False``), so the user trains in train mode,
+    every local step normalising with its own batch statistics (cases/users.py:345-353), and the attacker has to do the same
+    (base_attack.py:192-197); the payload then has ``buffers=None``, as in :func:`make_case`."""
     import copy
 
     base = dict(IMAGENET if data == "imagenet" else CIFAR10)
@@ -181,7 +185,7 @@ def make_fedavg_case(model_name="resnet18", data="imagenet", num_data_points=4, 
     x = torch.randn((num_data_points, *meta.shape), generator=gen)
     y = torch.randperm(meta.classes, generator=gen)[:num_data_points]
     server_params = [p.detach().clone() for p in model.parameters()]
-    local = copy.deepcopy(model).eval()
+    local = copy.deepcopy(model).train(no_buffers)
     optimizer = torch.optim.SGD(local.parameters(), lr=lr)
     seen, label_list = 0, []
     for _ in range(steps):
@@ -192,7 +196,8 @@ def make_fedavg_case(model_name="resnet18", data="imagenet", num_data_points=4, 
         loss_fn(local(xs), ys).backward()
         optimizer.step()
     shared_grads = [(pl - ps).clone().detach() for pl, ps in zip(local.parameters(), server_params)]
-    server_payload = [dict(parameters=[p for p in model.parameters()], buffers=[b for b in model.buffers()], metadata=meta)]
+    payload_buffers = None if no_buffers else [b for b in model.buffers()]
+    server_payload = [dict(parameters=[p for p in model.parameters()], buffers=payload_buffers, metadata=meta)]
     shared_data = [dict(gradients=shared_grads, buffers=None,
                         metadata=dict(num_data_points=num_data_points, labels=None,
                                       local_hyperparams=dict(lr=lr, steps=steps, data_per_step=data_per_step, labels=label_list)))]
