@@ -86,6 +86,7 @@ class Op:
     beta: int = -1
     eps: float = 1e-5
     bn_module: Optional[str] = None  # qualified module name (running stats are read from it)
+    module: Optional[str] = None     # linear: qualified module name
     # gradient accumulation flags for the reverse sweeps (set by finalize())
     acc_in: bool = False
     acc_res: bool = False
@@ -100,6 +101,11 @@ class Program:
     num_classes: int = 0
     seq_len: int = 0  # > 0: token-sequence program (rows = batch * seq_len), causal next-token loss over rows
     logits_valid: int = 0  # > 0: number of real classes when the logits tensor is padded to the GEMM tile width
+    # the layers the reference's priors single out by module *registration* order (regularizers.py): the BN op of the first
+    # registered BatchNorm2d (DeepInversion's first_bn_multiplier) and the op of the last registered Linear (the features prior);
+    # -1 where the program has none or does not record it
+    di_first_op: int = -1
+    feature_op: int = -1
 
     def describe(self):
         lines = []
@@ -268,7 +274,7 @@ def compile_model(model, input_shape):
                 if feat != mod.in_features:
                     raise UnsupportedModelError(f"linear {node.target}: {feat} features arrive, {mod.in_features} expected")
                 tout = new_tensor(ti.N, mod.out_features, 1, 1)
-                prim.append(dict(kind="linear", tin=tin, tout=tout, w=pidx(mod.weight), b=pidx(mod.bias)))
+                prim.append(dict(kind="linear", tin=tin, tout=tout, w=pidx(mod.weight), b=pidx(mod.bias), module=node.target))
                 if ti.H * ti.W > 1 and tin != 0:
                     # internal activations are NHWC: permute the weight columns once.  The candidate itself (tensor 0) stays
                     # NCHW, so a Linear fed directly by it (the reference's `linear` model, model_preparation.py:238,313)
@@ -340,7 +346,7 @@ def compile_model(model, input_shape):
         if k == "conv":
             op = Op(OP_CONV, p["tin"], p["tout"], R=p["R"], S=p["S"], stride=p["stride"], pad=p["pad"], w=p["w"], b=p["b"])
         elif k == "linear":
-            op = Op(OP_LINEAR, p["tin"], p["tout"], w=p["w"], b=p["b"])
+            op = Op(OP_LINEAR, p["tin"], p["tout"], w=p["w"], b=p["b"], module=p["module"])
         elif k == "maxpool":
             op = Op(OP_MAXPOOL, p["tin"], p["tout"], R=p["R"], S=p["R"], stride=p["stride"], pad=p["pad"])
         elif k == "avgpool":
@@ -395,8 +401,24 @@ def compile_model(model, input_shape):
         if op.res >= 0:
             op.acc_res = op.res in written
             written.add(op.res)
+    _registered_prior_layers(model, prog)
     _compact_tensors(prog)
     return prog
+
+
+def _registered_prior_layers(model, prog):
+    """``prog.di_first_op`` / ``prog.feature_op``: the op of the first BatchNorm2d and of the last Linear in ``model.modules()``
+    order, which is the order the reference's DeepInversion and feature priors hook them in.  A network may register its modules
+    in another order than it runs them; the engine refuses the priors on such a network (engine.Engine)."""
+    rank, order = {}, {}
+    for name, m in model.named_modules(remove_duplicate=False):   # a module registered under two names ranks where modules() lists it
+        order[name] = rank.setdefault(id(m), len(rank))
+    bn = [i for i, op in enumerate(prog.ops) if op.kind == OP_BNACT and op.has_bn]
+    lin = [i for i, op in enumerate(prog.ops) if op.kind == OP_LINEAR]
+    if bn:
+        prog.di_first_op = min(bn, key=lambda i: (order[prog.ops[i].bn_module], i))
+    if lin:
+        prog.feature_op = max(lin, key=lambda i: (order[prog.ops[i].module], i))
 
 
 def _compact_tensors(prog):

@@ -276,6 +276,24 @@ def make_cfg(cfg_attack, noise_seed=0):
     return c
 
 
+def _check_prior_layers(prog, c):
+    """The reference's DeepInversion prior weights the first *registered* BatchNorm2d by ``first_bn_multiplier`` and its features
+    prior reads the input of the last *registered* Linear (regularizers.py); the engine applies them to the first BN op and the
+    last Linear op that run.  Where the two orders pick different layers the engine would optimise another objective than the
+    reference, so the prior is refused, naming both layers."""
+    ops = prog.ops
+    bn = [i for i, op in enumerate(ops) if op.kind == C.OP_BNACT and op.has_bn]
+    lin = [i for i, op in enumerate(ops) if op.kind == C.OP_LINEAR]
+    if c.di_scale > 0 and c.di_first_bn_multiplier != 1.0 and bn and prog.di_first_op != bn[0]:
+        raise EngineError(f"deep_inversion: BatchNorm '{ops[prog.di_first_op].bn_module}' is registered first but "
+                          f"'{ops[bn[0]].bn_module}' runs first; first_bn_multiplier belongs to the first registered one: register "
+                          f"the BatchNorm layers in the order forward() runs them")
+    if c.feat_scale > 0 and lin and prog.feature_op != lin[-1]:
+        raise EngineError(f"features: Linear '{ops[prog.feature_op].module}' is registered last but '{ops[lin[-1]].module}' runs "
+                          f"last; the prior reads the input of the last registered one: register the Linear layers in the order "
+                          f"forward() runs them")
+
+
 class Engine:
     """One engine = one model replica + one trial state on one GPU."""
 
@@ -294,6 +312,8 @@ class Engine:
         self.input_shape = tuple(int(s) for s in input_shape)
         self.ccfg = make_cfg(cfg_attack, noise_seed)
         prog = self.prog
+        if program is None:
+            _check_prior_layers(prog, self.ccfg)
         tens = (TensorDesc * len(prog.tensors))(*[TensorDesc(t.N, t.C, t.H, t.W) for t in prog.tensors])
         pds = []
         for p in prog.params:

@@ -168,7 +168,7 @@ class PriorMultiStepChecker(SC.MultiStepChecker):
 
     def _objective_of(self, k):
         o = dict(self.obj)
-        o.update(tv=None, norm=None, di=None, features=None, task_regularization=0.0)
+        o.update(tv=None, norm=None, di=None, features=None, orthogonality=None, task_regularization=0.0)
         task_seed = 0.0
         if k == self.K - 1:
             lr = self.glue.lr

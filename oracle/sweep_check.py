@@ -113,6 +113,9 @@ stored BN and feature inputs), with the configuration scalars at the fp32 values
     within 4 ulp; squares and square roots are within it), every add / subtract one ``u``; propagated to first order
     through p and q and summed with the double reduction's ``n 2^-53``; the norm ``s / p mean(x^p)`` costs ``POW_C u |x|^p``
     per element;
+  * orthogonality (``obj["orthogonality"]``, ``orthogonality_relation``): ``(1/D) sum_k (S_k^2 - Q_k)`` from the fp32 batch sums
+    S_k / Q_k of x^2 / x^4 at each of the D positions, added into the ``norm`` term; its candidate gradient
+    ``(4/D) x_ik (S_k - x_ik^2)`` joins the candidate-gradient relation of sweep TB; 0 with fewer than two images;
   * ``deep_inversion``: per BN layer ``mult (||rv - var|| + ||rm - mean||)`` from the batch mean and biased variance of the
     stored BN input (``mult = float32(scale x first_bn_multiplier)`` at the first BN layer), with the bound of the fp32
     statistics used for the DeepInversion adjoint: ``|mult| TRAIN_C (M + 8) u (nm kap_m + nv kap_v)``;
@@ -331,6 +334,30 @@ def row_kernel_relations(kernel, z=None, q=None, g=None, p=None, zd=None, labels
     raise ValueError(kernel)
 
 
+def orthogonality_relation(x):
+    """OrthogonalityRegularization (regularizers.py:169-178) as ``orthogonality_kernel`` forms it on the candidate x [N, ...]:
+    (value, value bound, candidate gradient, gradient bound).  Per position k of the D = numel / N, the kernel sums S_k = sum_j x_jk^2
+    and Q_k = sum_j x_jk^4 over the batch in fp32 (every term >= 0: S_k within ``(N + 2) u S_k``, Q_k within ``(N + 3) u Q_k``), the
+    value ``(1/D) sum_k (S_k^2 - Q_k)`` in double (``2 S e_S + e_Q`` per position and the double reduction's ``(D + 4) 2^-53``), the
+    gradient ``(4/D) x_ik (S_k - x_ik^2)`` in fp32 (the difference carries ``e_S + u x^2 + u |S - x^2|``, the three products
+    one u each).  With fewer than two images the term is exactly 0."""
+    N = x.shape[0]
+    if N < 2:
+        return 0.0, 0.0, torch.zeros_like(x), torch.zeros_like(x)
+    xf = x.reshape(N, -1)
+    D = xf.shape[1]
+    x2 = xf * xf
+    S, Q = x2.sum(dim=0), (x2 * x2).sum(dim=0)
+    eS, eQ = (N + 2) * U * S, (N + 3) * U * Q
+    val = float((S * S - Q).sum()) / D
+    bound = float((2 * S * eS + eQ).sum() + (D + 4) * D53 * (S * S + Q).sum()) / D
+    c = 4.0 / D
+    diff = S - x2
+    grad = c * xf * diff
+    egrad = c * xf.abs() * (eS + U * x2 + U * diff.abs()) + 3 * U * grad.abs()
+    return val, bound, grad.view_as(x), egrad.view_as(x)
+
+
 def worst_element(y, ref, bound):
     """(worst error / bound ratio, flat index of that element); NaN counts as infinitely wrong, an exact match as 0."""
     err = (y - ref).abs()
@@ -379,7 +406,10 @@ class SweepChecker:
     """``params``: float64 parameters in ``model.parameters()`` order (what the engine loaded); ``bn``: per op (rm, rv) or None;
     ``g``: target gradients; ``objective``: dict(kind, scale, task_regularization, tv=dict(scale, inner_exp, outer_exp, eps,
     double_opponents) | None, norm=dict(scale, p) | None, di=dict(scale, first_bn_multiplier) | None,
-    features=dict(scale, measured) | None)."""
+    features=dict(scale, measured) | None, and optionally orthogonality=True (the term is added into the ``norm`` slot, as the
+    engine accumulates it there)).  DeepInversion's ``first_bn_multiplier`` goes to the first *registered* BN layer and the
+    features prior reads the last *registered* Linear (``prog.di_first_op`` / ``prog.feature_op``, the reference's rule), not
+    to the first / last one that runs."""
 
     def __init__(self, prog, params, bn, g, labels, objective, source):
         self.prog, self.src = prog, source
@@ -745,8 +775,7 @@ class SweepChecker:
                         mag = mag + self._gemm_dgrad(op, x.shape, V.abs(), dB.abs())
                         K = 2 * K
                     add(op.tin, i, ref, (K + 2) * U2 * mag, mag)
-                if tang and self.obj["features"] is not None and op.kind == C.OP_LINEAR and \
-                        i == max(j for j, o in enumerate(prog.ops) if o.kind == C.OP_LINEAR):
+                if tang and self.obj["features"] is not None and op.kind == C.OP_LINEAR and i == self._feature_op():
                     fs = self.obj["features"]
                     diff = x.reshape(x.shape[0], -1) - fs["measured"].double().reshape(x.shape[0], -1)
                     adj = (2.0 * fs["scale"] / diff.numel() * diff).view_as(x)
@@ -913,7 +942,15 @@ class SweepChecker:
                   (Pch + 4) * U2 * du.abs().sum(dim=(0, 2, 3)))
 
     def _first_bn(self):
-        return min(j for j, o in enumerate(self.prog.ops) if o.kind == C.OP_BNACT and o.has_bn)
+        """The BN op whose DeepInversion term carries ``first_bn_multiplier``: the first registered BatchNorm2d (the first BN op
+        when the program does not record registration order, e.g. token programs)."""
+        first = getattr(self.prog, "di_first_op", -1)
+        return first if first >= 0 else min(j for j, o in enumerate(self.prog.ops) if o.kind == C.OP_BNACT and o.has_bn)
+
+    def _feature_op(self):
+        """The Linear op whose input the features prior reads: the last registered Linear (else the last Linear op)."""
+        last = getattr(self.prog, "feature_op", -1)
+        return last if last >= 0 else max(j for j, o in enumerate(self.prog.ops) if o.kind == C.OP_LINEAR)
 
     def _di_layer(self, i, z):
         """Batch statistics of the BN input ``z`` of op i against the running statistics: (M, mean, var, nm, nv, kap_m, kap_v),
@@ -1127,6 +1164,10 @@ class SweepChecker:
             ref = ref + gp
             tvs = o["tv"]["scale"] if o["tv"] is not None else 0.0
             bound = bound + 64 * U * (gp.abs() + 4 * tvs / x.numel())
+        if o.get("orthogonality"):   # added into the candidate gradient after the other priors: one more rounding of the sum
+            _, _, og, eog = orthogonality_relation(x)
+            ref = ref + og
+            bound = bound + eog + 2 * U * (ref.abs() + og.abs())
         if o["task_regularization"] != 0:
             dt = self.T("delta", 0)
             ref = ref + o["task_regularization"] * dt
@@ -1228,8 +1269,7 @@ class SweepChecker:
 
     def _features_term(self):
         fs = self.obj["features"]
-        lin = max(j for j, o in enumerate(self.prog.ops) if o.kind == C.OP_LINEAR)
-        x = self.T("val", self.prog.ops[lin].tin)
+        x = self.T("val", self.prog.ops[self._feature_op()].tin)
         diff = x.reshape(x.shape[0], -1) - fs["measured"].double().reshape(x.shape[0], -1)
         n, s = diff.numel(), f32(fs["scale"])
         sq = float(diff.pow(2).sum())
@@ -1251,6 +1291,9 @@ class SweepChecker:
             ref["total_variation"] = self._tv_term(x)
         if o["norm"] is not None:
             ref["norm"] = self._norm_term(x)
+        if o.get("orthogonality"):   # accumulated into the norm slot (after the norm prior, in double)
+            v, b = orthogonality_relation(x)[:2]
+            ref["norm"] = (ref["norm"][0] + v, ref["norm"][1] + b + D53 * abs(ref["norm"][0] + v))
         if o["di"] is not None:
             ref["deep_inversion"] = self._di_term()
         if o["features"] is not None:
@@ -1363,7 +1406,7 @@ class MultiStepChecker:
 
     def _step_objective(self):
         o = dict(self.obj)
-        o.update(tv=None, norm=None, di=None, features=None, task_regularization=0.0)
+        o.update(tv=None, norm=None, di=None, features=None, orthogonality=None, task_regularization=0.0)
         return o
 
     def _absorb(self, chk, step):
@@ -1488,4 +1531,8 @@ class MultiStepChecker:
             ref = ref + gp
             tvs = o["tv"]["scale"] if o.get("tv") is not None else 0.0
             bound = bound + 64 * U * (gp.abs() + 4 * tvs / x.numel())
+        if o.get("orthogonality"):
+            _, _, og, eog = orthogonality_relation(x)
+            ref = ref + og
+            bound = bound + eog + 2 * U * (ref.abs() + og.abs())
         self._cmp(None, "GX", "candidate gradient (sum over the local steps + priors)", gl.grad.double(), ref, bound + U * ref.abs())

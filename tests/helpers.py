@@ -169,6 +169,65 @@ def odd_case(seed=5, batch=3):
     return model, (batch, 3, 15, 13), y, [g.detach() for g in grads]
 
 
+class BNRegisteredLate(torch.nn.Module):
+    """conv -> BN -> ReLU -> conv -> BN -> ReLU -> avg-pool -> Linear, with the second BN registered before the first: the first
+    registered BatchNorm2d, which the reference's DeepInversion prior weights by ``first_bn_multiplier``, is not the first that
+    runs.  ``in_order``: the same layers registered in the order they run (same parameter and buffer names)."""
+
+    def __init__(self, in_order=False):
+        super().__init__()
+        if not in_order:
+            self.bn2 = torch.nn.BatchNorm2d(16)
+        self.conv1 = torch.nn.Conv2d(3, 8, 3, padding=1)
+        self.bn1 = torch.nn.BatchNorm2d(8)
+        self.conv2 = torch.nn.Conv2d(8, 16, 3, stride=2, padding=1)
+        if in_order:
+            self.bn2 = torch.nn.BatchNorm2d(16)
+        self.pool = torch.nn.AdaptiveAvgPool2d(1)
+        self.fc = torch.nn.Linear(16, 10)
+
+    def forward(self, x):
+        x = torch.relu(self.bn1(self.conv1(x)))
+        x = torch.relu(self.bn2(self.conv2(x)))
+        return self.fc(torch.flatten(self.pool(x), 1))
+
+
+class LinearRegisteredLast(torch.nn.Module):
+    """conv -> ReLU -> avg-pool -> proj (Linear 16 -> 16) -> ReLU -> fc (Linear 16 -> 10), with proj registered after fc: the last
+    registered Linear, whose input the reference's features prior reads (and whose weight / bias gradients are the last two
+    entries the feature targets are derived from), is not the last that runs.  ``in_order``: registered in the order they run."""
+
+    def __init__(self, in_order=False):
+        super().__init__()
+        self.conv = torch.nn.Conv2d(3, 16, 3, stride=2, padding=1)
+        self.pool = torch.nn.AdaptiveAvgPool2d(1)
+        if in_order:
+            self.proj = torch.nn.Linear(16, 16)
+        self.fc = torch.nn.Linear(16, 10)
+        if not in_order:
+            self.proj = torch.nn.Linear(16, 16)
+
+    def forward(self, x):
+        x = torch.flatten(self.pool(torch.relu(self.conv(x))), 1)
+        return self.fc(torch.relu(self.proj(x)))
+
+
+def registration_case(cls, in_order=False, seed=3, batch=2, size=12):
+    """(model in eval mode with random BN, input shape, labels, target gradients) of a :class:`BNRegisteredLate` /
+    :class:`LinearRegisteredLast`; the ``in_order`` twin has exactly the same parameters and buffers."""
+    torch.manual_seed(seed)
+    model = synthetic.randomize_bn(cls(), seed + 1).eval()
+    if in_order:
+        twin = cls(in_order=True)
+        twin.load_state_dict(model.state_dict())
+        model = twin.eval()
+    gen = torch.Generator().manual_seed(seed + 7)
+    x = torch.randn(batch, 3, size, size, generator=gen)
+    y = torch.randint(0, 10, (batch,), generator=gen)
+    grads = torch.autograd.grad(torch.nn.functional.cross_entropy(model(x), y), list(model.parameters()))
+    return model, (batch, 3, size, size), y, [g.detach() for g in grads]
+
+
 def sweep_objective(cfg, features=None):
     """The objective dict of ``oracle.sweep_check.SweepChecker`` for an attack config."""
     reg = cfg.get("regularization") or {}
@@ -190,6 +249,8 @@ def sweep_objective(cfg, features=None):
         obj["di"] = dict(scale=reg["deep_inversion"]["scale"], first_bn_multiplier=reg["deep_inversion"].get("first_bn_multiplier", 10))
     if on("features") and features is not None:
         obj["features"] = dict(scale=reg["features"]["scale"], measured=features)
+    if on("orthogonality"):   # the reference never multiplies this term by its scale (engine.make_cfg)
+        obj["orthogonality"] = True
     return obj
 
 

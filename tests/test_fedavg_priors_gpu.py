@@ -145,8 +145,9 @@ def make_engine(case, backend):
     return eng
 
 
-def check_engine(name, backend, keep_tangents=False):
-    case = build_case(name)
+def check_engine(name, backend, keep_tangents=False, case=None):
+    """``case``: a tuple as build_case returns it, instead of the named one."""
+    case = build_case(name) if case is None else case
     model, shared, local, cfg, x, _ = case
     K, dps = local["steps"], local["data_per_step"]
     eng = make_engine(case, backend)

@@ -45,10 +45,10 @@ def test_every_sweep_buffer_of_the_case(name, backend):
         eng.close()
 
 
-def fedavg_case(name, steps=2, lr=1e-2):
+def fedavg_case(name, steps=2, lr=1e-2, model_shape=None):
     """The case as a FedAvg update: ``steps`` SGD steps on consecutive slices of twice the case's batch (synthetic.make_fedavg_case),
-    in MS.build_case's form."""
-    model, shape, _, _, _ = build(name)
+    in MS.build_case's form.  ``model_shape``: (model, input shape) of another network instead of the named case's."""
+    model, shape = model_shape or build(name)[:2]
     dps, n = shape[0], 2 * shape[0]
     gen = torch.Generator().manual_seed(23)
     x = torch.randn((n, *shape[1:]), generator=gen)
