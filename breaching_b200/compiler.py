@@ -24,8 +24,9 @@ import torch.fx
 OP_CONV, OP_BNACT, OP_MAXPOOL, OP_AVGPOOL, OP_LINEAR = 1, 2, 3, 4, 5
 # token-sequence models (the TAG / transformer path, SURVEY section 8 rows a15 / a16): tensors are [rows = batch x seq_len, C, 1, 1]
 OP_POSADD, OP_LAYERNORM, OP_ATTENTION = 6, 7, 8
+OP_POSCONST = 9   # + a constant positional table (the fixed sinusoidal positions): no parameter, ``Op.table`` [seq_len, C]
 OP_NAMES = {OP_CONV: "conv", OP_BNACT: "bnact", OP_MAXPOOL: "maxpool", OP_AVGPOOL: "avgpool", OP_LINEAR: "linear",
-            OP_POSADD: "posadd", OP_LAYERNORM: "layernorm", OP_ATTENTION: "attention"}
+            OP_POSADD: "posadd", OP_LAYERNORM: "layernorm", OP_ATTENTION: "attention", OP_POSCONST: "posconst"}
 
 # how a parameter tensor is laid out in the engine arena relative to torch's layout
 PERM_NONE, PERM_OIHW_TO_OHWI, PERM_LINEAR_CHW_TO_HWC = 0, 1, 2
@@ -87,6 +88,7 @@ class Op:
     eps: float = 1e-5
     bn_module: Optional[str] = None  # qualified module name (running stats are read from it)
     module: Optional[str] = None     # linear: qualified module name
+    table: Optional[torch.Tensor] = None   # posconst: the float32 table the op adds, a copy of the model's buffer
     # gradient accumulation flags for the reverse sweeps (set by finalize())
     acc_in: bool = False
     acc_res: bool = False
@@ -445,13 +447,28 @@ def bn_modules(model, prog):
     return [modules[op.bn_module] if (op.kind == OP_BNACT and op.has_bn) else None for op in prog.ops]
 
 
+def _fixed_positions(pos, T, d):
+    """The table ``pe[0, :T]`` of a fixed positional module (a ``pe`` buffer [1, max_len, d], no parameters, dropout 0)."""
+    pe = getattr(pos, "pe", None)
+    if not isinstance(pe, torch.Tensor) or any(True for _ in pos.parameters()):
+        raise UnsupportedModelError("pos_encoder must be a learnable embedding or a constant `pe` buffer without parameters")
+    for m in pos.modules():
+        if isinstance(m, torch.nn.Dropout) and m.p > 0:
+            raise UnsupportedModelError(f"dropout p = {m.p} on the positional encoding is not lowered (the engine adds the table as it is)")
+    if pe.dim() != 3 or pe.shape[0] != 1 or pe.shape[2] != d or pe.shape[1] < T:
+        raise UnsupportedModelError(f"positional table of shape {tuple(pe.shape)} does not cover [1, {T}, {d}]")
+    return pe[0, :T].detach().to(device="cpu", dtype=torch.float32).contiguous().clone()
+
+
 def compile_transformer(model, batch, seq_len, pad_vocab=True):
     """Lower the reference's ``TransformerModel`` (cases/models/language_models.py:150-205) *as the attack runs it* -- token
     embedding bypassed, the candidate is the embedding sequence [batch, seq_len, d] (base_attack.py:76-128) -- to the layer
-    program: learnable positional embedding added, post-norm encoder layers (self-attention without mask, ReLU FFN), linear
-    decoder.  ``model`` needs ``pos_encoder.embedding``, ``transformer_encoder.layers`` and ``decoder`` (``synthetic.TransformerLM``
-    has the reference's attribute names).  Parameter indices follow ``model.parameters()`` with the token embedding removed,
-    i.e. the order of the shared gradient list after base_attack.py:88-95.
+    program: positional embedding added, post-norm encoder layers (self-attention without mask, ReLU FFN), linear decoder.
+    ``model`` needs ``pos_encoder``, ``transformer_encoder.layers`` and ``decoder`` (``synthetic.TransformerLM`` has the
+    reference's attribute names).  A learnable ``pos_encoder.embedding`` (LearnablePositionalEmbedding) lowers to OP_POSADD; a
+    ``pos_encoder`` with a ``pe`` buffer and no parameters (the fixed sinusoidal PositionalEmbedding, language_models.py:89-130)
+    lowers to OP_POSCONST, which adds the model's own float32 values ``pe[0, :seq_len]``.  Parameter indices follow
+    ``model.parameters()`` with the token embedding removed, i.e. the order of the shared gradient list after base_attack.py:88-95.
 
     The program is the contract between this lowering and the sweeps: ``csrc/engine.cu`` executes it on the GPU (token ops in
     ``csrc/tokens.cu``), ``oracle/program_interp.py`` on the CPU (float64-verified against autograd and the reference's TAG
@@ -469,9 +486,17 @@ def compile_transformer(model, batch, seq_len, pad_vocab=True):
         prog.tensors.append(TensorDesc(len(prog.tensors), rows, C, 1, 1))
         return len(prog.tensors) - 1
 
+    enc = getattr(model, "encoder", None)
+    if isinstance(enc, torch.nn.Embedding) and model.decoder.weight is enc.weight:
+        raise UnsupportedModelError("tied token embedding and decoder weights (transformer3t) are not lowered: the attack's run-embedding "
+                                    "prologue removes the gradient entry they share")
     x = new_tensor(d)   # tensor 0: the candidate embeddings
     cur = new_tensor(d)
-    prog.ops.append(Op(OP_POSADD, x, cur, w=pidx["pos_encoder.embedding.weight"], S=int(seq_len)))
+    pos = model.pos_encoder
+    if hasattr(pos, "embedding"):
+        prog.ops.append(Op(OP_POSADD, x, cur, w=pidx["pos_encoder.embedding.weight"], S=int(seq_len)))
+    else:
+        prog.ops.append(Op(OP_POSCONST, x, cur, S=int(seq_len), table=_fixed_positions(pos, int(seq_len), d)))
     for li, layer in enumerate(model.transformer_encoder.layers):
         if getattr(layer, "norm_first", False) or not getattr(layer.self_attn, "batch_first", True):
             raise UnsupportedModelError("only post-norm, batch-first encoder layers (the reference's configuration) are lowered")

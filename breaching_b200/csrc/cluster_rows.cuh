@@ -27,6 +27,14 @@ __device__ __forceinline__ double ld_cluster_f64(const double* local, unsigned r
   asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(raddr) : "memory");
   return v;
 }
+__device__ __forceinline__ float ld_cluster_f32(const float* local, unsigned rank) {
+  const uint32_t saddr = (uint32_t)__cvta_generic_to_shared(local);
+  uint32_t raddr;
+  asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(saddr), "r"(rank));
+  float v;
+  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(raddr) : "memory");
+  return v;
+}
 
 // The row plan, one rule for the kernels and the host: a row of C elements on a cluster of cs CTAs is cut into segments of
 // row_segment_len(C, cs) elements (4-element aligned starts so that float4 access stays possible); a segment of at most

@@ -6,6 +6,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <limits>
 #include <string>
 #include <vector>
@@ -314,6 +315,8 @@ struct bre_engine {
   bool graph_ready = false;
   int launch_count = 0, launches_per_iter = 0;
   bool model_loaded = false, targets_loaded = false, trial_begun = false;
+  bool params_loaded = false;          // model_loaded = the parameters and every constant table (const_missing: ops still without one)
+  std::vector<int> const_missing;
   int trial_index = 0;   // global index of the trials begun from now on (bre_engine_set_trial_index)
 
   template <typename T>
@@ -532,6 +535,9 @@ struct bre_engine {
         case BRE_OP_POSADD:
           BRE_LAUNCH(launch_token_posadd(t[op.tin].val, Wp(op.w), t[op.tout].val, to.N, to.C, op.S, round_val(op.tout), stream));
           break;
+        case BRE_OP_POSCONST:
+          BRE_LAUNCH(launch_token_posadd(t[op.tin].val, tok_a[i], t[op.tout].val, to.N, to.C, op.S, round_val(op.tout), stream));
+          break;
         case BRE_OP_LAYERNORM:
           BRE_LAUNCH(launch_token_layernorm(0, t[op.tin].val, nullptr, nullptr, nullptr, Wp(op.gamma), Wp(op.beta), nullptr, nullptr, op.eps,
                                             to.N, to.C, tok_a[i], t[op.tout].val, 0, round_val(op.tout), stream));
@@ -630,6 +636,10 @@ struct bre_engine {
         }
         case BRE_OP_POSADD:      // gradient of the positional table; the candidate's own delta only for the task-loss term
           BRE_LAUNCH(launch_token_pos_grad(t[op.tout].d, Gp(op.w), to.N, to.C, op.S, stream));
+          if (task_grad_from_backward())
+            BRE_CUDA_CHECK(cudaMemcpyAsync(t[0].d, t[op.tout].d, (size_t)to.N * to.C * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+          break;
+        case BRE_OP_POSCONST:    // identity: no parameter gradient; the candidate's own delta only for the task-loss term
           if (task_grad_from_backward())
             BRE_CUDA_CHECK(cudaMemcpyAsync(t[0].d, t[op.tout].d, (size_t)to.N * to.C * sizeof(float), cudaMemcpyDeviceToDevice, stream));
           break;
@@ -734,6 +744,9 @@ struct bre_engine {
         }
         case BRE_OP_POSADD:      // the candidate's tangent is zero: only the direction component of the positional table
           BRE_LAUNCH(launch_token_posadd(nullptr, Vp(op.w), t[op.tout].tval, to.N, to.C, op.S, round_val(op.tout), stream));
+          break;
+        case BRE_OP_POSCONST:    // the candidate's tangent passes unchanged: it is zero
+          BRE_CUDA_CHECK(cudaMemsetAsync(t[op.tout].tval, 0, (size_t)to.N * to.C * sizeof(float), stream));
           break;
         case BRE_OP_LAYERNORM:
           BRE_LAUNCH(launch_token_layernorm(2, t[op.tin].val, t[op.tin].tval, nullptr, nullptr, Wp(op.gamma), Wp(op.beta), Vp(op.gamma),
@@ -900,6 +913,7 @@ struct bre_engine {
           break;
         }
         case BRE_OP_POSADD:      // d objective / d candidate = tangent delta of the embedded sequence
+        case BRE_OP_POSCONST:
           BRE_CUDA_CHECK(cudaMemcpyAsync(t[0].td, t[op.tout].td, (size_t)to.N * to.C * sizeof(float), cudaMemcpyDeviceToDevice, stream));
           break;
         case BRE_OP_LAYERNORM:
@@ -1159,7 +1173,7 @@ int bre_engine_create(const bre_tensor_desc* tensors, int32_t n_tensors, const b
     if (op.tin < 0 || op.tin >= n_tensors || op.tout <= 0 || op.tout >= n_tensors || op.res >= n_tensors) { set_error("op tensor id out of range"); return fail(BRE_ERR_INVALID); }
     if (op.tin == 0 || op.res == 0) {
       ++consumers0;
-      if (op.res == 0 || (op.kind != BRE_OP_CONV && op.kind != BRE_OP_LINEAR && op.kind != BRE_OP_POSADD)) { set_error("the candidate must feed exactly one conv/linear/posadd layer"); return fail(BRE_ERR_UNSUPPORTED); }
+      if (op.res == 0 || (op.kind != BRE_OP_CONV && op.kind != BRE_OP_LINEAR && op.kind != BRE_OP_POSADD && op.kind != BRE_OP_POSCONST)) { set_error("the candidate must feed exactly one conv/linear/posadd layer"); return fail(BRE_ERR_UNSUPPORTED); }
     }
     if (op.kind == BRE_OP_BNACT && op.has_bn) n_bn = op.bn_buffer + 1 > n_bn ? op.bn_buffer + 1 : n_bn;
     if ((op.kind == BRE_OP_CONV || op.kind == BRE_OP_LINEAR) && (op.w < 0 || op.w >= n_params)) { set_error("conv/linear without weight"); return fail(BRE_ERR_INVALID); }
@@ -1219,9 +1233,13 @@ int bre_engine_create(const bre_tensor_desc* tensors, int32_t n_tensors, const b
   for (int i = 0; i < n_ops; ++i) {
     const bre_op_desc& op = ops[i];
     if (op.kind == BRE_OP_LAYERNORM) rc |= e->alloc(&e->tok_a[i], 2LL * tensors[op.tin].N);
-    if (op.kind == BRE_OP_ATTENTION || op.kind == BRE_OP_POSADD) {
+    if (op.kind == BRE_OP_ATTENTION || op.kind == BRE_OP_POSADD || op.kind == BRE_OP_POSCONST) {
       if (op.S < 1 || tensors[op.tin].N % op.S != 0) { set_error("token op: rows must be a multiple of seq_len"); return fail(BRE_ERR_INVALID); }
       e->seq_len = op.S;
+    }
+    if (op.kind == BRE_OP_POSCONST) {   // the constant table [S, C] (bre_engine_load_constant)
+      rc |= e->alloc(&e->tok_a[i], (long long)op.S * tensors[op.tout].C);
+      e->const_missing.push_back(i);
     }
     if (op.kind == BRE_OP_ATTENTION) {
       const long long np = (long long)(tensors[op.tin].N / op.S) * op.R * op.S * op.S;
@@ -1361,7 +1379,23 @@ int bre_engine_load_model(bre_engine* e, const float* const* params, int32_t n_p
     const bre_op_desc& op = e->ops[e->stem_op];
     BRE_TRY(launch_stem_pad_rows(e->Wp(op.w), e->Wcol, e->td(op.tout).C, op.R * op.S * e->td(op.tin).C, e->stem_Kp, false, e->tc_round_env, e->stream));
   }
-  e->model_loaded = true;
+  e->params_loaded = true;
+  e->model_loaded = e->const_missing.empty();
+  return BRE_OK;
+}
+
+int bre_engine_load_constant(bre_engine* e, int32_t op, const float* table, int64_t numel) {
+  if (!e || !table || op < 0 || op >= (int)e->ops.size() || e->ops[op].kind != BRE_OP_POSCONST) {
+    set_error("bre_engine_load_constant: bad arguments (op must be a constant positional add)");
+    return BRE_ERR_INVALID;
+  }
+  const bre_op_desc& o = e->ops[op];
+  if (numel != (int64_t)o.S * e->td(o.tout).C) { set_error("bre_engine_load_constant: the table must hold seq_len x C elements"); return BRE_ERR_INVALID; }
+  BRE_CUDA_CHECK(cudaSetDevice(e->device));
+  BRE_CUDA_CHECK(cudaMemcpyAsync(e->tok_a[op], table, (size_t)numel * sizeof(float), cudaMemcpyDefault, e->stream));
+  BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  e->const_missing.erase(std::remove(e->const_missing.begin(), e->const_missing.end(), op), e->const_missing.end());
+  e->model_loaded = e->params_loaded && e->const_missing.empty();
   return BRE_OK;
 }
 

@@ -309,6 +309,210 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(int sweep, const
   }
 }
 
+// ---- multi-head self-attention, head split over a thread-block cluster ---------------------------------------------
+// For heads too wide for one CTA (the reference's transformer1: one head of 200, transformerS: one head of 512).  Grid
+// (B * heads, 1, c), cluster (1, 1, c): CTA rank r owns the columns [r w, min(dh, (r + 1) w)), w = ceil(dh / c), of Q, K, V, of
+// their tangents and of dO / dO' (the last CTA takes the remainder).  Every contraction over the head width -- S, S' (F, TF) and
+// dP, dP' (B, TB) -- is formed by each CTA over its own columns, published in its shared memory and summed by every CTA over
+// the cluster in rank order through distributed shared memory: the same T x T values in every CTA, no atomics.  The softmax and
+// the row reductions of its derivatives then run replicated in every CTA, and each output column is a contraction over T of
+// data the CTA holds.  Rank 0 writes P / P' to global memory.  Operands and outputs per sweep as for attention_kernel.
+// Shared memory per CTA: 8 T w floats (row stride w | 1: odd, so that lanes reading different rows hit different banks) and
+// 6 T^2 floats (P, three T x T scratch matrices, two partial sums).
+__host__ __device__ __forceinline__ int att_cluster_width(int dh, int c) { return (dh + c - 1) / c; }
+__host__ __device__ __forceinline__ int att_cluster_ld(int dh, int c) { return att_cluster_width(dh, c) | 1; }
+inline size_t att_cluster_smem(int T, int dh, int c) { return (size_t)(8LL * T * att_cluster_ld(dh, c) + 6LL * T * T) * sizeof(float); }
+
+template <bool kRound>
+__global__ void __launch_bounds__(ATT_THREADS) attention_cluster_kernel(int sweep, const float* __restrict__ qkv, const float* __restrict__ in1,
+                                                                      const float* __restrict__ in2, const float* __restrict__ in3, int T,
+                                                                      int heads, int dh, float* __restrict__ P, float* __restrict__ Pd,
+                                                                      float* __restrict__ out, int accumulate) {
+  constexpr bool round_out = kRound;
+  pdl_prologue();
+  extern __shared__ float sm[];
+  const int b = blockIdx.x / heads, h = blockIdx.x % heads;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = ATT_THREADS / 32;
+  const int rank = (int)cluster_rank(), nc = (int)cluster_size();
+  const int d = heads * dh;
+  const int wmax = att_cluster_width(dh, nc), ld = att_cluster_ld(dh, nc);
+  const int c0 = min(dh, rank * wmax), w = min(dh, c0 + wmax) - c0;   // this CTA's columns of the head
+  const float scale = 1.0f / sqrtf((float)dh);
+  const int TT = T * T;
+  float* sQ = sm;                 // [T][ld]
+  float* sK = sQ + T * ld;
+  float* sV = sK + T * ld;
+  float* sA = sV + T * ld;        // dO (B)  /  Q' (TF, TB)
+  float* sB = sA + T * ld;        // K'
+  float* sC = sB + T * ld;        // V'
+  float* sdO = sC + T * ld;       // dO  (TB)
+  float* sdOd = sdO + T * ld;     // dO' (TB)
+  float* sP = sdOd + T * ld;      // [T][T]
+  float* sM = sP + TT;            // dS (B) / P' (TF, TB)
+  float* sN = sM + TT;            // dS' (TB)
+  float* sdS = sN + TT;           // dS  (TB)
+  float* sR = sdS + TT;           // [2][T][T] this CTA's partial contractions
+  const long long row0 = (long long)b * T;
+  const long long pb = (long long)blockIdx.x * TT;
+  const int hc = h * dh + c0;     // first global column of this CTA within a [rows, d] third
+  auto load_qkv = [&](const float* src, float* q, float* k, float* v) {
+    for (int e = tid; e < T * w; e += ATT_THREADS) {
+      const int i = e / w, c = e - i * w;
+      const float* r = src + (row0 + i) * 3 * d + hc + c;
+      q[i * ld + c] = r[0]; k[i * ld + c] = r[d]; v[i * ld + c] = r[2 * d];
+    }
+  };
+  auto load_rows = [&](const float* src, float* dst) {
+    for (int e = tid; e < T * w; e += ATT_THREADS) {
+      const int i = e / w, c = e - i * w;
+      dst[i * ld + c] = src[(row0 + i) * d + hc + c];
+    }
+  };
+  auto dot = [&](const float* x, const float* y) {
+    float s = 0.f;
+    for (int c = 0; c < w; ++c) s = fmaf(x[c], y[c], s);
+    return s;
+  };
+  // the partials of sR[0 .. n T^2) summed over the cluster in rank order into dst0 (and dst1)
+  auto cluster_sum = [&](int n, float* dst0, float* dst1) {
+    cluster_barrier();                          // every CTA's partials are published
+    for (int e = tid; e < n * TT; e += ATT_THREADS) {
+      float s = 0.f;
+      for (int r = 0; r < nc; ++r) s += ld_cluster_f32(sR + e, (unsigned)r);
+      if (e < TT) dst0[e] = s; else dst1[e - TT] = s;
+    }
+    cluster_barrier();                          // every peer has read them: sR may be rewritten and the CTA may retire
+  };
+  auto store_qkv_grad = [&](int i, int c, float dq, float dk, float dv) {
+    float* o = out + (row0 + i) * 3 * d + hc + c;
+    const float vq = dq * scale, vk = dk * scale;
+    const float rq = accumulate ? o[0] + vq : vq, rk = accumulate ? o[d] + vk : vk, rv = accumulate ? o[2 * d] + dv : dv;
+    o[0] = round_out ? tf32_rna(rq) : rq;
+    o[d] = round_out ? tf32_rna(rk) : rk;
+    o[2 * d] = round_out ? tf32_rna(rv) : rv;
+  };
+  load_qkv(qkv, sQ, sK, sV);
+  if (sweep == 0) {
+    __syncthreads();
+    for (int e = tid; e < TT; e += ATT_THREADS) { const int i = e / T, j = e - i * T; sR[e] = dot(sQ + i * ld, sK + j * ld); }
+    cluster_sum(1, sP, nullptr);
+    for (int i = warp; i < T; i += nwarps) {                      // softmax of row i
+      float mx = -3.0e38f;
+      for (int j = lane; j < T; j += 32) { const float sc = sP[i * T + j] * scale; sP[i * T + j] = sc; mx = fmaxf(mx, sc); }
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      float den = 0.f;
+      for (int j = lane; j < T; j += 32) { const float e = expf(sP[i * T + j] - mx); sP[i * T + j] = e; den += e; }
+      den = warp_sum(den);
+      const float rden = 1.0f / den;
+      for (int j = lane; j < T; j += 32) {
+        const float p = sP[i * T + j] * rden;
+        sP[i * T + j] = p;
+        if (rank == 0) P[pb + i * T + j] = p;
+      }
+    }
+    __syncthreads();
+    for (int e = tid; e < T * w; e += ATT_THREADS) {              // O = P V
+      const int i = e / w, c = e - i * w;
+      float o = 0.f;
+      for (int j = 0; j < T; ++j) o = fmaf(sP[i * T + j], sV[j * ld + c], o);
+      out[(row0 + i) * d + hc + c] = round_out ? tf32_rna(o) : o;
+    }
+    return;
+  }
+  for (int e = tid; e < TT; e += ATT_THREADS) sP[e] = P[pb + e];
+  if (sweep == 1) {
+    load_rows(in1, sA);                                           // dO
+    __syncthreads();
+    for (int e = tid; e < TT; e += ATT_THREADS) { const int i = e / T, j = e - i * T; sR[e] = dot(sA + i * ld, sV + j * ld); }
+    cluster_sum(1, sM, nullptr);                                  // dP
+    for (int i = warp; i < T; i += nwarps) {                      // dS = P (dP - r), r = sum_j dP_ij P_ij
+      float r = 0.f;
+      for (int j = lane; j < T; j += 32) r = fmaf(sM[i * T + j], sP[i * T + j], r);
+      r = warp_sum(r);
+      for (int j = lane; j < T; j += 32) sM[i * T + j] = sP[i * T + j] * (sM[i * T + j] - r);
+    }
+    __syncthreads();
+    for (int e = tid; e < T * w; e += ATT_THREADS) {
+      const int i = e / w, c = e - i * w;
+      float dq = 0.f, dk = 0.f, dv = 0.f;
+      for (int j = 0; j < T; ++j) {
+        dq = fmaf(sM[i * T + j], sK[j * ld + c], dq);
+        dk = fmaf(sM[j * T + i], sQ[j * ld + c], dk);
+        dv = fmaf(sP[j * T + i], sA[j * ld + c], dv);
+      }
+      store_qkv_grad(i, c, dq, dk, dv);
+    }
+    return;
+  }
+  if (sweep == 2) {
+    load_qkv(in1, sA, sB, sC);                                    // Q', K', V'
+    __syncthreads();
+    for (int e = tid; e < TT; e += ATT_THREADS) {
+      const int i = e / T, j = e - i * T;
+      sR[e] = dot(sA + i * ld, sK + j * ld) + dot(sQ + i * ld, sB + j * ld);
+    }
+    cluster_sum(1, sM, nullptr);                                  // S' / scale
+    for (int i = warp; i < T; i += nwarps) {                      // P' = P (S' - sum_j P S')
+      float acc = 0.f;
+      for (int j = lane; j < T; j += 32) { const float sd = sM[i * T + j] * scale; sM[i * T + j] = sd; acc = fmaf(sP[i * T + j], sd, acc); }
+      acc = warp_sum(acc);
+      for (int j = lane; j < T; j += 32) {
+        const float pd = sP[i * T + j] * (sM[i * T + j] - acc);
+        sM[i * T + j] = pd;
+        if (rank == 0) Pd[pb + i * T + j] = pd;
+      }
+    }
+    __syncthreads();
+    for (int e = tid; e < T * w; e += ATT_THREADS) {              // O' = P' V + P V'
+      const int i = e / w, c = e - i * w;
+      float o = 0.f;
+      for (int j = 0; j < T; ++j) o += sM[i * T + j] * sV[j * ld + c] + sP[i * T + j] * sC[j * ld + c];
+      out[(row0 + i) * d + hc + c] = round_out ? tf32_rna(o) : o;
+    }
+    return;
+  }
+  // sweep 3: tangent backward
+  float* sQd = sA; float* sKd = sB; float* sVd = sC;
+  load_qkv(in3, sQd, sKd, sVd);
+  float* sPd = sM;
+  for (int e = tid; e < TT; e += ATT_THREADS) sPd[e] = Pd[pb + e];
+  load_rows(in2, sdO);
+  load_rows(in1, sdOd);
+  __syncthreads();
+  for (int e = tid; e < TT; e += ATT_THREADS) {
+    const int i = e / T, j = e - i * T;
+    sR[e] = dot(sdO + i * ld, sV + j * ld);                                                     // dP
+    sR[TT + e] = dot(sdOd + i * ld, sV + j * ld) + dot(sdO + i * ld, sVd + j * ld);             // dP'
+  }
+  cluster_sum(2, sdS, sN);
+  for (int i = warp; i < T; i += nwarps) {                        // dS, dS' of row i
+    float r = 0.f, rd = 0.f;
+    for (int j = lane; j < T; j += 32) {
+      const float dp = sdS[i * T + j], dpd = sN[i * T + j];
+      r = fmaf(dp, sP[i * T + j], r);
+      rd += dpd * sP[i * T + j] + dp * sPd[i * T + j];
+    }
+    r = warp_sum(r);
+    rd = warp_sum(rd);
+    for (int j = lane; j < T; j += 32) {
+      const float dp = sdS[i * T + j], dpd = sN[i * T + j];
+      sN[i * T + j] = sPd[i * T + j] * (dp - r) + sP[i * T + j] * (dpd - rd);   // dS'
+      sdS[i * T + j] = sP[i * T + j] * (dp - r);                               // dS
+    }
+  }
+  __syncthreads();
+  for (int e = tid; e < T * w; e += ATT_THREADS) {
+    const int i = e / w, c = e - i * w;
+    float dq = 0.f, dk = 0.f, dv = 0.f;
+    for (int j = 0; j < T; ++j) {
+      dq += sN[i * T + j] * sK[j * ld + c] + sdS[i * T + j] * sKd[j * ld + c];
+      dk += sN[j * T + i] * sQ[j * ld + c] + sdS[j * T + i] * sQd[j * ld + c];
+      dv += sPd[j * T + i] * sdO[j * ld + c] + sP[j * T + i] * sdOd[j * ld + c];
+    }
+    store_qkv_grad(i, c, dq, dk, dv);
+  }
+}
+
 // ---- positional embedding ------------------------------------------------------------------------------------------
 template <bool kRound>
 __global__ void posadd_kernel(const float* __restrict__ x, const float* __restrict__ pos, float* __restrict__ out, long long total, int C, int T) {
@@ -552,26 +756,58 @@ int launch_token_ln_param_grad(const float* x, const float* dy, const float* sta
   if (lerr != cudaSuccess) { set_error(std::string("token layernorm parameter gradient: ") + cudaGetErrorString(lerr)); return -2; }
   return check_launch("token layernorm parameter gradient");
 }
+int token_attention_plan(int T, int dh, int cluster) {
+  const size_t resident = (size_t)(8LL * T * dh + 4LL * T * T) * sizeof(float);
+  if (cluster == 0) {
+    if (resident <= kAttSmemLimit) return 1;
+    for (int c = 2; c <= kRowClusterMax && c <= dh; ++c)
+      if (att_cluster_smem(T, dh, c) <= kAttSmemLimit) return c;
+    return -1;
+  }
+  if (cluster < 1 || cluster > kRowClusterMax) return -1;
+  return (cluster == 1 ? resident : att_cluster_smem(T, dh, cluster)) <= kAttSmemLimit ? cluster : -1;
+}
+
 int launch_token_attention(int sweep, const float* qkv, const float* in1, const float* in2, const float* in3, int B, int T, int heads, int dh,
-                           float* P, float* Pd, float* out, int accumulate, bool round_out, cudaStream_t s) {
-  // the whole head stays resident in shared memory (8 T dh + 4 T^2 floats) under the 200 KB opt-in; longer sequences need a tiled kernel
-  const size_t smem = (size_t)(8LL * T * dh + 4LL * T * T) * sizeof(float);
-  if (smem > kAttSmemLimit) {
-    set_error("token attention: seq_len " + std::to_string(T) + " with head size " + std::to_string(dh) + " needs " + std::to_string(smem) +
-              " B of shared memory, over the " + std::to_string(kAttSmemLimit) + " B opt-in limit of the resident-head kernel");
+                           float* P, float* Pd, float* out, int accumulate, bool round_out, cudaStream_t s, int cluster) {
+  // a head resident in one CTA's shared memory (8 T dh + 4 T^2 floats) under the 200 KB opt-in when it fits; otherwise split over the
+  // columns of the smallest cluster whose CTAs fit (the T x T working set stays whole in every CTA: longer sequences need a tiled kernel)
+  const int c = token_attention_plan(T, dh, cluster);
+  if (c < 0) {
+    const size_t resident = (size_t)(8LL * T * dh + 4LL * T * T) * sizeof(float);
+    const int cc = cluster > 1 ? cluster : kRowClusterMax;
+    if (cluster < 0 || cluster > kRowClusterMax) {
+      set_error("token attention: cluster size " + std::to_string(cluster) + " is not in 0 (automatic) .. " + std::to_string(kRowClusterMax));
+    } else if (cluster == 1) {
+      set_error("token attention: seq_len " + std::to_string(T) + " with head size " + std::to_string(dh) + " needs " + std::to_string(resident) +
+                " B of shared memory, over the " + std::to_string(kAttSmemLimit) + " B opt-in limit of the resident-head kernel");
+    } else {
+      set_error("token attention: seq_len " + std::to_string(T) + " with head size " + std::to_string(dh) + " needs " + std::to_string(resident) +
+                " B of shared memory, over the " + std::to_string(kAttSmemLimit) + " B opt-in limit of the resident-head kernel; split over " +
+                std::to_string(cc) + " CTAs it needs " + std::to_string(att_cluster_smem(T, dh, cc)) + " B per CTA");
+    }
     return -4;
   }
   static bool attr_done = false;
   if (!attr_done) {
     if (cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmemLimit) != cudaSuccess ||
-        cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmemLimit) != cudaSuccess) {
+        cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmemLimit) != cudaSuccess ||
+        cudaFuncSetAttribute(attention_cluster_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmemLimit) != cudaSuccess ||
+        cudaFuncSetAttribute(attention_cluster_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttSmemLimit) != cudaSuccess) {
       set_error("token attention: shared memory opt-in failed");
       return -2;
     }
     attr_done = true;
   }
-  const cudaError_t lerr = launch_kernel(round_out ? attention_kernel<true> : attention_kernel<false>, dim3(B * heads), dim3(ATT_THREADS), smem, s, 1, sweep,
-                                         qkv, in1, in2, in3, T, heads, dh, P, Pd, out, accumulate);
+  cudaError_t lerr;
+  if (c == 1) {
+    const size_t smem = (size_t)(8LL * T * dh + 4LL * T * T) * sizeof(float);
+    lerr = launch_kernel(round_out ? attention_kernel<true> : attention_kernel<false>, dim3(B * heads), dim3(ATT_THREADS), smem, s, 1, sweep,
+                         qkv, in1, in2, in3, T, heads, dh, P, Pd, out, accumulate);
+  } else {
+    lerr = launch_kernel(round_out ? attention_cluster_kernel<true> : attention_cluster_kernel<false>, dim3(B * heads, 1, c), dim3(ATT_THREADS),
+                         att_cluster_smem(T, dh, c), s, c, sweep, qkv, in1, in2, in3, T, heads, dh, P, Pd, out, accumulate);
+  }
   if (lerr != cudaSuccess) { set_error(std::string("token attention: ") + cudaGetErrorString(lerr)); return -2; }
   return check_launch("token attention");
 }
@@ -755,7 +991,27 @@ int bre_token_attention(int32_t sweep, const float* qkv, const float* in1, const
     set_error("bre_token_attention: bad arguments");
     return -1;
   }
-  return launch_token_attention(sweep, qkv, in1, in2, in3, B, T, heads, dh, P, Pd, out, 0, round_out != 0, (cudaStream_t)stream);
+  return launch_token_attention(sweep, qkv, in1, in2, in3, B, T, heads, dh, P, Pd, out, 0, round_out != 0, (cudaStream_t)stream, 0);
+}
+
+// The same with the kernel chosen by the caller: cluster = 0 picks as bre_token_attention does, 1 runs the resident-head kernel,
+// 2 .. 8 split the head over that many CTAs.
+int bre_token_attention_ex(int32_t sweep, const float* qkv, const float* in1, const float* in2, const float* in3, int32_t B, int32_t T,
+                           int32_t heads, int32_t dh, float* P, float* Pd, float* out, int32_t round_out, void* stream, int32_t cluster) {
+  using namespace bre;
+  if (!qkv || !out || !P || B < 1 || T < 1 || heads < 1 || dh < 1 || sweep < 0 || sweep > 3) {
+    set_error("bre_token_attention_ex: bad arguments");
+    return -1;
+  }
+  return launch_token_attention(sweep, qkv, in1, in2, in3, B, T, heads, dh, P, Pd, out, 0, round_out != 0, (cudaStream_t)stream, cluster);
+}
+
+// CTAs per (sequence, head) that the attention sweeps run with for this shape (1 = the resident-head kernel), or -1 when refused.
+int bre_token_attention_plan(int32_t T, int32_t dh, int32_t cluster, int32_t* ctas) {
+  using namespace bre;
+  if (!ctas || T < 1 || dh < 1) { set_error("bre_token_attention_plan: bad arguments"); return -1; }
+  *ctas = token_attention_plan(T, dh, cluster);
+  return 0;
 }
 
 }  // extern "C"

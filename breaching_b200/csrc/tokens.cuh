@@ -12,8 +12,12 @@ int launch_token_layernorm(int sweep, const float* x, const float* in1, const fl
                            int accumulate, bool round_out, cudaStream_t s);
 int launch_token_ln_param_grad(const float* x, const float* dy, const float* stats, int rows, int C, float* g_gamma, float* g_beta,
                                cudaStream_t s);
+// cluster: 0 = the resident-head kernel when the head fits one CTA, else the smallest cluster (2 .. 8 CTAs) whose column slices fit;
+// 1 = the resident-head kernel; 2 .. 8 = the head split over that many CTAs.  A shape that does not fit is refused (-4).
 int launch_token_attention(int sweep, const float* qkv, const float* in1, const float* in2, const float* in3, int B, int T, int heads, int dh,
-                           float* P, float* Pd, float* out, int accumulate, bool round_out, cudaStream_t s);
+                           float* P, float* Pd, float* out, int accumulate, bool round_out, cudaStream_t s, int cluster = 0);
+// the CTAs per (sequence, head) launch_token_attention runs with for (T, dh, cluster), -1 = refused
+int token_attention_plan(int T, int dh, int cluster);
 // out[row] = (x ? x[row] : 0) + pos[row mod T]      (learnable positional embedding, language_models.py:133-146)
 int launch_token_posadd(const float* x, const float* pos, float* out, int rows, int C, int T, bool round_out, cudaStream_t s);
 // g_pos[t] = sum over sequences of d[b*T + t]        (rows t >= T of the embedding table keep a zero gradient)

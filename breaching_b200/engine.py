@@ -99,7 +99,8 @@ EXPORTS = [
     "bre_engine_debug_step_param", "bre_engine_debug_tensor", "bre_engine_debug_op", "bre_engine_launches_per_iteration", "bre_engine_set_option", "bre_match_reduce",
     "bre_total_variation", "bre_conv_gemm", "bre_last_error", "bre_version",
     "bre_engine_load_soft_labels", "bre_engine_label_gradient", "bre_engine_set_labels",
-    "bre_token_layernorm", "bre_token_attention", "bre_token_match",
+    "bre_token_layernorm", "bre_token_attention", "bre_token_match", "bre_token_attention_ex", "bre_token_attention_plan",
+    "bre_engine_load_constant",
     "bre_engine_param_gradients", "bre_engine_bn_batch_stats", "bre_engine_forward", "bre_image_mse",
     "bre_engine_begin_joint_trial", "bre_engine_get_joint_labels", "bre_resize_bilinear",
     "bre_engine_set_augmentations", "bre_engine_last_augmentation", "bre_augment_view",
@@ -157,6 +158,9 @@ def load_library(path=None):
     lib.bre_conv_gemm.argtypes = [i32, i32, vp, vp, vp, vp, vp] + [i32] * 9 + [vp]
     lib.bre_token_layernorm.argtypes = [i32, vp, vp, vp, vp, vp, vp, vp, vp, f32, i32, i32, vp, vp, vp, vp, i32, vp]
     lib.bre_token_attention.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, i32, vp]
+    lib.bre_token_attention_ex.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, i32, vp, i32]
+    lib.bre_token_attention_plan.argtypes = [i32, i32, i32, P(i32)]
+    lib.bre_engine_load_constant.argtypes = [vp, i32, vp, i64]
     lib.bre_token_match.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp]
     lib.bre_engine_begin_joint_trial.argtypes = [vp, vp, vp, i64, vp, i32]
     lib.bre_engine_get_joint_labels.argtypes = [vp, i32, vp]
@@ -380,6 +384,11 @@ class Engine:
         pa, ma, va = self._ptr_array(params), self._ptr_array(means), self._ptr_array(vars_)
         rc = self.lib.bre_engine_load_model(self.h, pa, len(params), ma, va, len(mods))
         _check(self.lib, rc, "bre_engine_load_model")
+        for i, op in enumerate(self.prog.ops):   # constant tables of the program (the fixed positional encoding)
+            if op.kind == C.OP_POSCONST:
+                table = _f32c(op.table)
+                rc = self.lib.bre_engine_load_constant(self.h, i, _ptr(table), table.numel())
+                _check(self.lib, rc, "bre_engine_load_constant")
 
     def load_targets(self, gradients, labels, mean=None, std=None, tensor_weights=None):
         grads = [_f32c(g) for g in gradients]
@@ -980,15 +989,29 @@ def token_match(rec, emb, subset=None):
     return out
 
 
-def token_attention(sweep, qkv, B, T, heads, P, Pd, in1=None, in2=None, in3=None, round_out=False):
+def token_attention(sweep, qkv, B, T, heads, P, Pd, in1=None, in2=None, in3=None, round_out=False, cluster=None):
     """Stand-alone multi-head self-attention sweep (csrc/tokens.cu); qkv [B*T, 3 d].  ``round_out``: store ``out`` on the TF32
-    grid.  A head that does not fit the kernel's shared memory (8 T dh + 4 T^2 floats over 200 KB) raises."""
+    grid.  ``cluster``: None or 0 = the engine's choice (the resident-head kernel when 8 T dh + 4 T^2 floats fit 200 KB of shared
+    memory, else the head split over the smallest cluster of CTAs whose column slices fit), 1 = the resident-head kernel, 2 .. 8 =
+    the head split over that many CTAs.  A shape no kernel holds raises."""
     lib = load_library()
     d = qkv.shape[1] // 3
     out = torch.empty(qkv.shape[0], d if sweep in (0, 2) else 3 * d, device=qkv.device)
     stream = torch.cuda.current_stream(qkv.device).cuda_stream
+    args = (sweep, _ptr(qkv), _ptr(in1), _ptr(in2), _ptr(in3), B, T, heads, d // heads, _ptr(P), _ptr(Pd), _ptr(out), int(bool(round_out)),
+            ctypes.c_void_p(stream))
     with torch.cuda.device(qkv.device):
-        rc = lib.bre_token_attention(sweep, _ptr(qkv), _ptr(in1), _ptr(in2), _ptr(in3), B, T, heads, d // heads, _ptr(P), _ptr(Pd), _ptr(out),
-                                     int(bool(round_out)), ctypes.c_void_p(stream))
+        if cluster is None:
+            rc = lib.bre_token_attention(*args)
+        else:
+            rc = lib.bre_token_attention_ex(*args, int(cluster))
     _check(lib, rc, "bre_token_attention")
     return out
+
+
+def token_attention_plan(T, dh, cluster=0):
+    """CTAs per (sequence, head) the attention sweeps run with (1 = the resident-head kernel), or None when the shape is refused."""
+    lib = load_library()
+    n = ctypes.c_int32()
+    _check(lib, lib.bre_token_attention_plan(int(T), int(dh), int(cluster), ctypes.byref(n)), "bre_token_attention_plan")
+    return None if n.value < 0 else n.value

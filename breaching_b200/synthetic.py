@@ -226,18 +226,48 @@ def make_multi_query_case(model_name="convnet-tiny", data="cifar", batch=1, seed
     return model, loss_fn, payload, shared, true
 
 
+class SinusoidalPositions(torch.nn.Module):
+    """Fixed positional encoding of the reference's ``PositionalEmbedding`` (language_models.py:89-130, dropout 0): the constant
+    buffer ``pe`` [1, max_len, d] holds sin(t w_i) in the even and cos(t w_i) in the odd columns, w_i = 10000^(-2i/d), computed
+    in float32 as the reference computes it; the module adds ``pe[:, :T]`` and has no parameters."""
+
+    def __init__(self, d, max_len=5000):
+        super().__init__()
+        import math
+
+        t = torch.arange(0, max_len, dtype=torch.float).unsqueeze(1)
+        freq = torch.exp(torch.arange(0, d, 2).float() * (-math.log(10000.0) / d))
+        pe = torch.zeros(max_len, d)
+        pe[:, 0::2] = torch.sin(t * freq)
+        pe[:, 1::2] = torch.cos(t * freq)
+        self.dropout = torch.nn.Dropout(p=0.0)
+        self.register_buffer("pe", pe.unsqueeze(0))
+
+    def forward(self, x):
+        return self.dropout(x + self.pe[:, : x.shape[1], :])
+
+
 class TransformerLM(torch.nn.Module):
     """Architecture of the reference's ``TransformerModel`` (cases/models/language_models.py:150-205, BASELINE config 5:
     ntokens 50257, ninp 96, nhead 8, nhid 1536, nlayers 3, dropout 0, learnable positional embedding): token embedding
     (scaled by sqrt(ninp) at init), positional embedding added, ``nn.TransformerEncoder`` of post-norm ReLU layers
-    (batch first, no mask), linear decoder.  Module names follow the reference so that ``parameters()`` has its order."""
+    (batch first, no mask), linear decoder.  Module names follow the reference so that ``parameters()`` has its order.
+    ``positional="fixed"``: the sinusoidal ``pos_encoder.pe`` buffer of the reference's fixed presets (transformer3f, transformer1,
+    transformerS) instead of the learnable ``pos_encoder.embedding``; ``max_positions`` is then the buffer's length (the
+    reference's 5000 by default)."""
 
-    def __init__(self, ntokens=50257, ninp=96, nhead=8, nhid=1536, nlayers=3, max_positions=1024):
+    def __init__(self, ntokens=50257, ninp=96, nhead=8, nhid=1536, nlayers=3, max_positions=None, positional="learnable"):
         super().__init__()
         import math
 
-        self.pos_encoder = torch.nn.Module()
-        self.pos_encoder.embedding = torch.nn.Embedding(max_positions, ninp)
+        if positional == "learnable":
+            self.pos_encoder = torch.nn.Module()
+            self.pos_encoder.embedding = torch.nn.Embedding(max_positions or 1024, ninp)
+        elif positional == "fixed":
+            self.pos_encoder = SinusoidalPositions(ninp, max_positions or 5000)
+        else:
+            raise ValueError(f"unknown positional embedding {positional}")
+        self.positional = positional
         layer = torch.nn.TransformerEncoderLayer(ninp, nhead, nhid, 0.0, batch_first=True)
         self.transformer_encoder = torch.nn.TransformerEncoder(layer, nlayers, enable_nested_tensor=False)
         self.encoder = torch.nn.Embedding(ntokens, ninp)
@@ -248,7 +278,7 @@ class TransformerLM(torch.nn.Module):
 
     @property
     def pos_embedding(self):
-        return self.pos_encoder.embedding
+        return self.pos_encoder.embedding if self.positional == "learnable" else None
 
     @property
     def layers(self):
@@ -261,8 +291,11 @@ class TransformerLM(torch.nn.Module):
 
     def forward(self, input_ids=None, inputs_embeds=None):
         inputs = self.encoder(input_ids) if inputs_embeds is None else inputs_embeds
-        positions = torch.arange(inputs.shape[1], device=inputs.device)
-        inputs = inputs + self.pos_encoder.embedding(positions[None, :])
+        if self.positional == "fixed":
+            inputs = self.pos_encoder(inputs)
+        else:
+            positions = torch.arange(inputs.shape[1], device=inputs.device)
+            inputs = inputs + self.pos_encoder.embedding(positions[None, :])
         return self.decoder(self.transformer_encoder(inputs))
 
 
@@ -282,12 +315,14 @@ class CausalLoss(torch.nn.Module):
         return causal_loss(outputs, labels)
 
 
-def make_text_case(batch=1, seq_len=8, seed=233, ntokens=50, ninp=16, nhead=4, nhid=24, nlayers=2):
+def make_text_case(batch=1, seq_len=8, seed=233, ntokens=50, ninp=16, nhead=4, nhid=24, nlayers=2, positional="learnable"):
     """BASELINE config 5 in miniature: a causal language model user (cases/data/datasets_text.py token batches, users.py
     single step) on ``TransformerLM``.  Returns ``(model, loss_fn, server_payload, shared_data, true_user_data)``; the shared
-    gradient list includes the token-embedding entry (the attack removes it, base_attack.py:88-95)."""
+    gradient list includes the token-embedding entry (the attack removes it, base_attack.py:88-95).  ``positional="fixed"``:
+    the sinusoidal positions of the reference's transformer3f / transformer1 / transformerS (a buffer, no gradient entry)."""
     torch.manual_seed(seed)
-    model = TransformerLM(ntokens, ninp, nhead, nhid, nlayers, max_positions=max(64, seq_len)).eval()
+    max_pos = max(64, seq_len) if positional == "learnable" else None
+    model = TransformerLM(ntokens, ninp, nhead, nhid, nlayers, max_positions=max_pos, positional=positional).eval()
     gen = torch.Generator().manual_seed(seed + 7)
     with torch.no_grad():  # non-trivial LayerNorm parameters / biases
         for p in model.parameters():
@@ -298,7 +333,7 @@ def make_text_case(batch=1, seq_len=8, seed=233, ntokens=50, ninp=16, nhead=4, n
     params = [p for p in model.parameters()]
     grads = torch.autograd.grad(loss_fn(model(tokens), tokens), params)
     meta = DataConfig(name="synthetic-text", modality="text", task="causal-lm", vocab_size=ntokens, shape=(seq_len,), classes=ntokens)
-    server_payload = [dict(parameters=params, buffers=[], metadata=meta)]
+    server_payload = [dict(parameters=params, buffers=[b for b in model.buffers()], metadata=meta)]
     shared_data = [dict(gradients=[g.detach().clone() for g in grads], buffers=None,
                         metadata=dict(num_data_points=batch, labels=None, local_hyperparams=None))]
     return model, loss_fn, server_payload, shared_data, dict(data=tokens, labels=tokens)

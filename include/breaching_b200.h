@@ -40,7 +40,9 @@ enum bre_op_kind { BRE_OP_CONV = 1, BRE_OP_BNACT = 2, BRE_OP_MAXPOOL = 3, BRE_OP
                    /* token-sequence programs (transformer / TAG path): tensors are [rows = batch * seq_len, C, 1, 1] */
                    BRE_OP_POSADD = 6,      /* out = candidate + positional embedding `w` of position (row mod seq_len) */
                    BRE_OP_LAYERNORM = 7,   /* gamma, beta, eps */
-                   BRE_OP_ATTENTION = 8 }; /* tin = fused (q | k | v) projection, R = heads, S = seq_len, no mask */
+                   BRE_OP_ATTENTION = 8,   /* tin = fused (q | k | v) projection, R = heads, S = seq_len, no mask */
+                   BRE_OP_POSCONST = 9 };  /* out = candidate + constant table [S, C] of position (row mod S), w = -1: the fixed
+                                              sinusoidal positions (no parameter; table from bre_engine_load_constant) */
 enum bre_param_perm { BRE_PERM_NONE = 0, BRE_PERM_OIHW_TO_OHWI = 1, BRE_PERM_LINEAR_CHW_TO_HWC = 2 };
 
 typedef struct bre_tensor_desc { int32_t N, C, H, W; } bre_tensor_desc; /* tensor 0 = candidate (NCHW) */
@@ -111,6 +113,9 @@ void bre_engine_destroy(bre_engine* e);
  * Pointers: device or host. */
 int bre_engine_load_model(bre_engine* e, const float* const* params, int32_t n_params,
                           const float* const* bn_mean, const float* const* bn_var, int32_t n_bn);
+/* The constant table of op `op` (a BRE_OP_POSCONST op: [S, C] fp32, numel = S * C; device or host), a buffer of the model such as
+ * the reference's PositionalEmbedding.pe[0, :S].  Every such op needs its table before the first evaluation. */
+int bre_engine_load_constant(bre_engine* e, int32_t op, const float* table, int64_t numel);
 
 /* The user's shared gradient (shared_data[i]["gradients"], users.py:176-186), same order/layout as params,
  * per-tensor TAG weights (objectives.py:115-124; NULL = all ones), labels (int64, [N]),
@@ -365,12 +370,20 @@ int bre_langevin_noise(uint64_t seed, uint32_t trial, uint32_t it, uint64_t firs
  *   attention: qkv [rows, 3 d] = (q | k | v) projections, heads x dh = d, no mask; in1..in3 per sweep: (1) dO [rows, d] |
  *              (2) (qkv)' | (3) dO', dO, (qkv)'; P / Pd [B, heads, T, T] are written by sweeps 0 / 2 and read later.
  * round_out != 0 stores `out` on the TF32 grid (cvt.rna), as the engine does for the operands of tensor-core GEMMs.  The attention
- * kernel keeps a whole head in shared memory: 8 T dh + 4 T^2 floats must fit in 200 KB, otherwise the call fails (-4). */
+ * sweeps keep a whole head in one CTA's shared memory when 8 T dh + 4 T^2 floats fit in 200 KB; a wider head is split by columns
+ * over the smallest thread-block cluster of c <= 8 CTAs whose slices fit (8 T (ceil(dh / c) | 1) + 6 T^2 floats per CTA, the
+ * contractions over dh reduced through distributed shared memory in rank order); otherwise the call fails (-4). */
 int bre_token_layernorm(int32_t sweep, const float* x, const float* in1, const float* in2, const float* in3, const float* gamma,
                         const float* beta, const float* v_gamma, const float* v_beta, float eps, int32_t rows, int32_t C, float* stats,
                         float* out, float* g_gamma, float* g_beta, int32_t round_out, void* stream);
 int bre_token_attention(int32_t sweep, const float* qkv, const float* in1, const float* in2, const float* in3, int32_t B, int32_t T,
                         int32_t heads, int32_t dh, float* P, float* Pd, float* out, int32_t round_out, void* stream);
+/* The attention sweeps with the kernel chosen by the caller: cluster = 0 picks as bre_token_attention does, 1 = the resident-head
+ * kernel, 2 .. 8 = the head split over that many CTAs (the last takes the remainder of dh); -4 when that kernel does not fit. */
+int bre_token_attention_ex(int32_t sweep, const float* qkv, const float* in1, const float* in2, const float* in3, int32_t B, int32_t T,
+                           int32_t heads, int32_t dh, float* P, float* Pd, float* out, int32_t round_out, void* stream, int32_t cluster);
+/* Host only: *ctas = the CTAs per (sequence, head) that bre_token_attention_ex(.., cluster) runs with (1 = resident), -1 = refused. */
+int bre_token_attention_plan(int32_t T, int32_t dh, int32_t cluster, int32_t* ctas);
 
 /* Token recovery of the text attacks (replaces `_postprocess_text_data._max_similarity`, breaching/attacks/base_attack.py:126-133):
  * tokens[n] = argmax_v <r_n - mean, e_v - mean> / |r_n - mean|^2 / |e_v - mean|^2 over the V rows of emb [*, d] (rows picked through
