@@ -205,19 +205,22 @@ class OptimizationJointAttacker(OptimizationBasedAttacker):
 
     def _run_joint_trial(self, engine, candidate, candidate_labels, stats, trial, dryrun=False, iterations=None):
         """optimization_with_label_attack.py:89-143.  Adam / AdamW / SGD trials run entirely on the device (both leaves stepped
-        by the engine's fused kernels from one CUDA graph, ``bre_engine_begin_joint_trial``); L-BFGS -- which branches on a few
-        scalars per inner iteration -- and engine stand-ins without that entry point are driven from the host."""
+        by the engine's fused kernels from one CUDA graph, ``bre_engine_begin_joint_trial``), and so do L-BFGS trials of
+        classification models without augmentations or Langevin noise (``bre_engine_begin_lbfgs_trial``); token models with L-BFGS
+        and engine stand-ins without those entry points are driven from the host."""
         opt = self.cfg.optim
         T = int(opt.max_iterations)
         table = lr_table(opt.step_size, cfg_get(opt, "step_size_decay"), cfg_get(opt, "warmup", 0), T)
-        if str(opt.optimizer).lower() in _OPTIMIZERS and hasattr(engine, "begin_joint_trial") and not getattr(self, "host_driven", False):
+        name = str(opt.optimizer).lower()
+        if not getattr(self, "host_driven", False) and (
+                (name in _OPTIMIZERS and hasattr(engine, "begin_joint_trial"))
+                or (name == "l-bfgs" and candidate_labels.dim() == 2 and self._lbfgs_on_device(engine))):
             return self._run_joint_trial_device(engine, candidate, candidate_labels, stats, trial, table, dryrun, iterations)
         x = candidate.detach().clone().contiguous()
         ell = candidate_labels.detach().clone().contiguous()
         best, best_l, fmin = x.clone(), ell.clone(), float("inf")
         dm, ds = self.dm.to(x.device), self.ds.to(x.device)
         lo, hi = -dm / ds, (1 - dm) / ds
-        name = str(opt.optimizer).lower()
         if name == "l-bfgs":
             flat = torch.cat([x.view(-1), ell.view(-1)])   # torch's L-BFGS treats all leaves as one flat vector
             x, ell = flat[: x.numel()].view_as(x), flat[x.numel():].view_as(ell)
@@ -258,7 +261,10 @@ class OptimizationJointAttacker(OptimizationBasedAttacker):
         if candidate_labels.dim() == 3:      # token models: the engine works on rows = batch * seq_len
             x = x.reshape(-1, x.shape[-1], 1, 1)
         clock, t0 = self.last_timing, time.perf_counter()
-        engine.begin_joint_trial(x, candidate_labels.detach().contiguous(), table, trial=trial)
+        if str(self.cfg.optim.optimizer).lower() == "l-bfgs":   # data and labels as one flat vector, as torch's L-BFGS sees them
+            engine.begin_lbfgs_trial(x, table, label_logits=candidate_labels.detach().contiguous(), trial=trial)
+        else:
+            engine.begin_joint_trial(x, candidate_labels.detach().contiguous(), table, trial=trial)
         clock["trial_begin"] = clock.get("trial_begin", 0.0) + time.perf_counter() - t0
         t0 = time.perf_counter()
         T = int(self.cfg.optim.max_iterations)

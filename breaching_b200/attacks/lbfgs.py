@@ -4,11 +4,15 @@ attacks/auxiliaries/common.py:18; used by the ``beyondinfering`` / ``wei`` / ``d
 The reference hands the closure of ``_compute_objective`` (optimization_based_attack.py:146-189) to torch's L-BFGS with
 its defaults -- 20 inner iterations and at most 25 closure evaluations per ``step``, history of 100 curvature pairs, no line
 search, ``tolerance_grad=1e-7``, ``tolerance_change=1e-9`` -- and the optimiser state persists over the outer iterations of
-``_run_trial``.  Here every closure evaluation is one pass of the CUDA engine (forward, gradient, matching objective,
-second backward: ``Engine.objective_and_gradient``); the direction update is the classic two-loop recursion over a ring of
-curvature pairs held in two ``[history, n]`` device buffers.  It is sequential by nature (each inner iteration needs a few
-scalar reductions on the host to take the same early exits as the reference), so it is driven from Python; the arithmetic
-that dominates -- the closure -- stays on the engine.
+``_run_trial``.
+
+Trials with one engine, no augmentations and no Langevin noise run on the device (``Engine.begin_lbfgs_trial``, csrc/lbfgs.cu):
+one captured graph per ``optimizer.step``, its inner loop a conditional WHILE node, the direction the two-loop recursion
+re-associated over Gram matrices of the ring, every scalar and early exit on the device.  The constants below are the ones it
+is given.  ``DeviceLBFGS`` is the host loop for the remaining cases (several model queries, augmentations, Langevin noise,
+token models) and the reference the device path is tested against: every closure evaluation is one pass of the CUDA engine
+(``Engine.objective_and_gradient``), the direction update the classic two-loop recursion over a ring of curvature pairs held in
+two ``[history, n]`` device buffers, driven from Python with a few host reductions per inner iteration.
 """
 import math
 

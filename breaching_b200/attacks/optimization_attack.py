@@ -247,9 +247,9 @@ class OptimizationBasedAttacker:
         T = int(opt.max_iterations)
         table = lr_table(opt.step_size, cfg_get(opt, "step_size_decay"), cfg_get(opt, "warmup", 0), T)
         name = str(opt.optimizer).lower()
-        if name == "l-bfgs" or isinstance(engine, _EngineSum):
-            # host-driven loops, every closure evaluation on the engine(s): L-BFGS (common.py:18), and multi-query attacks,
-            # whose candidate gradient is a sum over engines and cannot use one engine's fused on-device step
+        if (name == "l-bfgs" and not self._lbfgs_on_device(engine)) or isinstance(engine, _EngineSum):
+            # host-driven loops, every closure evaluation on the engine(s): L-BFGS (common.py:18) where the device loop does not
+            # apply, and multi-query attacks, whose candidate gradient is a sum over engines and cannot use one engine's fused step
             from . import augment, lbfgs
 
             if augment.has_view_stages(self.cfg):
@@ -258,12 +258,15 @@ class OptimizationBasedAttacker:
             best, history = lbfgs.run_trial(engine, candidate, self.cfg, table, -dm / ds, (1 - dm) / ds, dryrun)
             stats[f"Trial_{trial}_Val"].extend(history)
             return best.detach()
-        if hasattr(engine, "set_augmentations"):
-            plan = self._augmentation_plan(candidate)
-            if plan is not None or getattr(engine, "_aug_active", False):   # (re-setting invalidates the captured graph: only when needed)
-                engine.set_augmentations(plan)
-                engine._aug_active = plan is not None
-        engine.begin_trial(candidate, table, trial=trial)   # the global index: ranks sharing one noise seed still draw different fields
+        if name == "l-bfgs":   # one iteration = one optimizer.step, its inner loop inside the captured graph
+            engine.begin_lbfgs_trial(candidate, table, trial=trial)
+        else:
+            if hasattr(engine, "set_augmentations"):
+                plan = self._augmentation_plan(candidate)
+                if plan is not None or getattr(engine, "_aug_active", False):   # (re-setting invalidates the captured graph: only when needed)
+                    engine.set_augmentations(plan)
+                    engine._aug_active = plan is not None
+            engine.begin_trial(candidate, table, trial=trial)   # the global index: ranks sharing one noise seed still draw different fields
         callback = int(cfg_get(opt, "callback", 0) or 0)
         chunk = callback if callback > 0 else T
         total = 1 if dryrun else T
@@ -291,6 +294,12 @@ class OptimizationBasedAttacker:
         engine.sync()
         stats[f"Trial_{trial}_Val"].extend(engine.history().tolist())
         return engine.best().detach()
+
+    def _lbfgs_on_device(self, engine):
+        """L-BFGS trials run on the device with one engine, no augmentations and no Langevin noise; multi-query attacks, augmented
+        configs and Langevin noise keep the host loop of attacks/lbfgs.py."""
+        return (hasattr(engine, "begin_lbfgs_trial") and not isinstance(engine, _EngineSum) and not cfg_get(self.cfg, "augmentations")
+                and not float(cfg_get(self.cfg.optim, "langevin_noise", 0.0) or 0.0))
 
     def _augmentation_plan(self, candidate):
         """cfg.augmentations -> the engine's view pipeline (optimization_based_attack.py:42-48); colour constants are drawn once per

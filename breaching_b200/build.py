@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libbreaching_b200.so")
-SOURCES = ["engine.cu", "igemm_simt.cu", "igemm_tc.cu", "layers.cu", "objective.cu", "tokens.cu", "analysis.cu", "linear_small.cu", "stem_cols.cu", "augment.cu"]
+SOURCES = ["engine.cu", "igemm_simt.cu", "igemm_tc.cu", "layers.cu", "objective.cu", "tokens.cu", "analysis.cu", "linear_small.cu", "stem_cols.cu", "augment.cu", "lbfgs.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
     "-Xcompiler", "-fPIC,-O3,-Wall", "-Xptxas", "-v",

@@ -19,6 +19,7 @@
 #include "objective.cuh"
 #include "augment.cuh"
 #include "cluster_rows.cuh"
+#include "lbfgs.cuh"
 
 namespace bre {
 void set_pdl(bool on);
@@ -1091,7 +1092,114 @@ struct bre_engine {
     return 0;
   }
 
+  // ---- L-BFGS trials (bre_engine_begin_lbfgs_trial) ---------------------------------------------------------------------------
+  // One iteration = one torch.optim.LBFGS step: the closure, a WHILE node over the inner iterations (direction kernels, x += t d,
+  // the re-evaluation under an IF node, the stop tests), then box projection, best-so-far and the history commit.
+  bool lbfgs = false;
+  LbfgsView lb;
+  cudaStream_t lb_streams[3] = {nullptr, nullptr, nullptr};   // capture streams: loop body, re-evaluation, its weight-gradient side stream
+  LbfgsSegs lbfgs_segs() const {
+    LbfgsSegs s;
+    s.x[0] = x; s.best[0] = best; s.n[0] = nx;
+    s.x[1] = joint ? ell : nullptr; s.best[1] = joint ? ell_best : nullptr; s.n[1] = joint ? n_ell : 0;
+    s.lo = lo; s.hi = hi; s.C = xC; s.HW = xH * xW; s.boxed = cfg.boxed;
+    return s;
+  }
+  // the closure handed to torch's L-BFGS (optimization_based_attack.py:146-189; joint: optimization_with_label_attack.py:145-189):
+  // one evaluation, each leaf's gradient folded and post-processed by the step kernel into the flat gradient lb.g, then the
+  // closure's bookkeeping (first = the step's first closure, which sets `loop`)
+  int lbfgs_closure(bool first, cudaGraphConditionalHandle loop) {
+    if (joint) {
+      BRE_LAUNCH(launch_row_softmax(ell, soft_q_buf, td(logits).N, classes(), stream));
+      soft_q = soft_q_buf;
+    }
+    BRE_TRY(evaluate());
+    if (joint) BRE_TRY(label_gradient_on_device());
+    StepArgs a = step_args();
+    a.grad_out = lb.g;
+    if (cfg.grad_clip >= 0.f) BRE_LAUNCH(launch_grad_norm(a, sc, dpartials, dcounter, stream));
+    BRE_LAUNCH(launch_pixel_step(a, sc, stream));
+    if (joint) {
+      StepArgs b = a;
+      b.x = ell; b.m = ell_m; b.v = ell_v; b.best = ell_best; b.grad = label_grad; b.grad_task = nullptr;
+      b.n = n_ell; b.C = 1; b.HW = 1; b.cfg.boxed = 0; b.grad_out = lb.g + nx;
+      if (cfg.grad_clip >= 0.f) BRE_LAUNCH(launch_grad_norm(b, sc, dpartials, dcounter, stream));
+      BRE_LAUNCH(launch_pixel_step(b, sc, stream));
+    }
+    BRE_LAUNCH(launch_lbfgs_closure_tail(lb, first, sc, value_task_reg(), loop, 1, stream));
+    return 0;
+  }
+  // appends a conditional node after what `st` has captured so far; *body = the graph it runs
+  int add_conditional(cudaStream_t st, cudaGraphConditionalHandle h, cudaGraphConditionalNodeType type, cudaGraph_t* body) {
+    cudaStreamCaptureStatus status;
+    cudaGraph_t graph = nullptr;
+    const cudaGraphNode_t* deps = nullptr;
+    size_t n_deps = 0;
+    BRE_CUDA_CHECK(cudaStreamGetCaptureInfo(st, &status, nullptr, &graph, &deps, &n_deps));
+    cudaGraphNodeParams p = {};
+    p.type = cudaGraphNodeTypeConditional;
+    p.conditional.handle = h; p.conditional.type = type; p.conditional.size = 1;
+    cudaGraphNode_t node;
+    BRE_CUDA_CHECK(cudaGraphAddNode(&node, graph, deps, n_deps, &p));
+    BRE_CUDA_CHECK(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
+    *body = p.conditional.phGraph_out[0];
+    return 0;
+  }
+  // captures what `fn` launches into `body`, with the engine's streams swapped for (st, st_side): a stream already joined to one
+  // capture cannot join another
+  template <typename F>
+  int capture_into(cudaGraph_t body, cudaStream_t st, cudaStream_t st_side, F fn) {
+    BRE_CUDA_CHECK(cudaStreamBeginCaptureToGraph(st, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+    cudaStream_t s0 = stream, s1 = side;
+    stream = st; side = st_side;
+    const int rc = fn();
+    stream = s0; side = s1;
+    cudaGraph_t g = nullptr;
+    const cudaError_t err = cudaStreamEndCapture(st, &g);
+    if (rc != 0) return rc;
+    if (err != cudaSuccess) { set_error(std::string("L-BFGS body capture failed: ") + cudaGetErrorString(err)); return BRE_ERR_CUDA; }
+    return 0;
+  }
+  int capture_lbfgs() {
+    cudaStreamCaptureStatus status;
+    cudaGraph_t graph = nullptr;
+    BRE_CUDA_CHECK(cudaStreamGetCaptureInfo(stream, &status, nullptr, &graph, nullptr, nullptr));
+    if (status != cudaStreamCaptureStatusActive) { set_error("L-BFGS iterations run from a captured graph only"); return BRE_ERR_STATE; }
+    cudaGraphConditionalHandle loop;
+    BRE_CUDA_CHECK(cudaGraphConditionalHandleCreate(&loop, graph, 0, 0));
+    BRE_TRY(lbfgs_closure(true, loop));
+    cudaGraph_t body = nullptr;
+    BRE_TRY(add_conditional(stream, loop, cudaGraphCondTypeWhile, &body));
+    BRE_TRY(capture_into(body, lb_streams[0], lb_streams[2], [&]() -> int {
+      cudaStreamCaptureStatus st;
+      cudaGraph_t bg = nullptr;
+      BRE_CUDA_CHECK(cudaStreamGetCaptureInfo(stream, &st, nullptr, &bg, nullptr, nullptr));
+      cudaGraphConditionalHandle eval;
+      BRE_CUDA_CHECK(cudaGraphConditionalHandleCreate(&eval, bg, 0, 0));
+      BRE_LAUNCH(launch_lbfgs_direction(lb, lr_table, n_lr, sc, eval, 1, stream));
+      BRE_LAUNCH(launch_lbfgs_step(lb, lbfgs_segs(), stream));
+      cudaGraph_t reeval = nullptr;
+      BRE_TRY(add_conditional(stream, eval, cudaGraphCondTypeIf, &reeval));
+      BRE_TRY(capture_into(reeval, lb_streams[1], lb_streams[2], [&]() -> int { return lbfgs_closure(false, 0); }));
+      BRE_LAUNCH(launch_lbfgs_tail(lb, loop, stream));
+      return 0;
+    }));
+    BRE_LAUNCH(launch_lbfgs_finish(lb, lbfgs_segs(), sc, stream));
+    BRE_LAUNCH(launch_commit(sc, history, lr_cap, value_task_reg(), stream));
+    return 0;
+  }
+  int iteration_lbfgs() {
+    // captured without programmatic dependent launch: edges into and out of conditional bodies are plain stream order
+    const bool pdl = use_pdl();
+    set_pdl(false);
+    const int rc = capture_lbfgs();
+    set_pdl(pdl);
+    consume_serialize_once();   // evaluate()'s request concerns programmatic launches only
+    return rc;
+  }
+
   int iteration() {
+    if (lbfgs) return iteration_lbfgs();
     if (joint) return iteration_joint();
     BRE_TRY(evaluate());
     StepArgs a = step_args();
@@ -1337,6 +1445,7 @@ void bre_engine_destroy(bre_engine* e) {
   for (cudaEvent_t ev : e->ev_fork) if (ev) cudaEventDestroy(ev);
   if (e->ev_join) cudaEventDestroy(e->ev_join);
   if (e->side) cudaStreamDestroy(e->side);
+  for (cudaStream_t st : e->lb_streams) if (st) cudaStreamDestroy(st);
   for (void* p : e->allocs) cudaFree(p);
   if (e->stream) cudaStreamDestroy(e->stream);
   delete e;
@@ -1619,7 +1728,7 @@ int bre_engine_begin_trial(bre_engine* e, const float* candidate, const float* l
   BRE_CUDA_CHECK(cudaMemsetAsync(e->m, 0, e->nx * sizeof(float), e->stream));
   BRE_CUDA_CHECK(cudaMemsetAsync(e->v, 0, e->nx * sizeof(float), e->stream));
   BRE_TRY(reset_trial_state(e));
-  if (e->joint) { e->joint = false; e->graph_ready = false; }
+  if (e->joint || e->lbfgs) { e->joint = false; e->lbfgs = false; e->graph_ready = false; }
   e->trial_begun = true;
   return BRE_OK;
 }
@@ -1646,6 +1755,53 @@ int bre_engine_begin_joint_trial(bre_engine* e, const float* candidate, const fl
   e->soft_q = e->soft_q_buf;
   e->joint = true;
   e->graph_ready = false;
+  return BRE_OK;
+}
+
+int bre_engine_begin_lbfgs_trial(bre_engine* e, const float* candidate, const float* label_logits, int64_t n_label, const float* lr_table,
+                                 int32_t n_lr, const bre_lbfgs_consts* k) {
+  if (!e || !k || k->history < 1 || k->history > BRE_LBFGS_MAX_HISTORY || k->max_iter < 1 || k->max_eval < 1) {
+    set_error("bre_engine_begin_lbfgs_trial: bad arguments");
+    return BRE_ERR_INVALID;
+  }
+  if (e->aug_on || e->seq_len > 0 || e->cfg.langevin_noise > 0.f || !e->use_graph) {
+    set_error("L-BFGS trials on the device: augmentations, Langevin noise, token programs and use_graph=0 are not supported");
+    return BRE_ERR_UNSUPPORTED;
+  }
+  BRE_TRY(label_logits ? bre_engine_begin_joint_trial(e, candidate, label_logits, n_label, lr_table, n_lr)
+                       : bre_engine_begin_trial(e, candidate, lr_table, n_lr));
+  BRE_CUDA_CHECK(cudaSetDevice(e->device));
+  LbfgsView& v = e->lb;
+  const long long n = e->nx + (label_logits ? e->n_ell : 0);
+  if (v.n != n || v.k.history != k->history) {   // (a previous allocation stays with the engine until it is destroyed)
+    v.n = n; v.R = k->history + 1; v.gram_blocks = lbfgs_gram_blocks(n);
+    BRE_TRY(e->alloc(&v.S, (long long)v.R * n)); BRE_TRY(e->alloc(&v.Y, (long long)v.R * n));
+    BRE_TRY(e->alloc(&v.g, n)); BRE_TRY(e->alloc(&v.prev_g, n)); BRE_TRY(e->alloc(&v.d, n));
+    BRE_TRY(e->alloc(&v.gram, 2LL * v.R * v.R + 3LL * v.R));
+    BRE_TRY(e->alloc(&v.partials, lbfgs_partials_size(n, k->history)));
+    BRE_TRY(e->alloc(&v.counter, 1));
+    BRE_TRY(e->alloc(&v.st, 1));
+  }
+  v.k = *k;
+  for (cudaStream_t& st : e->lb_streams)
+    if (!st) BRE_CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  bre_lbfgs_scalars h;
+  memset(&h, 0, sizeof(h));
+  h.h_diag = 1.0;
+  BRE_CUDA_CHECK(cudaMemcpyAsync(v.st, &h, sizeof(h), cudaMemcpyHostToDevice, e->stream));
+  BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));   // `h` is a stack object
+  e->lbfgs = true;
+  e->graph_ready = false;
+  return BRE_OK;
+}
+
+int bre_engine_lbfgs_counters(bre_engine* e, int32_t* out) {
+  if (!e || !out || !e->lb.st) { set_error("bre_engine_lbfgs_counters: no L-BFGS trial"); return BRE_ERR_STATE; }
+  BRE_CUDA_CHECK(cudaSetDevice(e->device));
+  bre_lbfgs_scalars h;
+  BRE_CUDA_CHECK(cudaMemcpyAsync(&h, e->lb.st, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
+  BRE_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  out[0] = h.total_iters; out[1] = h.func_evals; out[2] = h.count; out[3] = h.first;
   return BRE_OK;
 }
 

@@ -8,12 +8,6 @@ namespace bre {
 
 namespace {
 
-__device__ __forceinline__ double total_objective(const Scalars* sc, float task_reg) {
-  double phi = sc->match + sc->tv + sc->norm + sc->di + sc->feat;
-  if (task_reg != 0.f) phi += (double)task_reg * sc->task_loss;
-  return phi;
-}
-
 // --------------------------------------------------------------------------------------------------
 // matching reduction
 // --------------------------------------------------------------------------------------------------
@@ -457,6 +451,7 @@ __global__ void __launch_bounds__(256) pixel_step_kernel(StepArgs a, Scalars* sc
     float gr = raw_gradient(a, sc, i, lr) * clip_mul;
     if (cfg.signed_mode == BRE_SIGN_HARD) gr = gr > 0.f ? 1.f : (gr < 0.f ? -1.f : gr);  // keeps 0 and NaN like torch.sign
     else if (cfg.signed_mode == BRE_SIGN_SOFT) gr = tanhf(gr * soft) / soft;
+    if (a.grad_out != nullptr) { a.grad_out[i] = gr; continue; }
     float x = a.x[i];
     if (cfg.optimizer == BRE_OPT_SGD) {
       float dgr = gr;

@@ -6,6 +6,13 @@
 
 namespace bre {
 
+// the recorded objective of an evaluation: matching term + priors (+ task_regularization * task loss)
+__device__ __forceinline__ double total_objective(const Scalars* sc, float task_reg) {
+  double phi = sc->match + sc->tv + sc->norm + sc->di + sc->feat;
+  if (task_reg != 0.f) phi += (double)task_reg * sc->task_loss;
+  return phi;
+}
+
 constexpr int kChunk = 1024;  // arena granularity of the matching reduction (per-chunk TAG weight)
 
 // Sums over [0, n): <G,g>, |G|^2, |g|^2, sum (G-g)^2, sum w_chunk |G-g| (all masked where |g| <= mask_value when
@@ -43,6 +50,7 @@ struct StepArgs {   // closure tail + optimiser + projection + best-so-far (opti
   const float* lo; const float* hi;           // per-channel box
   long long n; int C; int HW;
   bre_attack_cfg cfg;
+  float* grad_out = nullptr;   // set: pixel_step writes the processed gradient here and does not step (the L-BFGS closure)
 };
 int launch_grad_norm(const StepArgs& a, Scalars* sc, double* partials, int* counter, cudaStream_t s);
 int launch_pixel_step(const StepArgs& a, Scalars* sc, cudaStream_t s);

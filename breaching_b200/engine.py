@@ -52,6 +52,25 @@ class StepScalars(ctypes.Structure):   # bre_step_scalars
                [("grad_norm_sq", ctypes.c_double), ("last_objective", ctypes.c_double)]
 
 
+class LbfgsConsts(ctypes.Structure):   # bre_lbfgs_consts
+    _fields_ = [(n, ctypes.c_int32) for n in ("max_iter", "max_eval", "history", "reserved")] + \
+               [(n, ctypes.c_double) for n in ("tol_grad", "tol_change", "curvature_min")]
+
+
+class LbfgsScalars(ctypes.Structure):   # bre_lbfgs_scalars
+    _fields_ = [(n, ctypes.c_double) for n in ("h_diag", "t", "loss", "prev_loss", "first_loss", "gtd", "d_max", "g_max", "g_abs_sum", "ys")] + \
+               [("first_terms", ctypes.c_double * 6)] + \
+               [(n, ctypes.c_int32) for n in ("first", "count", "total_iters", "inner", "evals", "func_evals", "brk", "converged", "pushed",
+                                              "reserved")]
+
+
+def lbfgs_consts():
+    """torch.optim.LBFGS's defaults as the C struct (their one definition is breaching_b200/attacks/lbfgs.py)."""
+    from .attacks import lbfgs
+
+    return LbfgsConsts(lbfgs.MAX_ITER, lbfgs.MAX_EVAL, lbfgs.HISTORY, 0, lbfgs.TOL_GRAD, lbfgs.TOL_CHANGE, lbfgs.CURVATURE_MIN)
+
+
 class AttackCfg(ctypes.Structure):
     _fields_ = [
         ("objective", ctypes.c_int32),
@@ -108,6 +127,7 @@ EXPORTS = [
     "bre_engine_set_augmentations_ex", "bre_engine_set_augmentation_stages_ex", "bre_augment_view_ex", "bre_engine_augmentation_flips",
     "bre_engine_set_trial_index", "bre_engine_debug_step_state", "bre_optimizer_step", "bre_langevin_noise",
     "bre_debug_last_gemm_plan", "bre_gemm_plan", "bre_debug_row_plan", "bre_row_op",
+    "bre_engine_begin_lbfgs_trial", "bre_engine_lbfgs_counters", "bre_lbfgs_direction",
 ]
 
 
@@ -189,6 +209,9 @@ def load_library(path=None):
     lib.bre_gemm_plan.argtypes = [i32] * 12 + [P(i32)]
     lib.bre_debug_row_plan.argtypes = [i32, P(i32), P(i32)]
     lib.bre_row_op.argtypes = [i32, vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, vp, vp, vp, vp]
+    lib.bre_engine_begin_lbfgs_trial.argtypes = [vp, vp, vp, i64, vp, i32, P(LbfgsConsts)]
+    lib.bre_engine_lbfgs_counters.argtypes = [vp, P(i32)]
+    lib.bre_lbfgs_direction.argtypes = [vp, vp, vp, vp, vp, vp, vp, i64, P(LbfgsConsts), vp]
     for name in EXPORTS:
         if name not in ("bre_last_error", "bre_version", "bre_engine_destroy"):
             getattr(lib, name).restype = ctypes.c_int
@@ -242,7 +265,8 @@ def make_cfg(cfg_attack, noise_seed=0):
     name = str(opt["optimizer"]).lower()
     if name not in OPTIMIZERS and name != "l-bfgs":
         raise ValueError(f"Invalid optimizer {opt['optimizer']} given.")
-    # L-BFGS trials are driven by attacks/lbfgs.py through objective_and_gradient(); the fused on-device step is unused then
+    # L-BFGS trials (Engine.begin_lbfgs_trial, or the host loop of attacks/lbfgs.py) use the step kernel only to post-process the
+    # gradient; its optimiser fields are unused then
     c.optimizer, c.beta1, c.beta2, c.adam_eps, c.weight_decay, c.momentum, c.nesterov = OPTIMIZERS["gd" if name == "l-bfgs" else name]
     signed = cfg_get(opt, "signed")
     c.signed_mode = {"hard": 1, "soft": 2}.get(signed, 0) if isinstance(signed, str) else 0
@@ -458,6 +482,29 @@ class Engine:
         self._label_shape = tuple(label_logits.shape)
         _check(self.lib, self.lib.bre_engine_begin_joint_trial(self.h, _ptr(cand), _ptr(ell), ell.numel(), _ptr(lr), lr.numel()),
                "bre_engine_begin_joint_trial")
+
+    def begin_lbfgs_trial(self, candidate, lr_table, label_logits=None, trial=0):
+        """L-BFGS trial on the device (torch.optim.LBFGS with the defaults of attacks/lbfgs.py): each ``run`` iteration is one
+        ``optimizer.step`` with its inner loop inside the captured graph.  ``label_logits`` [N, classes]: the label leaf of a joint
+        trial, optimised as one flat vector after the candidate."""
+        self.set_trial_index(trial)
+        cand = _f32c(candidate, self.device)
+        if cand.numel() != self.numel:
+            raise EngineError(f"candidate has {cand.numel()} elements, engine expects {self.numel}")
+        ell = None if label_logits is None else _f32c(label_logits, self.device)
+        lr = torch.as_tensor(lr_table, dtype=torch.float32).contiguous().cpu()
+        torch.cuda.synchronize(self.device)
+        if ell is not None:
+            self._label_shape = tuple(label_logits.shape)
+        consts = lbfgs_consts()
+        _check(self.lib, self.lib.bre_engine_begin_lbfgs_trial(self.h, _ptr(cand), _ptr(ell), 0 if ell is None else ell.numel(), _ptr(lr),
+                                                               lr.numel(), ctypes.byref(consts)), "bre_engine_begin_lbfgs_trial")
+
+    def lbfgs_counters(self):
+        """dict(inner_iterations, closures, pairs, first_slot) of the running L-BFGS trial (one host sync)."""
+        out = (ctypes.c_int32 * 4)()
+        _check(self.lib, self.lib.bre_engine_lbfgs_counters(self.h, out), "bre_engine_lbfgs_counters")
+        return dict(zip(("inner_iterations", "closures", "pairs", "first_slot"), list(out)))
 
     def joint_labels(self, best=True):
         out = torch.empty(self._label_shape, dtype=torch.float32, device=self.device)
@@ -753,6 +800,36 @@ def optimizer_step(x, m, v, best, grad, ccfg, lr_table, history, scalars, grad_t
                                     ctypes.byref(io), ctypes.c_void_p(stream))
     _check(lib, rc, "bre_optimizer_step")
     return {name: getattr(io, name) for name, _ in StepScalars._fields_}
+
+
+def lbfgs_direction(S, Y, gram, state, g, prev_g, d, consts=None):
+    """One inner iteration's direction through the engine's L-BFGS kernels on caller-owned CUDA tensors (updated in place; see
+    ``bre_lbfgs_direction``): S, Y [history + 1, n] fp32 rings, ``gram`` fp64 [2 (h+1)^2 + 3 (h+1)], ``state`` a CUDA uint8 tensor
+    holding one ``LbfgsScalars``, g / prev_g / d [n] fp32.  Returns the state after the call as an ``LbfgsScalars``."""
+    lib = load_library()
+    consts = consts or lbfgs_consts()
+    R = consts.history + 1
+    n = g.numel()
+    for t in (S, Y, g, prev_g, d):
+        assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
+    assert S.numel() == R * n and Y.numel() == R * n and prev_g.numel() == n and d.numel() == n
+    assert gram.is_cuda and gram.dtype == torch.float64 and gram.numel() == 2 * R * R + 3 * R
+    assert state.is_cuda and state.dtype == torch.uint8 and state.numel() == ctypes.sizeof(LbfgsScalars)
+    stream = torch.cuda.current_stream(g.device).cuda_stream
+    with torch.cuda.device(g.device):
+        rc = lib.bre_lbfgs_direction(_ptr(S), _ptr(Y), _ptr(gram), _ptr(state), _ptr(g), _ptr(prev_g), _ptr(d), n, ctypes.byref(consts),
+                                     ctypes.c_void_p(stream))
+    _check(lib, rc, "bre_lbfgs_direction")
+    return LbfgsScalars.from_buffer_copy(bytes(state.cpu().numpy().tobytes()))
+
+
+def lbfgs_state(scalars=None, device="cuda"):
+    """A device ``LbfgsScalars`` block (CUDA uint8 tensor) holding ``scalars`` (default: a fresh optimiser, h_diag = 1)."""
+    if scalars is None:
+        scalars = LbfgsScalars()
+        scalars.h_diag = 1.0
+    raw = bytes(bytearray(scalars))
+    return torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(device)
 
 
 def langevin_noise(seed, trial, it, n, first=0, device="cuda"):

@@ -432,6 +432,40 @@ enum { BRE_ROW_SOFTMAX = 0, BRE_ROW_SOFTMAX_CHAIN = 1, BRE_ROW_TOKEN_CE_FWD = 2,
 int bre_row_op(int32_t op, const float* in0, const float* in1, const float* in2, const int64_t* labels, int32_t rows, int32_t C, int32_t Vs,
                int32_t T, float coef, int32_t round_out, float* out0, float* out1, float* out2, void* stream);
 
+/* ---- L-BFGS on the device (torch.optim.LBFGS without line search; breaching/attacks/auxiliaries/common.py:18) ------------- */
+/* torch's constants, passed in by the caller (breaching_b200/attacks/lbfgs.py holds them): max_iter inner iterations and max_eval
+ * closure evaluations per optimizer.step, `history` curvature pairs (<= BRE_LBFGS_MAX_HISTORY), tolerance_grad, tolerance_change and
+ * the curvature threshold a pair must pass (y.s > curvature_min). */
+enum { BRE_LBFGS_MAX_HISTORY = 128 };
+typedef struct bre_lbfgs_consts {
+  int32_t max_iter, max_eval, history, reserved;
+  double tol_grad, tol_change, curvature_min;
+} bre_lbfgs_consts;
+/* Scalar state of one optimiser (device memory).  The ring has history + 1 slots: live pairs are slots (first + k) % (history + 1),
+ * k < count, oldest first; a candidate pair is written to the one spare slot and becomes live only if it passes the curvature test. */
+typedef struct bre_lbfgs_scalars {
+  double h_diag, t, loss, prev_loss, first_loss, gtd, d_max, g_max, g_abs_sum, ys;
+  double first_terms[6];   /* objective terms of the first closure of the step (match, task_loss, tv, norm, di, feat) */
+  int32_t first, count, total_iters, inner, evals, func_evals, brk, converged, pushed, reserved;
+} bre_lbfgs_scalars;
+
+/* L-BFGS trial on the device: one bre_engine_run iteration = one optimizer.step (closure, then a conditional-graph loop of up to
+ * max_iter inner iterations, the re-evaluation of each under a conditional node) followed by the box projection, best-so-far (the
+ * loss before the step against the candidate after it) and the history commit (optimization_based_attack.py:90-143 with
+ * `optimizer.step(closure)`).  label_logits (device or host, NULL unless joint): [N, classes] label leaf of the joint attacker
+ * (optimization_with_label_attack.py), optimised as one flat vector after the candidate.  Refused (BRE_ERR_UNSUPPORTED) with
+ * augmentations, Langevin noise, token programs or with the option use_graph off. */
+int bre_engine_begin_lbfgs_trial(bre_engine* e, const float* candidate, const float* label_logits, int64_t n_label, const float* lr_table,
+                                 int32_t n_lr, const bre_lbfgs_consts* consts);
+/* out[4] = inner iterations and closure evaluations over the trial, live pairs, oldest slot (synchronises the engine stream). */
+int bre_engine_lbfgs_counters(bre_engine* e, int32_t* out);
+/* One inner iteration's direction on caller-owned device buffers (parity tests): when state->total_iters > 0 the candidate pair
+ * (y = g - prev_g, s = t * d) is written to the spare slot of S / Y [history + 1, n] and pushed if it passes the curvature test;
+ * then d = -H g (torch's two-loop recursion, evaluated over the Gram matrices), prev_g = g, total_iters += 1.  gram (device doubles):
+ * [SY (h+1)^2 | YY (h+1)^2 | rho h+1 | coefficients 2 (h+1)] with h = consts->history, SY[i][j] = s_i.y_j; state: device. */
+int bre_lbfgs_direction(float* S, float* Y, double* gram, bre_lbfgs_scalars* state, const float* g, float* prev_g, float* d, int64_t n,
+                        const bre_lbfgs_consts* consts, void* stream);
+
 const char* bre_last_error(void);
 const char* bre_version(void);
 
